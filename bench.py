@@ -8,7 +8,12 @@ N>1: BASELINE config 4 -- one process per GPU (torchrun), 16 keyframes per GPU (
 the whole-model objects (`full_model*`) include the NCCL all-gather of the per-rank `result` maps in their timed region.
 `--config hires` is BASELINE config 5: 512x1024, 64 planes, 6 source frames, batch 4 per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config default|hires]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config default|hires] [--dump-outputs DIR]
+
+`--dump-outputs DIR` writes what the timed path computed in its last timed step: DIR/cost_volume.npy and
+DIR/single_frame_cvs.npy (float32), each a fixed sample of DUMP_SAMPLES elements of the flattened output at the sorted indices
+drawn by torch.Generator().manual_seed(0) (the whole output when it is smaller).  The inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 
 `--impl reference` times the reference's CPU implementation of the path.  The reference is pure Python/PyTorch and
 cannot travel to the GPU box, so this arm runs the oracle port (oracle/cost_volume_oracle.py: the same torch CPU
@@ -33,6 +38,7 @@ B_PER_GPU_SHARDED = 16                     # BASELINE config 4: batch 128 sharde
 INV_LO, INV_HI = 0.0025, 0.33
 METRIC = "keyframes_per_s_256x512_D32_F4"
 ALG_BYTES_PER_KEYFRAME = 4 * H * W * (1 + F) * (3 + D)   # SURVEY.md §8d: every input read once, every output written once
+DUMP_SAMPLES = 4 * 1024 * 1024             # elements per dumped array (16 MiB of float32)
 
 
 def set_config(name):
@@ -41,24 +47,6 @@ def set_config(name):
         H, W, D, F, B_PER_GPU = 512, 1024, 64, 6, 4
         METRIC = "keyframes_per_s_512x1024_D64_F6"
     ALG_BYTES_PER_KEYFRAME = 4 * H * W * (1 + F) * (3 + D)
-
-
-def k1_traffic(config, batch):
-    """DRAM bytes per launch of the cost-volume kernel from the committed `ncu --set full` capture -- valid only for the
-    kernel source it was taken from: the file stores the SHA-256 of csrc/cost_volume.cu and of the launch shape; any
-    mismatch (a changed kernel, another batch) reports null instead of a stale number."""
-    import hashlib
-    p = ROOT / "profiles" / "r02_k1_traffic.json"
-    if not p.exists():
-        return None, "no capture committed"
-    rec = json.loads(p.read_text())
-    sha = hashlib.sha256((ROOT / "monorec_b200" / "csrc" / "cost_volume.cu").read_bytes()).hexdigest()
-    ent = rec.get(f"{config}_b{batch}")
-    if ent is None:
-        return None, f"no capture for config {config} at batch {batch}"
-    if ent.get("cost_volume_cu_sha256") != sha:
-        return None, "capture predates the current cost_volume.cu"
-    return float(ent["traffic_bytes_per_launch"]), "ncu --set full: dram__bytes_read.sum + dram__bytes_write.sum, " + ent.get("capture", "")
 
 
 def pin_to_gpu_numa_node(index):
@@ -82,8 +70,21 @@ def pin_to_gpu_numa_node(index):
 def hbm_peak():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
-        return float(json.loads(p.read_text())["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+        return float(json.loads(p.read_text())["hbm_gbs"]), "measured (burst copy)"
+    return 3350.0, "H100 SXM data sheet"
+
+
+def dump_outputs(dirname, arrays):
+    """Writes a fixed, seeded sample of each device tensor as float32 .npy (see the module docstring)."""
+    import numpy as np
+    out = Path(dirname)
+    out.mkdir(parents=True, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLES:
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLES,), generator=torch.Generator().manual_seed(0)).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(out / f"{name}.npy", flat.float().cpu().numpy())
 
 
 class ClockSampler:
@@ -226,6 +227,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-full-model", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write samples of the last timed step's cost volume and single-frame volumes as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -250,7 +253,7 @@ def main():
     # N = 1: the configuration the metric is quoted on (batch 8); N > 1: BASELINE config 4's shard size, 16 keyframes per GPU
     # (global batch 16 N = 128 at N = 8; weak scaling); hires: 4 per GPU at every N
     B = B_PER_GPU if (world == 1 or args.config == "hires") else B_PER_GPU_SHARDED
-    # rotating input sets whose images together exceed the 126 MB L2, so no step finds its inputs cached from the previous one
+    # rotating input sets whose images together exceed the 50 MB L2, so no step finds its inputs cached from the previous one
     set_bytes = B * (1 + F) * 3 * H * W * 4
     NSETS = max(2, min(4, -(-256 * 1024 * 1024 // set_bytes)))
     sets = []
@@ -297,6 +300,8 @@ def main():
         barrier()
     ms = ev0.elapsed_time(ev1)
     launches = _lib.launch_count(reset=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"cost_volume": cv, "single_frame_cvs": sfcv})
     t = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -308,7 +313,7 @@ def main():
     if rank == 0:
         peak, peak_src = hbm_peak()
         achieved = ALG_BYTES_PER_KEYFRAME * B / (kernel_ms * 1e-3) / 1e9
-        traffic, traffic_note = k1_traffic(args.config, B)
+        traffic, traffic_note = None, "not measured"
         cfg_name = ("BASELINE config 5 (hi-res)" if args.config == "hires" else
                     ("BASELINE config 2: fused warp+SSIM kernel only" if world == 1 else
                      f"BASELINE config 4 shard size: {B} keyframes per GPU, global batch {B * world} over {world} GPUs"))
@@ -318,12 +323,12 @@ def main():
                 "config": {"workload": f"cost_volume_{H}x{W}_D{D}_F{F} ({cfg_name})",
                            "batch_per_gpu": B, "global_batch": B * world, "src_frames": F, "depth_planes": D,
                            "height": H, "width": W, "parallelism": f"dp{world} (independent keyframes, no collective)",
-                           "l2": f"inputs rotate over {NSETS} sets ({NSETS * set_bytes >> 20} MiB) > 126 MB L2; "
+                           "l2": f"inputs rotate over {NSETS} sets ({NSETS * set_bytes >> 20} MiB) > 50 MB L2; "
                                  f"{(1 + F) * B * D * H * W * 4 >> 20} MiB of outputs per step",
                            "host_numa_cpus": numa_cpus},
                 "gpu_launches": launches,
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                             "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_note, "peak_source": f"{peak_src} (burst copy)",
+                             "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_note, "peak_source": peak_src,
                              "kernel": "cost_volume_kernel (the events bracket mr_cost_volume_fwd: one launch)",
                              "kernel_ms": kernel_ms,
                              "algorithmic_bytes_per_launch": ALG_BYTES_PER_KEYFRAME * B},
@@ -406,9 +411,10 @@ def main():
                 line[key] = {"value": world * B / (fms * 1e-3), "unit": "keyframes/s", "ms_per_forward": fms,
                              "batch_per_gpu": B, "global_batch": B * world, "conv_arithmetic": mode,
                              "gathered_result_shape": list(res.shape),
-                             "roofline": {"bound": "tensor", "achieved": tach, "peak": tpeak if tpeak else 1400.0,
-                                          "unit": "TFLOP/s", "frac": tach / (tpeak if tpeak else 1400.0),
-                                          "peak_source": "measured (sustained bf16 GEMM)" if tpeak else "fallback",
+                             "roofline": {"bound": "tensor", "achieved": tach, "peak": tpeak if tpeak else 989.0,
+                                          "unit": "TFLOP/s", "frac": tach / (tpeak if tpeak else 989.0),
+                                          "peak_source": "measured (sustained bf16 GEMM)" if tpeak else
+                                                         "H100 SXM data sheet (dense bf16)",
                                           "flops_per_forward": conv_flops,
                                           "note": "MaskModule + DepthModule multiply-adds (x2) over the whole forward time "
                                                   "(cost volume, ResNet-18 trunk and the all-gather included in the time)"},

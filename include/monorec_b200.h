@@ -1,5 +1,5 @@
 /*
- * monorec_b200.h -- C ABI of libmonorec_b200.so (sm_100a kernels for MonoRec's hot path).
+ * monorec_b200.h -- C ABI of libmonorec_b200.so (sm_90a kernels for MonoRec's hot path).
  *
  * The reference (Brummi/MonoRec) is pure Python/PyTorch and has no FFI of its own; these entry points are
  * what a binding for the hot path replaces (SURVEY.md §8b).  Every entry point cites the reference code it
@@ -152,13 +152,13 @@ typedef struct mr_conv_desc {
 } mr_conv_desc;
 
 int mr_conv2d_nhwc(const mr_conv_desc* desc, void* stream);
-/* Same descriptor on the tensor cores (tcgen05, kind::tf32: TF32 products, fp32 accumulation in TMEM, fp32 storage).
+/* Same descriptor on the tensor cores (wgmma, tf32: TF32 products, fp32 accumulation in registers, fp32 storage).
  * `weight` is packed as [kh*kw][n_pad][k_pad] (K contiguous): Cout padded to n_pad (multiple of 16, <= 256), every source
  * padded to a multiple of 32 channels (k_pad = sum).  Needs src_c[i] % 4 == 0 and upsample2 == 0 (nearest-x2 upsampling is
  * expressed as sub-pixel convolutions on this path).  round_out: round stored activations to TF32 (nearest).
  * With src_dtype = MR_DT_F16 the sources and the packed weights are half, a K chunk is 64 channels (every source padded to
  * a multiple of 64) or, if the caller packed every source to a multiple of 32 instead and that gives a different k_pad,
- * 32 channels (64-byte swizzle rows); the MMA is kind::f16; dst_dtype selects half or float output.
+ * 32 channels (64-byte swizzle rows); the MMA is f16; dst_dtype selects half or float output.
  * Stride-1 layers whose packed weights fit in shared memory twice per SM run on the "halo" variant of the kernel (same
  * results).  Tuning switches (environment, read once): MONOREC_B200_TC_HALO=0|1|2, MONOREC_B200_TC_HALO_F16=0|1,
  * MONOREC_B200_TC_CTAS=n. */

@@ -1,4 +1,4 @@
-"""monorec_b200 -- B200-native (sm_100a) implementation of MonoRec's data-parallel hot path.
+"""monorec_b200 -- H100-native (sm_90a) implementation of MonoRec's data-parallel hot path.
 
 Only what the path needs lives here: `csrc/` (CUDA kernels + the C-ABI shared library) and the
 Python host-side mirror of the reference interface (`CostVolumeModule`, `MaskModule`,

@@ -80,7 +80,7 @@ def load(build_if_missing=True):
         from . import build as _build
         _build.build()
     if not LIB_PATH.exists():
-        raise MonorecLibraryError(f"{LIB_PATH} not found: run `python -m monorec_b200.build` (needs nvcc, sm_100a)")
+        raise MonorecLibraryError(f"{LIB_PATH} not found: run `python -m monorec_b200.build` (needs nvcc, sm_90a)")
     lib = ctypes.CDLL(str(LIB_PATH))
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol

@@ -1,4 +1,4 @@
-"""Builds libmonorec_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so must travel with the repo snapshot).
+"""Builds libmonorec_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache: the .so sits next to the package).
 
     python -m monorec_b200.build [--force] [--verbose]
 """
@@ -13,8 +13,7 @@ CSRC = PKG / "csrc"
 LIB = PKG / "libmonorec_b200.so"
 STAMP = PKG / ".libmonorec_b200.stamp"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--use_fast_math_off_placeholder"]
-FLAGS = [f for f in FLAGS if not f.endswith("_placeholder")]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
 for _knob in ("MR_CV_THREADS", "MR_CV_MINBLOCKS", "MR_CV_TILE_ROWS", "MR_CV_SKIP"):   # tuning knobs of the cost-volume kernel
     if os.environ.get(_knob):
         FLAGS.append(f"-D{_knob}=" + os.environ[_knob])

@@ -19,8 +19,8 @@ ACT_NONE, ACT_LEAKY, ACT_SIGMOID, ACT_ABSTANH = 0, 1, 2, 3
 LEAKY_SLOPE = 0.1  # model/layers.py:290, 318, 381
 KC = 32            # channels per K chunk of the tensor-core kernel (csrc/conv_tc.cu)
 
-# Arithmetic of the dense-contraction layers: "tf32" = tcgen05 tensor cores (kind::tf32, fp32 accumulate, fp32 storage),
-# "f16" = tcgen05 kind::f16 with half NHWC activations and weights (fp32 accumulate; BASELINE config 3),
+# Arithmetic of the dense-contraction layers: "tf32" = wgmma tensor cores (tf32, fp32 accumulate, fp32 storage),
+# "f16" = wgmma f16 with half NHWC activations and weights (fp32 accumulate; BASELINE config 3),
 # "fp32" = CUDA-core FMA kernel (bit-level parity path).  1-channel heads always use the CUDA-core dot-product kernel.
 MODE = os.environ.get("MONOREC_B200_CONV", "tf32").lower()
 # half sources of <= 32 channels: 32-channel K chunks (SWIZZLE_64B rows), in the tap-refetch kernel and inside the halo box alike

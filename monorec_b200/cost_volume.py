@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's CostVolumeModule (model/monorec/monorec_model.py:132-284).
 
-Same constructor arguments, same data_dict keys in and out; the arithmetic runs in the fused sm_100a kernel of
+Same constructor arguments, same data_dict keys in and out; the arithmetic runs in the fused sm_90a kernel of
 libmonorec_b200.so (csrc/cost_volume.cu) through the C ABI.  No torch fallback.
 """
 import os

@@ -1,4 +1,4 @@
-// Convolution engine, CUDA-core fp32 path (sm_100a).  See include/monorec_b200.h (mr_conv_desc) for what one call fuses:
+// Convolution engine, CUDA-core fp32 path (sm_90a).  See include/monorec_b200.h (mr_conv_desc) for what one call fuses:
 // TF-"SAME" padding, channel concatenation of up to three sources, nearest x2 upsampling on read, bias, activation and
 // strided (sub-pixel) output placement.  NHWC activations, weights [kh][kw][Cin][Cout].
 //

@@ -1,41 +1,43 @@
-// Convolution engine, tensor-core path: implicit GEMM on tcgen05 (5th-gen tensor cores) for sm_100a.
+// Convolution engine, tensor-core path: implicit GEMM on Hopper warpgroup MMA (wgmma) for sm_90a.
 //
-//   D[128 pixels x Cout] (fp32, TMEM)  +=  A[128 pixels x 32 ch] (smem, TMA)  x  B[Cout x 32 ch]^T (smem, TMA)     kind::tf32
+//   D[128 pixels x Cout] (fp32, registers)  +=  A[128 pixels x 32 ch] (smem, TMA)  x  B[Cout x 32 ch]^T (smem, TMA)     tf32
 //
-// One CTA owns an 8x16 tile of output pixels (UMMA M = 128) and all Cout (UMMA N = Cout padded to 16, <= 256).  The K
-// loop runs over (filter tap, concatenated source, 32-channel chunk):
+// One CTA owns 128 output pixels and all Cout (MMA N = Cout padded to 16, <= 256).  The K loop runs over (filter tap,
+// concatenated source, 32-channel chunk):
 //   * the A operand of a tap is the NHWC input tile shifted by the tap offset, fetched by ONE 4-D TMA box
 //     {32 ch, 16 px, 8 px, 1 img} (traversal stride = conv stride).  Out-of-bounds elements are zero-filled by the TMA unit,
 //     which IS the reference's PadSameConv2d (model/layers.py:220-252); channel concatenation (torch.cat,
 //     monorec_model.py:372-380, :541-545) is just one tensor map per source;
 //   * the B operand is the matching [Cout x 32] slice of the packed weights (2-D TMA);
-//   * both land in 128-byte-swizzled K-major shared-memory tiles that tcgen05.mma consumes through smem descriptors.
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer, warps 2..5 = epilogue (tcgen05.ld ->
-// bias -> activation -> NHWC store, optional sub-pixel placement).  The producer and issuer loops run on CONVERGED warps with
-// elect-predicated instructions (see umma_elect): their operands stay in uniform registers, ~7 SASS instructions per MMA.
-// Pipelines: smem full/empty mbarrier ring between TMA and MMA; tmem full/empty mbarriers between MMA and epilogue (the
-// accumulator is double-buffered in TMEM, the kernels are persistent over output tiles).
+//   * both land in 128-byte-swizzled K-major shared-memory tiles that wgmma.mma_async reads through smem descriptors.
+// Warp roles (288 threads): warps 0..7 = two consumer warpgroups, warpgroup g owns accumulator rows 64 g .. 64 g + 63 (one
+// m64nNk8 / m64nNk16 chain each, accumulator in registers, then bias -> activation -> NHWC store, optional sub-pixel
+// placement); warp 8 = TMA producer.  The producer loop runs on a CONVERGED warp with elect-predicated instructions (see
+// tma_load_4d_elect): its operands stay in uniform registers.
+// Pipeline: smem full/empty mbarrier ring between TMA and the consumers; one wgmma group stays in flight, and a stage is
+// released (one arrival per warpgroup) once the group that read it has retired.  The kernels are persistent over output
+// tiles, so the producer fills the next tile's stages while the consumers run an epilogue.
+// MMA N is a template parameter (Cout padded to 16); it is issued as m64n256 / n128 / n64 / n32 / n16 pieces.
 // Two kernels, chosen by the host code at the bottom of this file:
 //   conv_tc_halo_kernel  stride-1 layers: ONE input box per (tile, K chunk) with its halo, every filter tap a shifted
 //                        shared-memory descriptor into it; weights resident in shared memory, or -- when they do not fit
 //                        next to two input stages -- streamed slice by slice through a second ring; 64- or 128-byte rows;
 //   conv_tc_kernel       everything else (strided layers, the sub-pixel phases of Refine / Upconv -- up to four phases share
 //                        one launch): one input box and one weight slice per (tap, K chunk).
-// The epilogue is staged through shared memory (8 pixels x 64 contiguous bytes per store instruction); one-channel heads take
-// a single accumulator column.  K steps that hold only the zero padding behind a source's channels are skipped.
+// K steps that hold only the zero padding behind a source's channels are skipped.
 //
 // Reference being replaced: nn.Conv2d / nn.ConvTranspose2d + bias + LeakyReLU of model/layers.py:289-400 as used by
 // MaskModule / DepthModule (model/monorec/monorec_model.py:287-385, :476-557).
 #include "mr_common.cuh"
 #include <cuda.h>
 #include <cstdint>
-#include <type_traits>
 #include <cstdlib>
 #include <cuda_fp16.h>
 
 namespace {
 
-constexpr int kTcThreads = 192;
+constexpr int kTcThreads = 288;
+constexpr int kProducerWarp = 8;
 constexpr int kKC = 32;                 // fp32 channels per K chunk = one 128-byte swizzle row
 constexpr int kTileH = 8, kTileW = 16;  // 128 output pixels per CTA
 
@@ -46,16 +48,14 @@ struct TcArgs {
                                         // zero padding behind a source's channels is neither multiplied nor read from shared memory
     int kh, kw, sy, sx, pad_t, pad_l;
     int Ho, Wo, Cout, n_pad, tiles_x, tiles_per_img, total_tiles, stages;
-    uint32_t tmem_cols;
     const float* bias;
     float* dst;
     int dst_H, dst_W, dst_c, dst_coff, oy_step, ox_step, oy_off, ox_off;
     int act;
     float act_a, act_b;
     int round_out;                 // 1: round stored activations to TF32 (nearest) so the next layer's truncation is exact
-    int kc;                        // channels per K chunk: 32 (fp32 sources, kind::tf32) or 64 (half sources, kind::f16)
-    int f16, out_f16;              // half sources+weights / half destination
-    uint32_t idesc;                // UMMA instruction descriptor
+    int kc;                        // channels per K chunk: 32 (fp32 sources, tf32 MMA) or 64 (half sources, f16 MMA)
+    int out_f16;                   // half destination
     int row_bytes;                 // bytes of one K chunk row in shared memory = swizzle span: 128, or 64 (half sources, 32-channel chunks)
     // tap-refetch kernel: up to 4 "phases" (the sub-pixel convolutions of one Refine / Upconv layer) share one launch; tile
     // index = spatial tile * n_phase + phase, so the phases of a spatial tile run side by side and its input boxes are L2 hits
@@ -85,56 +85,15 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "}\n" ::"r"(bar), "r"(parity)
         : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-// K-major swizzled shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (1: unused for swizzled K-major) |
-//   [32,46) stride byte offset >> 4 (distance between 8-row groups) | [46,48) version = 1 | [49,52) base offset |
-//   [61,64) layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B.  Everything but the start address is layer-constant (desc_hi()).
-// ---- single-lane instructions issued from CONVERGED warp code ---------------------------------------------------------------
-// The producer and MMA warps used to run their loops under `if (lane == 0)`.  Every operand of UTMALDG / UTCHMMA / UTCBAR lives
-// in a uniform register, and inside a divergent region ptxas cannot keep values there: the SASS of the tap loop had ~20
-// instructions (R2UR.BROADCAST, ELECT, a waterfall branch) around every MMA, and that single-thread instruction stream -- not
-// the tensor pipe, shared memory or HBM -- paced the kernels.  Here all 32 lanes execute the loops (uniform arithmetic only) and
-// the instruction itself is predicated on elect.sync.
-template <bool F16>
-__device__ __forceinline__ void umma_elect(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi, uint32_t idesc,
-                                           uint32_t accumulate) {
-    if (F16)
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p, pe;\n\t"
-            ".reg .b64 da, db;\n\t"
-            "mov.b64 da, {%1, %2};\n\t"
-            "mov.b64 db, {%3, %4};\n\t"
-            "setp.ne.b32 p, %6, 0;\n\t"
-            "elect.sync _|pe, 0xffffffff;\n\t"
-            "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t"
-            "}\n" ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p, pe;\n\t"
-            ".reg .b64 da, db;\n\t"
-            "mov.b64 da, {%1, %2};\n\t"
-            "mov.b64 db, {%3, %4};\n\t"
-            "setp.ne.b32 p, %6, 0;\n\t"
-            "elect.sync _|pe, 0xffffffff;\n\t"
-            "@pe tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t"
-            "}\n" ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-            : "memory");
-}
-__device__ __forceinline__ void umma_commit_elect(uint32_t bar) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred pe;\n\t"
-        "elect.sync _|pe, 0xffffffff;\n\t"
-        "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t"
-        "}\n" ::"r"(bar)
-        : "memory");
-}
+// ---- single-lane instructions issued from a CONVERGED warp --------------------------------------------------------------
+// All 32 lanes of the producer warp execute its loops (uniform arithmetic only) and the instruction itself is predicated on
+// elect.sync: inside an `if (lane == 0)` region ptxas cannot keep the operands in uniform registers.
 __device__ __forceinline__ void mbar_expect_tx_elect(uint32_t bar, uint32_t bytes) {
     asm volatile(
         "{\n\t"
@@ -162,21 +121,201 @@ __device__ __forceinline__ void tma_load_2d_elect(uint32_t dst, const CUtensorMa
         "}\n" ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
-// shared-memory descriptor halves: low word = start address >> 4 | LBO (1, unused) << 16; high word = SBO >> 4 | version 1 << 14 |
-// layout << 29 (the K-major swizzled descriptor's bit layout is in the comment further up)
+
+// K-major swizzled shared-memory matrix descriptor of wgmma:
+//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (1: unused for swizzled K-major) |
+//   [32,46) stride byte offset >> 4 (distance between 8-row groups) | [49,52) base offset (0) | [62,64) layout: 1 = SWIZZLE_128B,
+//   2 = SWIZZLE_64B.  The swizzle is a function of the absolute shared-memory address (as TMA writes it), so a start address
+//   shifted by whole rows -- a filter tap inside the halo box -- needs no other field changed.  Everything but the start address
+//   is layer-constant (desc_hi()); advancing the low word by n moves the start by 16 n bytes.
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
 __device__ __forceinline__ uint32_t desc_hi(uint32_t sbo_bytes, uint32_t row_bytes) {
-    return (sbo_bytes >> 4) | (1u << 14) | ((row_bytes == 128 ? 2u : 4u) << 29);
+    return (sbo_bytes >> 4) | ((row_bytes == 128 ? 1u : 2u) << 30);
+}
+__device__ __forceinline__ uint64_t desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// m64nNk8 (tf32) / m64nNk16 (f16) with fp32 accumulators d[N / 2]; acc = 0 overwrites d (first K step of a tile)
+template <int N, bool F16>
+__device__ __forceinline__ void wgmma(float* d, uint64_t da, uint64_t db, uint32_t acc);
+
+template <> __device__ __forceinline__ void wgmma<16, false>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<16, true>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<32, false>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<32, true>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<64, false>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<64, true>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<128, false>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<128, true>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<256, false>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<256, true>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+        "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(da), "l"(db), "r"(acc));
 }
 
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
+// The whole accumulator row block [64 x N] as descending power-of-two pieces (N = 48 -> n32 + n16): piece p reads the weight
+// rows [n0, n0 + p) (descriptor start advanced by n0 rows of b_row16 * 16 bytes) into d[n0 / 2 ..).
+template <int N, bool F16>
+__device__ __forceinline__ void mma_tile(float* d, uint64_t da, uint64_t db, uint32_t b_row16, uint32_t acc) {
+    constexpr int P = N >= 256 ? 256 : N >= 128 ? 128 : N >= 64 ? 64 : N >= 32 ? 32 : 16;
+    wgmma<P, F16>(d, da, db, acc);
+    if constexpr (N > P) mma_tile<N - P, F16>(d + P / 2, da, db + (uint64_t)(P * b_row16), b_row16, acc);
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ float act_fn(float v, int act, float a, float b) {
     switch (act) {
@@ -187,198 +326,75 @@ __device__ __forceinline__ float act_fn(float v, int act, float a, float b) {
     }
 }
 
-// Epilogue of one accumulator row (= one output pixel): 32 columns per step (two x16 TMEM loads, one wait), bias from shared
-// memory, activation, optional TF32 rounding, 16-byte NHWC stores.
-__device__ __forceinline__ void epilogue_row(uint32_t trow, const TcArgs& a, const float* bias_s, float* op, bool live,
-                                             bool vec_ok) {
-    __half* oph = reinterpret_cast<__half*>(op);   // when a.out_f16 the caller computed `op` in half elements
-    for (int n0 = 0; n0 < a.n_pad; n0 += 32) {
-        uint32_t r0[16], r1[16];
-        const bool second = n0 + 16 < a.n_pad;
-        tmem_ld16_nowait(trow + (uint32_t)n0, r0);
-        if (second) tmem_ld16_nowait(trow + (uint32_t)(n0 + 16), r1);
-        tmem_ld_wait();
-        if (!live) continue;
+// Epilogue of one warpgroup's 64 accumulator rows.  wgmma fragment: warp w of the warpgroup holds rows 16 w + lane / 4 (+ 8),
+// d[4 j + 2 i + c] is row 16 w + lane / 4 + 8 i, column 8 j + 2 (lane % 4) + c.  Row p of the tile is pixel (p / TW, p % TW).
+// Bias from shared memory, activation, optional TF32 rounding; two adjacent channels per store (4 lanes = 8 channels).
+template <int N, int TW, int TH>
+__device__ __forceinline__ void epilogue_wg(const float* d, const TcArgs& a, const float* bias_s, int p0, int lane, int b, int tile_y,
+                                            int tile_x, int oy_off, int ox_off) {
+    const bool pair_ok = ((a.dst_c | a.dst_coff) & 1) == 0 && (reinterpret_cast<uintptr_t>(a.dst) & (a.out_f16 ? 3 : 7)) == 0;
+    const float slope = a.act == MR_ACT_LEAKY ? a.act_a : 1.0f;
+    const bool generic_act = a.act != MR_ACT_NONE && a.act != MR_ACT_LEAKY;
+    const int c0 = 2 * (lane & 3);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            if (h == 1 && !second) break;
-            const int nb = n0 + 16 * h;
-            float v[16];
+    for (int i = 0; i < 2; ++i) {
+        const int p = p0 + (lane >> 2) + 8 * i;
+        const int oy = tile_y * TH + p / TW, ox = tile_x * TW + p % TW;
+        if (oy >= a.Ho || ox >= a.Wo) continue;
+        const size_t oidx = (((size_t)b * a.dst_H + (oy * a.oy_step + oy_off)) * a.dst_W + (ox * a.ox_step + ox_off)) * a.dst_c +
+                            a.dst_coff;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                float x = __uint_as_float(h ? r1[j] : r0[j]) + bias_s[nb + j];
-                if (a.act == MR_ACT_LEAKY) x = fmaxf(x, a.act_a * x);          // slope in (0, 1)
-                else if (a.act != MR_ACT_NONE) x = act_fn(x, a.act, a.act_a, a.act_b);
+        for (int j = 0; j < N / 8; ++j) {
+            const int ch = 8 * j + c0;
+            if (ch >= a.Cout) break;
+            float v[2];
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+                float x = d[4 * j + 2 * i + c] + bias_s[ch + c];
+                x = generic_act ? act_fn(x, a.act, a.act_a, a.act_b) : fmaxf(x, slope * x);
                 if (a.round_out) x = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
-                v[j] = x;
+                v[c] = x;
             }
+            const bool two = ch + 1 < a.Cout;
             if (a.out_f16) {
-                if (vec_ok && nb + 16 <= a.Cout) {
-                    uint4 q0, q1;
-                    __half2* h0 = reinterpret_cast<__half2*>(&q0);
-                    __half2* h1 = reinterpret_cast<__half2*>(&q1);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) { h0[j] = __floats2half2_rn(v[2 * j], v[2 * j + 1]); h1[j] = __floats2half2_rn(v[8 + 2 * j], v[9 + 2 * j]); }
-                    *reinterpret_cast<uint4*>(oph + nb) = q0;
-                    *reinterpret_cast<uint4*>(oph + nb + 8) = q1;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (nb + j < a.Cout) oph[nb + j] = __float2half_rn(v[j]);
-                }
-            } else if (vec_ok && nb + 16 <= a.Cout) {
-#pragma unroll
-                for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(op + nb + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+                __half* o = reinterpret_cast<__half*>(a.dst) + oidx + ch;
+                if (pair_ok && two) *reinterpret_cast<__half2*>(o) = __floats2half2_rn(v[0], v[1]);
+                else { o[0] = __float2half_rn(v[0]); if (two) o[1] = __float2half_rn(v[1]); }
             } else {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    if (nb + j < a.Cout) op[nb + j] = v[j];
+                float* o = a.dst + oidx + ch;
+                if (pair_ok && two) *reinterpret_cast<float2*>(o) = make_float2(v[0], v[1]);
+                else { o[0] = v[0]; if (two) o[1] = v[1]; }
             }
         }
     }
 }
 
-// out-of-line copy of the generic epilogue for the staged kernel's rare fallback (keeps its hot code small)
-// (`a` by value: a reference would force the kernel's parameter block onto the local stack for the hot path as well)
-__device__ __noinline__ void epilogue_row_outofline(uint32_t trow, const TcArgs a, const float* bias_s, float* op, bool live, bool vec_ok) {
-    epilogue_row(trow, a, bias_s, op, live, vec_ok);
-}
-
-// ---- staged epilogue -----------------------------------------------------------------------------------------------------------
-// The source-level profile of round 1's register epilogue (profiles/r01_k2_fullres_f16_quad_ncu_details.txt and the source page of
-// the same capture) shows ~900 executed instructions per warp and tile spread over a 12 700-instruction kernel body
-// (23 % of the stall samples are instruction-fetch misses) -- per-element activation switches, predicates and 48 SEL + 16
-// SHFL per quad transpose.  This variant keeps the per-tile decisions out of the element loop (LeakyReLU as max(x, slope*x)
-// with slope = 1 for "no activation", rounding as a template parameter) and transposes through a 2 KB per-warp staging
-// buffer in shared memory instead of shuffles: every thread writes the 64 bytes of its pixel (4 x STS.128, XOR-swizzled,
-// conflict-free), then lane l reads chunk l%4 of pixel l/4 + 8k and stores it, so that one store instruction covers 8
-// pixels x 64 contiguous bytes.  One step = 16 fp32 or 32 half output channels.
-template <bool OUT_F16, bool ROUND>
-__device__ __forceinline__ void epilogue_staged(uint32_t trow, const TcArgs& a, const float* bias_s, uint32_t stg, uint8_t* const (&qptr)[4],
-                                                const bool (&qlive)[4], int lane, float slope) {
-    constexpr int kCols = OUT_F16 ? 32 : 16;        // output channels per 64-byte step
-    constexpr int kChunk = OUT_F16 ? 8 : 4;         // channels per 16-byte chunk
-    const uint32_t wrow = stg + (uint32_t)lane * 64u;
-    const uint32_t wsw = ((uint32_t)lane >> 1) & 3u;
-    const uint32_t c = (uint32_t)lane & 3u;
-    uint32_t raddr[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const uint32_t q = ((uint32_t)lane >> 2) + 8u * k;
-        raddr[k] = stg + q * 64u + ((c ^ ((q >> 1) & 3u)) << 4);
+// Stage release behind the in-flight wgmma group: after the group that read stages X is committed, the previous group is
+// waited for and the barriers of ITS stages get this warpgroup's arrival.
+struct Releaser {
+    uint32_t prev0 = 0, prev1 = 0;
+    __device__ __forceinline__ void after_commit(uint32_t bar0, uint32_t bar1, bool leader) {
+        wgmma_wait<1>();
+        if (leader) { if (prev0) mbar_arrive(prev0); if (prev1) mbar_arrive(prev1); }
+        prev0 = bar0; prev1 = bar1;
     }
-    for (int n0 = 0; n0 < a.n_pad; n0 += kCols) {
-        uint32_t r0[16], r1[16];
-        tmem_ld16_nowait(trow + (uint32_t)n0, r0);
-        const bool second = OUT_F16 && (n0 + 16 < a.n_pad);
-        if (second) tmem_ld16_nowait(trow + (uint32_t)(n0 + 16), r1);
-        tmem_ld_wait();
-        uint4 e[4];
-        if (OUT_F16) {
-            __half2* h = reinterpret_cast<__half2*>(e);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                float x0 = __uint_as_float(r0[2 * j]) + bias_s[n0 + 2 * j], x1 = __uint_as_float(r0[2 * j + 1]) + bias_s[n0 + 2 * j + 1];
-                h[j] = __floats2half2_rn(fmaxf(x0, slope * x0), fmaxf(x1, slope * x1));
-            }
-            if (second) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    float x0 = __uint_as_float(r1[2 * j]) + bias_s[n0 + 16 + 2 * j], x1 = __uint_as_float(r1[2 * j + 1]) + bias_s[n0 + 17 + 2 * j];
-                    h[8 + j] = __floats2half2_rn(fmaxf(x0, slope * x0), fmaxf(x1, slope * x1));
-                }
-            } else {
-                e[2] = make_uint4(0u, 0u, 0u, 0u);
-                e[3] = make_uint4(0u, 0u, 0u, 0u);
-            }
-        } else {
-            uint32_t* w = reinterpret_cast<uint32_t*>(e);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-                float x = __uint_as_float(r0[j]) + bias_s[n0 + j];
-                x = fmaxf(x, slope * x);
-                w[j] = ROUND ? ((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u) : __float_as_uint(x);
-            }
-        }
-#pragma unroll
-        for (uint32_t cc = 0; cc < 4; ++cc)
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(wrow + ((cc ^ wsw) << 4)), "r"(e[cc].x), "r"(e[cc].y),
-                         "r"(e[cc].z), "r"(e[cc].w)
-                         : "memory");
-        __syncwarp();
-        const bool col_ok = n0 + (int)c * kChunk + kChunk <= a.Cout;
-        const size_t boff = ((size_t)n0 * (OUT_F16 ? 2 : 4)) + (size_t)c * 16;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            uint4 v;
-            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(raddr[k]) : "memory");
-            if (qlive[k] && col_ok) *reinterpret_cast<uint4*>(qptr[k] + boff) = v;
-        }
-        __syncwarp();
+    __device__ __forceinline__ void drain(bool leader) {
+        wgmma_wait<0>();
+        if (leader) { if (prev0) mbar_arrive(prev0); if (prev1) mbar_arrive(prev1); }
+        prev0 = prev1 = 0;
     }
-}
+};
 
-// One tile of the staged epilogue for a warp (TMEM lane quadrant q): output pointers / liveness of the 4 pixels each lane
-// stores for, then the 64-byte steps; tiles are kTW x kTH pixels with accumulator row p = y * kTW + x.  Layers the staged
-// path cannot take (unaligned channel slices, the rare activations) go through the generic out-of-line epilogue.
-template <int kTW, int kTH>
-__device__ __forceinline__ void staged_tile(const TcArgs& a, const float* bias_s, uint32_t stg, int q, int lane, int b, int tile_y,
-                                            int tile_x, uint32_t trow, bool lean_ok, bool vec_ok, float slope, int oy_off, int ox_off) {
-    if (lean_ok) {
-        const size_t esize = a.out_f16 ? 2 : 4;
-        uint8_t* qptr[4];
-        bool qlive[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {       // accumulator rows 32q + lane/4 + 8k
-            const int pq = 32 * q + (lane >> 2) + 8 * k;
-            const int qy = tile_y * kTH + pq / kTW, qx = tile_x * kTW + pq % kTW;
-            qlive[k] = (qy < a.Ho) && (qx < a.Wo);
-            const size_t qidx = (((size_t)b * a.dst_H + (qy * a.oy_step + oy_off)) * a.dst_W + (qx * a.ox_step + ox_off)) *
-                                    a.dst_c + a.dst_coff;
-            qptr[k] = reinterpret_cast<uint8_t*>(a.dst) + qidx * esize;
-        }
-        if (a.out_f16) epilogue_staged<true, false>(trow, a, bias_s, stg, qptr, qlive, lane, slope);
-        else if (a.round_out) epilogue_staged<false, true>(trow, a, bias_s, stg, qptr, qlive, lane, slope);
-        else epilogue_staged<false, false>(trow, a, bias_s, stg, qptr, qlive, lane, slope);
-    } else {
-        const int p = 32 * q + lane;
-        const int oy = tile_y * kTH + p / kTW, ox = tile_x * kTW + p % kTW;
-        const size_t oidx = (((size_t)b * a.dst_H + (oy * a.oy_step + oy_off)) * a.dst_W + (ox * a.ox_step + ox_off)) *
-                                a.dst_c + a.dst_coff;
-        const bool live = (oy < a.Ho) && (ox < a.Wo);
-        if (a.Cout == 1) {
-            // single-channel heads (sigmoid / a + b |tanh|): one accumulator column per pixel instead of the generic path's 16
-            // activations per pixel (measured: 24->1 3x3 at full resolution 123 us with the generic epilogue)
-            uint32_t r;
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(trow));
-            tmem_ld_wait();
-            float x = act_fn(__uint_as_float(r) + bias_s[0], a.act, a.act_a, a.act_b);
-            if (a.round_out) x = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
-            if (live) {
-                if (a.out_f16) reinterpret_cast<__half*>(a.dst)[oidx] = __float2half_rn(x);
-                else a.dst[oidx] = x;
-            }
-        } else {
-            float* op = a.out_f16 ? reinterpret_cast<float*>(reinterpret_cast<__half*>(a.dst) + oidx) : a.dst + oidx;
-            epilogue_row_outofline(trow, a, bias_s, op, live, vec_ok);
-        }
-    }
-}
-
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-
-// Persistent: each CTA loops over output tiles (tile = blockIdx.x, += gridDim.x).  The TMA->MMA shared-memory ring keeps
-// flowing across tile boundaries and the accumulator is double-buffered in TMEM, so the epilogue of tile i overlaps the
-// main loop of tile i+1.
+// Persistent: each CTA loops over output tiles (tile = blockIdx.x, += gridDim.x).  The TMA ring keeps flowing across tile
+// boundaries, so the loads of tile i+1 overlap the epilogue of tile i.  Tile = 8 rows x 16 columns, accumulator row
+// p = y * 16 + x.
+template <int N, bool F16>
 __global__ void __launch_bounds__(kTcThreads)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmB1,
                const __grid_constant__ CUtensorMap tmB2, const __grid_constant__ CUtensorMap tmB3, const TcArgs a) {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t bars[2 * 8 + 4];   // full[8], empty[8], tmem_full[2], tmem_empty[2]
-    __shared__ uint32_t tmem_base_s;
+    __shared__ __align__(8) uint64_t bars[2 * 8];   // full[8], empty[8]
     __shared__ float bias_s[256];
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // (the broadcast tells ptxas the role branches are warp-uniform)
@@ -387,34 +403,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
     const uint32_t stage_bytes = a_bytes + b_bytes;
     const int stages = a.stages;
     const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[8]);
-    const uint32_t tfull0 = smem_u32(&bars[16]), tempty0 = smem_u32(&bars[18]);
     const int chunks_per_tap = a.chunks[0] + a.chunks[1] + a.chunks[2];
     const int n_phase = a.n_phase;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < stages; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+        for (int s = 0; s < stages; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 256; i += kTcThreads) bias_s[i] = (a.bias != nullptr && i < a.Cout) ? __ldg(a.bias + i) : 0.f;
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         prefetch_tmap(&tmA0);
         if (a.n_src > 1) prefetch_tmap(&tmA1);
         if (a.n_src > 2) prefetch_tmap(&tmA2);
         prefetch_tmap(&tmB);
         if (n_phase > 1) { prefetch_tmap(&tmB1); prefetch_tmap(&tmB2); prefetch_tmap(&tmB3); }
     }
-    if (warp == 1) {   // TMEM allocation (power of two >= 32 columns), address published through shared memory
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)),
-                     "r"(a.tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_s;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ===================== TMA producer (whole warp, converged; the copies are issued by an elected lane) =====================
         int st = 0;
         uint32_t ph = 0;
@@ -443,75 +449,45 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
                     }
                 }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (whole warp, converged; the MMAs are issued by an elected lane) =====================
-        // instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 @[4,6), a/b format TF32 = 2 @[7,10)/[10,13),
-        // K-major A and B, N >> 3 @[17,23), M >> 4 @[24,29)
-        const uint32_t idesc = a.idesc;
+    } else if (warp < kProducerWarp) {
+        // ===================== consumer warpgroup wg: accumulator rows [64 wg, 64 wg + 64) =====================
+        const int wg = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
         const uint32_t dhi = desc_hi(8u * (uint32_t)a.row_bytes, (uint32_t)a.row_bytes);
-        const int ksteps = a.row_bytes / 32;   // UMMA K = 32 bytes (8 tf32 / 16 half): 4 (2) steps inside the 128 (64)-byte swizzle row
-        auto run = [&](auto f16tag) {
-        constexpr bool kF16 = decltype(f16tag)::value;
-        int st = 0, lt = 0;
+        const uint32_t a_off = 64u * (uint32_t)a.row_bytes * (uint32_t)wg;
+        const uint32_t b_row16 = (uint32_t)a.row_bytes >> 4;
+        const int ksteps = a.row_bytes / 32;   // MMA K = 32 bytes (8 tf32 / 16 half): 4 (2) steps inside the 128 (64)-byte swizzle row
+        float d[N / 2];
+        Releaser rel;
+        int st = 0;
         uint32_t ph = 0;
-        for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++lt) {
-            const int buf = lt & 1;
-            mbar_wait(tempty0 + 8 * buf, (((uint32_t)lt >> 1) & 1u) ^ 1u);   // epilogue has drained this accumulator
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t acc = tmem_d + (uint32_t)(buf * a.n_pad);
-            const int phs = tile % n_phase;
+        for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
+            const int sp = tile / n_phase, phs = tile - sp * n_phase;
+            const int b = sp / a.tiles_per_img, t = sp - b * a.tiles_per_img;
+            const int tile_y = t / a.tiles_x, tile_x = t - tile_y * a.tiles_x;
             const int total = a.ph_kh[phs] * a.ph_kw[phs] * chunks_per_tap;
             uint32_t accf = 0;
             int src = 0, jc = 0;                                             // source / chunk inside the source of step c
             for (int c = 0; c < total; ++c) {
                 mbar_wait(full0 + 8 * st, ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
                 const uint32_t sa = tile_base + st * stage_bytes;
-                const uint32_t alo = desc_lo(sa), blo = desc_lo(sa + a_bytes);
+                const uint32_t alo = desc_lo(sa + a_off), blo = desc_lo(sa + a_bytes);
                 const int ks = (jc == a.chunks[src] - 1) ? a.tail_ksteps[src] : ksteps;
-                umma_elect<kF16>(acc, alo, dhi, blo, dhi, idesc, accf);
-                if (ks > 1) umma_elect<kF16>(acc, alo + 2, dhi, blo + 2, dhi, idesc, 1u);
-                if (ks > 2) umma_elect<kF16>(acc, alo + 4, dhi, blo + 4, dhi, idesc, 1u);
-                if (ks > 3) umma_elect<kF16>(acc, alo + 6, dhi, blo + 6, dhi, idesc, 1u);
                 if (++jc == a.chunks[src]) { jc = 0; if (++src == a.n_src) src = 0; }
-                accf = 1u;
-                umma_commit_elect(empty0 + 8 * st);                          // frees the smem stage once these MMAs have read it
-                if (c == total - 1) umma_commit_elect(tfull0 + 8 * buf);     // accumulator complete
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    if (k < ks) mma_tile<N, F16>(d, desc(alo + 2 * k, dhi), desc(blo + 2 * k, dhi), b_row16, accf);
+                    accf = 1u;
+                }
+                wgmma_commit();
+                rel.after_commit(empty0 + 8 * st, 0, leader);                 // frees the previous stage once its group retired
                 if (++st == stages) { st = 0; ph ^= 1u; }
             }
+            rel.drain(leader);
+            epilogue_wg<N, kTileW, kTileH>(d, a, bias_s, 64 * wg + 16 * (warp & 3), lane, b, tile_y, tile_x, a.ph_oy_off[phs],
+                                           a.ph_ox_off[phs]);
         }
-        };
-        if (a.f16) run(std::true_type{}); else run(std::false_type{});
-    } else {
-        // ===================== epilogue, staged through shared memory (see epilogue_staged) =====================
-        __shared__ __align__(16) uint8_t stage_s[4][2048];
-        const int q = warp & 3;                 // TMEM lane quadrant this warp may read (the 4 epilogue warps have distinct ones)
-        const uint32_t stg = smem_u32(&stage_s[q][0]);
-        const bool vec_ok = ((a.dst_c | a.dst_coff) & (a.out_f16 ? 7 : 3)) == 0;
-        const bool lean_ok = vec_ok && (a.Cout & (a.out_f16 ? 7 : 3)) == 0 && !(a.out_f16 && a.round_out) &&
-                             (a.act == MR_ACT_NONE || a.act == MR_ACT_LEAKY);
-        const float slope = a.act == MR_ACT_LEAKY ? a.act_a : 1.0f;
-        int lt = 0;
-        for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++lt) {
-            const int sp = tile / n_phase, phs = tile - sp * n_phase;
-            const int b = sp / a.tiles_per_img, t = sp - b * a.tiles_per_img;
-            const int tile_y = t / a.tiles_x, tile_x = t - tile_y * a.tiles_x;
-            const int buf = lt & 1;
-            mbar_wait(tfull0 + 8 * buf, ((uint32_t)lt >> 1) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t trow = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(buf * a.n_pad);
-            staged_tile<kTileW, kTileH>(a, bias_s, stg, q, lane, b, tile_y, tile_x, trow, lean_ok, vec_ok, slope, a.ph_oy_off[phs],
-                                        a.ph_ox_off[phs]);
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty0 + 8 * buf);
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(a.tmem_cols));
     }
 }
 
@@ -524,23 +500,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
 //     (ky * P + kx) rows of 128 / 64 B, stride between 8-row groups = one halo row (P rows); the swizzle is a function of the
 //     absolute shared-memory address, so neither shift needs to be a multiple of the 8-row swizzle atom.
 //     L2->SM traffic drops from kh*kw boxes per tile to one.
-// Output tile = 16 rows x 8 columns (an 8-row MMA group = 8 adjacent pixels of one output row).
+// Output tile = 16 rows x 8 columns (an 8-row MMA group = 8 adjacent pixels of one output row); warpgroup wg computes output
+// rows 8 wg .. 8 wg + 7, accumulator row p = y * 8 + x.
 // -------------------------------------------------------------------------------------------------------------------------
-// ROWB: bytes per shared-memory row, 128 or 64 (half sources of <= 32 channels)
-template <int ROWB>
+template <int N, bool F16>
 __global__ void __launch_bounds__(kTcThreads)
 conv_tc_halo_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                     const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB, const TcArgs a) {
     extern __shared__ uint8_t smem_raw[];
-    constexpr int kBufs = 2;                                     // TMEM accumulators (double-buffered)
-    // afull[4], aempty[4], tmem_full[kBufs], tmem_empty[kBufs], bfull, streamed weights: bsfull[8], bsempty[8]
-    __shared__ __align__(8) uint64_t bars[2 * 4 + 2 * kBufs + 1 + 16];
-    __shared__ uint32_t tmem_base_s;
+    // afull[4], aempty[4], bfull, streamed weights: bsfull[8], bsempty[8]
+    __shared__ __align__(8) uint64_t bars[2 * 4 + 1 + 16];
     __shared__ float bias_s[256];
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // (the broadcast tells ptxas the role branches are warp-uniform)
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    constexpr uint32_t row_bytes = (uint32_t)ROWB;
+    const uint32_t row_bytes = (uint32_t)a.row_bytes;
     const uint32_t b_bytes = (uint32_t)a.n_pad * row_bytes;
     const int chunks_per_tap = a.chunks[0] + a.chunks[1] + a.chunks[2];
     const int taps = a.kh * a.kw;
@@ -552,35 +526,25 @@ conv_tc_halo_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_const
     const uint32_t a_tx = (uint32_t)(16 + a.kh - 1) * pitch * row_bytes;           // bytes one box delivers
     const uint32_t a_base = base + ((bres_bytes + 1023u) & ~1023u);
     const int stages = a.stages;
-    const uint32_t afull0 = smem_u32(&bars[0]), aempty0 = smem_u32(&bars[4]);
-    const uint32_t tfull0 = smem_u32(&bars[8]), tempty0 = smem_u32(&bars[8 + kBufs]), bfull = smem_u32(&bars[8 + 2 * kBufs]);
-    const uint32_t bsfull0 = smem_u32(&bars[9 + 2 * kBufs]), bsempty0 = smem_u32(&bars[17 + 2 * kBufs]);
+    const uint32_t afull0 = smem_u32(&bars[0]), aempty0 = smem_u32(&bars[4]), bfull = smem_u32(&bars[8]);
+    const uint32_t bsfull0 = smem_u32(&bars[9]), bsempty0 = smem_u32(&bars[17]);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < stages; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, 1); }
-        for (int s = 0; s < kBufs; ++s) { mbar_init(tfull0 + 8 * s, 1); mbar_init(tempty0 + 8 * s, 4); }
+        for (int s = 0; s < stages; ++s) { mbar_init(afull0 + 8 * s, 1); mbar_init(aempty0 + 8 * s, 2); }
         mbar_init(bfull, 1);
-        for (int s = 0; s < nbs; ++s) { mbar_init(bsfull0 + 8 * s, 1); mbar_init(bsempty0 + 8 * s, 1); }
+        for (int s = 0; s < nbs; ++s) { mbar_init(bsfull0 + 8 * s, 1); mbar_init(bsempty0 + 8 * s, 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 256; i += kTcThreads) bias_s[i] = (a.bias != nullptr && i < a.Cout) ? __ldg(a.bias + i) : 0.f;
-    if (warp == 0 && lane == 0) {
+    if (warp == kProducerWarp && lane == 0) {
         prefetch_tmap(&tmA0);
         if (a.n_src > 1) prefetch_tmap(&tmA1);
         if (a.n_src > 2) prefetch_tmap(&tmA2);
         prefetch_tmap(&tmB);
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)),
-                     "r"(a.tmem_cols));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_s;
 
-    if (warp == 0) {
+    if (warp == kProducerWarp) {
         // ===================== TMA producer (whole warp, converged; the copies are issued by an elected lane) =====================
         // resident weights: every (tap, chunk) slice [n_pad x chunk] once
         if (nbs == 0) {
@@ -615,88 +579,64 @@ conv_tc_halo_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_const
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (whole warp, converged; the MMAs are issued by an elected lane) =====================
-        const uint32_t idesc = a.idesc;
+    } else if (warp < kProducerWarp) {
+        // ===================== consumer warpgroup wg: output rows [8 wg, 8 wg + 8) of the 16-row tile =====================
+        const int wg = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
         const uint32_t dhi_a = desc_hi(pitch * row_bytes, row_bytes);      // stride between 8-row groups = one halo row
         const uint32_t dhi_b = desc_hi(8u * row_bytes, row_bytes);
         const uint32_t tap_dx = row_bytes >> 4, tap_dy = (pitch * row_bytes) >> 4;   // descriptor steps of one tap to the right / down
-        const uint32_t b_step = b_bytes >> 4;
+        const uint32_t b_step = b_bytes >> 4, b_row16 = row_bytes >> 4;
+        const uint32_t a_off = 8u * pitch * row_bytes * (uint32_t)wg;
+        const int ksteps = a.row_bytes / 32;
         if (nbs == 0) mbar_wait(bfull, 0);
-        auto run = [&](auto f16tag) {
-        constexpr bool kF16 = decltype(f16tag)::value;
-        int st = 0, bs = 0, lt = 0;
+        float d[N / 2];
+        Releaser rel;
+        int st = 0, bs = 0;
         uint32_t ph = 0, bph = 0;
-        for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++lt) {
-            const int buf = lt & (kBufs - 1);
-            mbar_wait(tempty0 + 8 * buf, (((uint32_t)lt >> 1) & 1u) ^ 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t acc = tmem_d + (uint32_t)(buf * a.n_pad);
+        for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x) {
+            const int b = tile / a.tiles_per_img, t = tile - b * a.tiles_per_img;
+            const int tile_y = t / a.tiles_x, tile_x = t - tile_y * a.tiles_x;
             uint32_t accf = 0;
             int src = 0, jc = 0;                                             // source / chunk inside the source of chunk cg
             for (int cg = 0; cg < chunks_per_tap; ++cg) {
-                const int ks = (jc == a.chunks[src] - 1) ? a.tail_ksteps[src] : ROWB / 32;
+                const int ks = (jc == a.chunks[src] - 1) ? a.tail_ksteps[src] : ksteps;
                 if (++jc == a.chunks[src]) { jc = 0; ++src; }
                 mbar_wait(afull0 + 8 * st, ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                uint32_t alo_row = desc_lo(a_base + st * a_bytes);
+                uint32_t alo_row = desc_lo(a_base + st * a_bytes + a_off);
                 uint32_t blo = desc_lo(base) + (uint32_t)cg * b_step;                 // resident: slice (tap 0, chunk cg)
                 for (int ky = 0; ky < a.kh; ++ky, alo_row += tap_dy) {
                     uint32_t alo = alo_row;
                     for (int kx = 0; kx < a.kw; ++kx, alo += tap_dx) {
                         if (nbs > 0) {
                             mbar_wait(bsfull0 + 8 * bs, bph);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
                             blo = desc_lo(base + (uint32_t)bs * b_bytes);
                         }
+                        wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < ROWB / 32; ++k) {   // 32 bytes of K per MMA (8 tf32 / 16 half): 4 per 128-byte row, 2 per 64-byte row
-                            if (k < ks) umma_elect<kF16>(acc, alo + 2 * k, dhi_a, blo + 2 * k, dhi_b, idesc, accf);
+                        for (int k = 0; k < 4; ++k) {   // 32 bytes of K per MMA (8 tf32 / 16 half): 4 per 128-byte row, 2 per 64-byte row
+                            if (k < ks) mma_tile<N, F16>(d, desc(alo + 2 * k, dhi_a), desc(blo + 2 * k, dhi_b), b_row16, accf);
                             accf = 1u;
                         }
-                        if (nbs > 0) {
-                            umma_commit_elect(bsempty0 + 8 * bs);   // frees the weight stage once these MMAs have read it
+                        if (nbs > 0) {   // one group per tap: frees the weight stage (and after the last tap the input stage)
+                            wgmma_commit();
+                            const bool last = ky == a.kh - 1 && kx == a.kw - 1;
+                            rel.after_commit(bsempty0 + 8 * bs, last ? aempty0 + 8 * st : 0u, leader);
                             if (++bs == nbs) { bs = 0; bph ^= 1u; }
                         } else {
                             blo += (uint32_t)chunks_per_tap * b_step;   // next tap, same chunk
                         }
                     }
                 }
-                umma_commit_elect(aempty0 + 8 * st);
-                if (cg == chunks_per_tap - 1) umma_commit_elect(tfull0 + 8 * buf);
+                if (nbs == 0) {
+                    wgmma_commit();
+                    rel.after_commit(aempty0 + 8 * st, 0u, leader);
+                }
                 if (++st == stages) { st = 0; ph ^= 1u; }
             }
+            rel.drain(leader);
+            epilogue_wg<N, 8, 16>(d, a, bias_s, 64 * wg + 16 * (warp & 3), lane, b, tile_y, tile_x, a.oy_off, a.ox_off);
         }
-        };
-        if (a.f16) run(std::true_type{}); else run(std::false_type{});
-    } else {
-        // ===================== epilogue, staged through shared memory (tile = 16 rows x 8 columns) =====================
-        __shared__ __align__(16) uint8_t stage_s[4][2048];
-        const int q = warp & 3;                 // TMEM lane quadrant
-        const uint32_t stg = smem_u32(&stage_s[warp - 2][0]);
-        const bool vec_ok = ((a.dst_c | a.dst_coff) & (a.out_f16 ? 7 : 3)) == 0;
-        const bool lean_ok = vec_ok && (a.Cout & (a.out_f16 ? 7 : 3)) == 0 && !(a.out_f16 && a.round_out) &&
-                             (a.act == MR_ACT_NONE || a.act == MR_ACT_LEAKY);
-        const float slope = a.act == MR_ACT_LEAKY ? a.act_a : 1.0f;
-        int lt = 0;
-        for (int tile = blockIdx.x; tile < a.total_tiles; tile += gridDim.x, ++lt) {
-            const int b = tile / a.tiles_per_img, t = tile - b * a.tiles_per_img;
-            const int tile_y = t / a.tiles_x, tile_x = t - tile_y * a.tiles_x;
-            const int buf = lt & (kBufs - 1);
-            mbar_wait(tfull0 + 8 * buf, ((uint32_t)lt >> 1) & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t trow = tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(buf * a.n_pad);
-            staged_tile<8, 16>(a, bias_s, stg, q, lane, b, tile_y, tile_x, trow, lean_ok, vec_ok, slope, a.oy_off, a.ox_off);
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty0 + 8 * buf);
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(a.tmem_cols));
     }
 }
 
@@ -715,6 +655,44 @@ EncodeTiledFn get_encode_fn() {
             fn = reinterpret_cast<EncodeTiledFn>(p);
     }
     return fn;
+}
+
+// the two kernels for MMA N = n_pad (16..256, multiple of 16) and the source type
+struct TcKernels {
+    const void* tap;
+    const void* halo;
+};
+template <int N>
+TcKernels tc_kernels_n(bool f16) {
+    if (f16) return {(const void*)conv_tc_kernel<N, true>, (const void*)conv_tc_halo_kernel<N, true>};
+    return {(const void*)conv_tc_kernel<N, false>, (const void*)conv_tc_halo_kernel<N, false>};
+}
+TcKernels tc_kernels(int n_pad, bool f16) {
+    switch (n_pad / 16) {
+        case 1: return tc_kernels_n<16>(f16);
+        case 2: return tc_kernels_n<32>(f16);
+        case 3: return tc_kernels_n<48>(f16);
+        case 4: return tc_kernels_n<64>(f16);
+        case 5: return tc_kernels_n<80>(f16);
+        case 6: return tc_kernels_n<96>(f16);
+        case 7: return tc_kernels_n<112>(f16);
+        case 8: return tc_kernels_n<128>(f16);
+        case 9: return tc_kernels_n<144>(f16);
+        case 10: return tc_kernels_n<160>(f16);
+        case 11: return tc_kernels_n<176>(f16);
+        case 12: return tc_kernels_n<192>(f16);
+        case 13: return tc_kernels_n<208>(f16);
+        case 14: return tc_kernels_n<224>(f16);
+        case 15: return tc_kernels_n<240>(f16);
+        default: return tc_kernels_n<256>(f16);
+    }
+}
+
+// CTAs of `kernel` one SM can hold as far as registers and static shared memory go
+int resident_ctas(const void* kernel) {
+    int n = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kTcThreads, 0) != cudaSuccess) return 1;
+    return n > 0 ? n : 1;
 }
 
 }  // namespace
@@ -768,40 +746,34 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     const int esize = f16 ? 2 : 4;
     const int cmult = f16 ? 8 : 4;            // pixel stride must be a multiple of 16 bytes for TMA
     a.row_bytes = kc * (f16 ? 2 : 4);
-    a.kc = kc; a.f16 = f16 ? 1 : 0; a.out_f16 = (d.dst_dtype == MR_DT_F16) ? 1 : 0;
-    // UMMA instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 @[4,6); a/b format @[7,10)/[10,13): TF32 = 2,
-    // F16 = 0; K-major A and B; N >> 3 @[17,23); M >> 4 @[24,29)
-    a.idesc = (1u << 4) | ((f16 ? 0u : 2u) << 7) | ((f16 ? 0u : 2u) << 10) | ((uint32_t)(n_pad >> 3) << 17) | ((128u >> 4) << 24);
+    a.kc = kc; a.out_f16 = (d.dst_dtype == MR_DT_F16) ? 1 : 0;
+    const TcKernels kern = tc_kernels(n_pad, f16);
     int ksum = 0;
     // "halo" variant (one input box per tile, resident weights): stride 1, taps reach at most 8 px to the right, weights fit
     int chunks_all = 0;
     for (int s = 0; s < d.n_src; ++s) chunks_all += (d.src_c[s] + kc - 1) / kc;
     const size_t bres = (size_t)d.kh * d.kw * chunks_all * n_pad * a.row_bytes;
     // MONOREC_B200_TC_HALO: unset = automatic, 0 = never, n = 1..4: at most n CTAs per SM (1: also layers that only fit once).
-    // History of the rule: with 16-px box rows only the 32-channel layers fitted twice per SM (32->32 3x3 over the single-frame
-    // volumes: 631 -> 452 us in TF32, 489 -> 203 us in half) and one CTA per SM lost to the tap-refetch kernel (48->48 3x3:
-    // 300 -> 335 us); with (8 + kw - 1)-px rows the 48-channel full-resolution layers fit twice as well (profiles/r02_k2_pitch.txt).
+    // Box rows are 8 + kw - 1 px, so a box holds exactly the pixels the taps touch and the 48-channel full-resolution layers
+    // fit twice per SM next to their weights.
     static const int halo_env = getenv("MONOREC_B200_TC_HALO") ? atoi(getenv("MONOREC_B200_TC_HALO")) : -1;
     static const bool halo_f16 = getenv("MONOREC_B200_TC_HALO_F16") ? (atoi(getenv("MONOREC_B200_TC_HALO_F16")) != 0) : true;
-    // (64-byte rows are fine inside the halo box too: half sources of <= 32 channels packed with 32-channel chunks; measured
-    // 429 -> 203 us on the 32->32 3x3 layer over the single-frame volumes, profiles/r02_k2_variants.txt)
-    // MONOREC_B200_TC_HALO_PITCH=16: the fixed 16-px rows of the first halo kernel (A/B measurements)
+    // (64-byte rows are fine inside the halo box too: half sources of <= 32 channels packed with 32-channel chunks)
+    // MONOREC_B200_TC_HALO_PITCH=16: fixed 16-px box rows (A/B measurements)
     static const int pitch_env = getenv("MONOREC_B200_TC_HALO_PITCH") ? atoi(getenv("MONOREC_B200_TC_HALO_PITCH")) : 0;
     const int halo_pitch = (pitch_env >= 8 + d.kw - 1) ? pitch_env : 8 + d.kw - 1;
     const size_t halo_a_bytes = ((size_t)(16 + d.kh - 1) * halo_pitch * a.row_bytes + 1023) & ~size_t(1023);
     const size_t bres_al = (bres + 1023) & ~size_t(1023);
-    uint32_t halo_cols = 32;               // TMEM columns one CTA allocates (two accumulators)
-    while (halo_cols < (uint32_t)(2 * n_pad)) halo_cols <<= 1;
+    // CTAs per SM the accumulator registers allow (the wider N, the more registers per consumer thread)
+    const int halo_reg_ctas = resident_ctas(kern.halo);
     auto halo_fit = [&](int ctas) {   // A stages that fit next to the resident weights with `ctas` CTAs per SM
-        if ((uint32_t)ctas * halo_cols > 512) return 0;
-        // 228 KB per SM, 1 KB reserved per CTA; static per CTA: 8 KB epilogue staging + 1 KB bias + barriers; 1 KB alignment slack
-        const size_t budget = (size_t)(ctas == 1 ? 210 : 228) * 1024 / ctas - (1 + 8 + 1 + 1) * 1024 - 512;
+        if (ctas > halo_reg_ctas) return 0;
+        // 228 KB per SM, 1 KB reserved per CTA; static per CTA: 1 KB bias + barriers; 1 KB alignment slack
+        const size_t budget = (size_t)(ctas == 1 ? 210 : 228) * 1024 / ctas - (1 + 1 + 1) * 1024 - 512;
         int st = bres_al + 1024 < budget ? (int)((budget - 1024 - bres_al) / halo_a_bytes) : 0;
         return st > 4 ? 4 : st;
     };
-    // CTAs per SM: up to three, each with at least two input stages (up to 4).  Measured after the issue loops moved to the
-    // uniform datapath (profiles/r02_k2_ctas2.txt): cap 2 / 3 / 4 -> half-mode forward 3.98 / 3.94 / 4.06 ms, 32->32 3x3 over
-    // the single-frame volumes 159 / 143 / 193 us (before that change 3-4 CTAs were slower than 2: profiles/r02_k2_ctas.txt).
+    // CTAs per SM: up to three, each with at least two input stages (up to 4).
     // MONOREC_B200_TC_HALO=n (1..4) caps / forces the count for measurements (1: also layers that only fit once).
     int halo_ctas = 0;
     if (n_phases == 1 && halo_env != 0 && (!f16 || halo_f16) && d.sy == 1 && d.sx == 1 && d.kw <= 9 && d.kh <= 7) {
@@ -811,14 +783,14 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     }
     // Weights that do not fit next to two input stages stream instead: the [n_pad x chunk] slice of each (chunk, tap) goes through
     // a ring of 3..8 stages behind the chunk's input box.  Per tile that is all the weights once (L2 hits) plus ONE input box per
-    // chunk, against kh*kw input boxes + the same weights in the tap-refetch kernel -- the multi-source decoder layers were bound
-    // by that L2->SM traffic (~12.7 TB/s aggregate on the 32+64->48 3x3 layer).  MONOREC_B200_TC_STREAM=0 disables it (A/B).
+    // chunk, against kh*kw input boxes + the same weights in the tap-refetch kernel, whose L2->SM traffic bounds the
+    // multi-source decoder layers.  MONOREC_B200_TC_STREAM=0 disables it (A/B).
     static const bool stream_on = getenv("MONOREC_B200_TC_STREAM") ? (atoi(getenv("MONOREC_B200_TC_STREAM")) != 0) : true;
     int b_stream = 0, stream_stages = 0;
     const size_t b_slice = (size_t)n_pad * a.row_bytes;
     if (halo_ctas == 0 && stream_on && n_phases == 1 && halo_env != 0 && (!f16 || halo_f16) && d.sy == 1 && d.sx == 1 && d.kw <= 9 &&
-        d.kh <= 7 && d.kh * d.kw > 1 && 2 * halo_cols <= 512) {
-        const size_t budget = (size_t)228 * 1024 / 2 - (1 + 8 + 1 + 1) * 1024 - 512 - 1024;
+        d.kh <= 7 && d.kh * d.kw > 1 && halo_reg_ctas >= 2) {
+        const size_t budget = (size_t)228 * 1024 / 2 - (1 + 1 + 1) * 1024 - 512 - 1024;
         if (budget > 2 * halo_a_bytes + 3 * b_slice) {
             int nb = (int)((budget - 2 * halo_a_bytes) / b_slice);
             if (nb > 8) nb = 8;
@@ -886,27 +858,21 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     const size_t stage_bytes = (size_t)(128 + n_pad) * a.row_bytes;
     a.tiles_per_img = tiles;
     a.total_tiles = tiles * d.B * n_phases;
-    // persistent grid: two CTAs per SM when two double-buffered accumulators fit TMEM (2 x 2 x n_pad <= 512 columns),
-    // otherwise one CTA per SM with a deeper ring
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    // persistent grid over the SMs of the current device
+    int dev = 0, sms = 0;
+    MR_CUDA(cudaGetDevice(&dev));
+    MR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     static const int kForceCtas = getenv("MONOREC_B200_TC_CTAS") ? atoi(getenv("MONOREC_B200_TC_CTAS")) : 0;   // tuning knob
-    // resident CTAs per SM: bounded by TMEM (each CTA holds a power-of-two >= 2 * n_pad columns of the 512) and capped at 4;
-    // with UMMA N = 32..64 one CTA cannot keep the tensor pipe busy, so several CTAs interleave their MMA chains
-    uint32_t cols_needed = 32;
-    while (cols_needed < (uint32_t)(2 * n_pad)) cols_needed <<= 1;
-    int ctas_per_sm = (int)(512 / cols_needed);
-    if (ctas_per_sm > 4) ctas_per_sm = 4;
-    if (kForceCtas > 0 && (uint32_t)kForceCtas * cols_needed <= 512) ctas_per_sm = kForceCtas;
-    const size_t budget = (size_t)(200 * 1024) / ctas_per_sm - 8 * 1024;
+    // resident CTAs per SM: bounded by the accumulator registers and capped at 4; with MMA N = 32..64 one CTA cannot keep the
+    // tensor pipe busy, so several CTAs interleave their MMA chains
+    const int reg_ctas = resident_ctas(kern.tap);
+    int ctas_per_sm = reg_ctas > 4 ? 4 : reg_ctas;
+    if (kForceCtas > 0 && kForceCtas <= reg_ctas) ctas_per_sm = kForceCtas;
+    const size_t budget = (size_t)(200 * 1024) / ctas_per_sm - 2 * 1024;
     int stages = (int)(budget / stage_bytes);
     if (stages > 8) stages = 8;
     if (stages < 2) stages = 2;
     a.stages = stages;
-    uint32_t cols = 32;
-    while (cols < (uint32_t)(2 * n_pad)) cols <<= 1;
-    a.tmem_cols = cols;
     a.bias = d.bias; a.dst = d.dst;
     a.dst_H = d.dst_H; a.dst_W = d.dst_W; a.dst_c = d.dst_c; a.dst_coff = d.dst_coff;
     a.oy_step = d.oy_step; a.ox_step = d.ox_step; a.oy_off = d.oy_off; a.ox_off = d.ox_off;
@@ -919,21 +885,18 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
         const size_t smem = halo_front + (size_t)halo_stages * halo_a_bytes + 1024;
         int grid = sms * halo_ctas;
         if (grid > a.total_tiles) grid = a.total_tiles;
-        auto launch_halo = [&](auto kernel, int threads) -> int {
-            MR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(212 * 1024)));
-            kernel<<<grid, threads, smem, (cudaStream_t)stream>>>(tmA[0], tmA[1], tmA[2], tmB, a);
-            return MR_OK;
-        };
-        const int lrc = a.row_bytes == 128 ? launch_halo(conv_tc_halo_kernel<128>, kTcThreads) : launch_halo(conv_tc_halo_kernel<64>, kTcThreads);
-        if (lrc != MR_OK) return lrc;
+        void* args[] = {&tmA[0], &tmA[1], &tmA[2], const_cast<CUtensorMap*>(&tmB), &a};
+        MR_CUDA(cudaFuncSetAttribute(kern.halo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(212 * 1024)));
+        MR_CUDA(cudaLaunchKernel(kern.halo, dim3(grid), dim3(kTcThreads), args, smem, (cudaStream_t)stream));
         MR_LAUNCH_CHECK("conv_tc_halo_kernel");
         return MR_OK;
     }
     const size_t smem = (size_t)stages * stage_bytes + 1024;
     int grid = sms * ctas_per_sm;
     if (grid > a.total_tiles) grid = a.total_tiles;
-    MR_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(212 * 1024)));
-    conv_tc_kernel<<<grid, kTcThreads, smem, (cudaStream_t)stream>>>(tmA[0], tmA[1], tmA[2], tmBs[0], tmBs[1], tmBs[2], tmBs[3], a);
+    void* args[] = {&tmA[0], &tmA[1], &tmA[2], &tmBs[0], &tmBs[1], &tmBs[2], &tmBs[3], &a};
+    MR_CUDA(cudaFuncSetAttribute(kern.tap, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(212 * 1024)));
+    MR_CUDA(cudaLaunchKernel(kern.tap, dim3(grid), dim3(kTcThreads), args, smem, (cudaStream_t)stream));
     MR_LAUNCH_CHECK("conv_tc_kernel");
     return MR_OK;
 }

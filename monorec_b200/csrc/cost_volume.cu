@@ -1,4 +1,4 @@
-// Fused plane-sweep cost volume for sm_100a (B200), second generation: TMA-staged source windows.
+// Fused plane-sweep cost volume for sm_90a (H100), second generation: TMA-staged source windows.
 //
 // Replaces CostVolumeModule.forward (reference: model/monorec/monorec_model.py:150-280) together with
 // Backprojection / point_projection (model/layers.py:43-71), F.grid_sample x2, SSIM (layers.py:119-137), the
@@ -134,11 +134,15 @@ __host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_
     return L;
 }
 
-// ---- packed fp32x2 helpers (FADD2 / FMUL2 / FFMA2 on sm_100a; a pair is either two columns or two samples) ----------
+// ---- fp32 pair helpers (a pair is either two columns or two samples).  sm_90a has no packed fp32x2 arithmetic, so each
+// helper is two scalar round-to-nearest operations; the _rn intrinsics keep ptxas from contracting them, so every result is
+// rounded exactly as a packed FADD2 / FMUL2 / FFMA2 would round it. ----------------------------------------------------
 __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 __device__ __forceinline__ float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }
 
 // single MUFU.RCP (flush-to-zero variant: no denormal pre/post-scaling code; operands here are never denormal)

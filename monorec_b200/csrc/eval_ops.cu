@@ -134,8 +134,11 @@ extern "C" int mr_sparse_metrics(const float* result, const float* target, const
     MR_CUDA(cudaMemsetAsync(workspace, 0, (size_t)mr_sparse_metrics_workspace(B), st));
     const int n = (a.r1 - a.r0) * (a.c1 - a.c0);
     int blocks = (n + 256 * 8 - 1) / (256 * 8);
+    int dev = 0, sms = 0;
+    MR_CUDA(cudaGetDevice(&dev));
+    MR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));   // at most one block per SM and image
+    if (blocks > sms) blocks = sms;
     if (blocks < 1) blocks = 1;
-    if (blocks > 148) blocks = 148;
     sparse_metric_sums_kernel<<<dim3(blocks, B), 256, 0, st>>>(a);
     MR_LAUNCH_CHECK("sparse_metric_sums_kernel");
     sparse_metric_finalize_kernel<<<1, 32, 0, st>>>(a.sums, B, out_metrics);

@@ -1,4 +1,4 @@
-// Photometric reprojection loss, forward and backward, for sm_100a (SURVEY.md 8f row 4: the training-side sibling of the
+// Photometric reprojection loss, forward and backward, for sm_90a (SURVEY.md 8f row 4: the training-side sibling of the
 // cost-volume kernel -- one predicted depth per pixel instead of D planes, Gaussian-window SSIM, a gradient).
 //
 // Replaces reprojection_loss (reference: model/loss_functions/common_losses.py:16-114) for the argument sets the reference's

@@ -2,7 +2,7 @@
 
 Only tests/, __graft_entry__.smoke() and bench.py's CPU-baseline legs may import this file.
 
-Reference being restated (all from /root/reference/model):
+Reference being restated (all from the reference's model/):
   layers.py:220-252   PadSameConv2d          TF-"SAME" asymmetric zero padding
   layers.py:289-335   ConvReLU2 / ConvReLU   (k,1) conv + LReLU + (1,k) conv + LReLU   /   kxk conv + LReLU
   layers.py:338-356   Upconv                 nearest x2, pad (0,1,0,1), 2x2 conv (no activation)

@@ -4,12 +4,12 @@ Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s cpu_baseline / `--impl
 import this file, and only as the checker / the CPU baseline.  The product path (monorec_b200/) never
 imports anything from `oracle/`.
 
-Reference being restated: /root/reference/model/monorec/monorec_model.py:150-284 (CostVolumeModule.forward,
+Reference being restated: the reference's model/monorec/monorec_model.py:150-284 (CostVolumeModule.forward,
 create_mask) with model/layers.py:43-71 (Backprojection, point_projection) and :91-139 (SSIM).
 
 Parity pin: the reference has no tests or golden vectors of its own ("parity unpinned" by the reference,
-SURVEY.md §4/§8c).  This oracle is pinned instead against outputs of the *reference itself* run in the dev
-container (tests/golden/make_golden.py imports it unmodified from /root/reference and writes
+SURVEY.md §4/§8c).  This oracle is pinned instead against outputs of the *reference itself* run on the CPU
+(tests/golden/make_golden.py imports it unmodified from a checkout of the reference and writes
 tests/golden/*.npz); tests/test_oracle_golden.py checks both restatements below against those files.
 
 Two independent restatements:

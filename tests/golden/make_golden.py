@@ -1,9 +1,7 @@
 #!/usr/bin/env python
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference from /root/reference on CPU fp32.
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (a checkout of Brummi/MonoRec) on CPU fp32:
 
-Run in the dev container only (the GPU box has no /root/reference):
-
-    python tests/golden/make_golden.py
+    MONOREC_REFERENCE=<path to the MonoRec checkout> python tests/golden/make_golden.py
 
 The reference has no tests or golden vectors of its own (SURVEY.md §4), so these files are the pin for
 both the oracle (oracle/*.py) and the CUDA path.  Nothing is copied from the reference: it is imported
@@ -37,7 +35,7 @@ import torch
 
 HERE = Path(__file__).resolve().parent
 REPO = HERE.parent.parent
-REF = Path(os.environ.get("MONOREC_REFERENCE", "/root/reference"))
+REF = Path(os.environ["MONOREC_REFERENCE"])
 sys.path.insert(0, str(REPO))
 
 from monorec_b200.synthetic import make_inputs, seeded_state_dict  # noqa: E402

@@ -1,4 +1,4 @@
-"""Parity of the convolution engine / MaskModule / DepthModule / MonoRecModel (through the C ABI) on a B200."""
+"""Parity of the convolution engine / MaskModule / DepthModule / MonoRecModel (through the C ABI) on an H100."""
 import numpy as np
 import pytest
 import torch
@@ -125,11 +125,11 @@ def test_full_model_matches_reference_golden(gain_tag, gain, conv_mode):
     dm = np.abs(out["cv_mask"].cpu().numpy() - g[f"{gain_tag}_cv_mask"]).max()
     dd = [np.abs(p.cpu().numpy() - g[f"{gain_tag}_depth{i}"]).max() for i, p in enumerate(out["predicted_inverse_depths"])]
     print(conv_mode, gain_tag, "mask max|d|", dm, "depth max|d|", dd)
-    # fp32 arithmetic: gated at 1e-4, a tenth of the north-star 1e-3 (measured on B200: 6.7e-6 for g1, 3.4e-7 for g07; the
-    # reference's own fp32-vs-fp64 deviation on this configuration is 1.7e-6 / 1.8e-7, tests/golden/model_fp64.npz).
+    # fp32 arithmetic: gated at 1e-4, a tenth of the north-star 1e-3 (the reference's own fp32-vs-fp64 deviation on this
+    # configuration is 1.7e-6 / 1.8e-7, tests/golden/model_fp64.npz).
     # TF32 arithmetic (10-bit mantissa products in every dense layer) is a documented reduced-precision mode, not the parity
-    # path: the responsive weight set g07 stays below the north-star 1e-3 (measured 2.0e-4); the g1 weights amplify the
-    # product rounding (measured 4.4e-3) and are gated at 1e-2.
+    # path: the responsive weight set g07 stays below the north-star 1e-3; the g1 weights amplify the product rounding and
+    # are gated at 1e-2.
     n_res, n_mask = _ref_noise("synth", gain_tag)
     if conv_mode == "fp32":
         tol = max(1e-4, 4 * max(n_res, n_mask))
@@ -164,7 +164,7 @@ def test_modules_match_oracle_per_stage(fp32_mode):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# tensor-core path (tcgen05 kind::tf32): same layers through PackedConv in "tf32" mode
+# tensor-core path (wgmma tf32): same layers through PackedConv in "tf32" mode
 # ---------------------------------------------------------------------------------------------------------------------
 TOL_TF32 = 3e-3   # TF32 products (10-bit mantissa, fp32 accumulate) vs fp32 reference, relative to max|ref| per layer
 
@@ -311,7 +311,7 @@ def test_full_size_model_modes_and_graph_replay():
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# half-precision storage (BASELINE config 3): tcgen05 kind::f16, half NHWC activations and weights, fp32 accumulation
+# half-precision storage (BASELINE config 3): wgmma f16, half NHWC activations and weights, fp32 accumulation
 # ---------------------------------------------------------------------------------------------------------------------
 TOL_F16 = 4e-3   # half inputs/weights/outputs (10-bit mantissa each) vs fp32 reference, relative to max|ref| per layer
 
@@ -403,12 +403,11 @@ def test_full_model_on_bundled_sample(mode, gain_tag, gain):
     against the unmodified reference (tests/golden/model_kitti_sample.npz, seeded weights).
 
     fp32 arithmetic (the parity path): |delta inverse depth| < max(1e-4, 4 x the reference's own fp32-vs-fp64 deviation), i.e.
-    ten times tighter than the north-star 1e-3 for the g1 weights (measured on B200: 5.5e-6; reference noise 2.3e-6).  The g07
-    weight set is chaotic on this image -- the reference itself moves by 8.3e-3 between fp32 and fp64 (tests/golden/
-    model_fp64.npz) -- so its max-norm gate is 4 x that and the informative gate is the share of pixels within 1e-3 (measured
-    0.99924 in every mode; max|d| 4.3e-3, inside the reference's own noise).
-    tf32 / f16 are reduced-precision arithmetic modes (10-bit mantissa products): gated at 1e-2 (measured 4.2e-3 / 3.9e-3 for
-    g1) and on the pixel share within 1e-3 (measured 0.961 / 0.959); cv_mask at 2e-2 (measured 7.6e-3 / 1.08e-2)."""
+    ten times tighter than the north-star 1e-3 for the g1 weights (reference noise 2.3e-6).  The g07 weight set is chaotic on
+    this image -- the reference itself moves by 8.3e-3 between fp32 and fp64 (tests/golden/model_fp64.npz) -- so its max-norm
+    gate is 4 x that and the informative gate is the share of pixels within 1e-3.
+    tf32 / f16 are reduced-precision arithmetic modes (10-bit mantissa products): gated at 1e-2 and on the pixel share within
+    1e-3; cv_mask at 2e-2."""
     from monorec_b200 import conv as K
     from monorec_b200.model import MonoRecModel
     from monorec_b200.synthetic import seeded_state_dict, to_device

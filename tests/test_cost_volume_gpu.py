@@ -1,4 +1,4 @@
-"""Parity of the fused sm_100a cost-volume kernel (through the C ABI) with the reference / oracle.  Needs a B200."""
+"""Parity of the fused sm_90a cost-volume kernel (through the C ABI) with the reference / oracle.  Needs an H100."""
 import numpy as np
 import pytest
 import torch

@@ -1,5 +1,5 @@
 """Informative same-box baseline: the oracle restatements (stock torch ops: grid_sample, avg_pool2d, conv3d, cuDNN convs)
-run on the B200 through PyTorch-CUDA, next to this repo's kernels.  Test/bench infrastructure only."""
+run on the GPU through PyTorch-CUDA, next to this repo's kernels.  Test/bench infrastructure only."""
 import sys
 from pathlib import Path
 
