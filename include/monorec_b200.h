@@ -160,8 +160,9 @@ int mr_conv2d_nhwc(const mr_conv_desc* desc, void* stream);
  * a multiple of 64) or, if the caller packed every source to a multiple of 32 instead and that gives a different k_pad,
  * 32 channels (64-byte swizzle rows); the MMA is f16; dst_dtype selects half or float output.
  * Stride-1 layers whose packed weights fit in shared memory twice per SM run on the "halo" variant of the kernel (same
- * results).  Tuning switches (environment, read once): MONOREC_B200_TC_HALO=0|1|2, MONOREC_B200_TC_HALO_F16=0|1,
- * MONOREC_B200_TC_CTAS=n. */
+ * results); larger weights stream through it, and everything else runs on the tap-refetch kernel (mr_conv2d_nhwc_tc_plan
+ * tells which).  Tuning switches (environment, read once): MONOREC_B200_TC_HALO=0|1..4, MONOREC_B200_TC_STREAM=0|1,
+ * MONOREC_B200_TC_HALO_F16=0|1, MONOREC_B200_TC_CTAS=n. */
 int mr_conv2d_nhwc_tc(const mr_conv_desc* desc, int n_pad, int k_pad, int round_out, void* stream);
 /* The sub-pixel convolutions of one layer -- Refine's ConvTranspose2d(k4,s2)+crop = four 2x2 filters (model/layers.py:380-400),
  * Upconv's nearest-x2 + pad + 2x2 conv = 1x1 / 1x2 / 2x1 / 2x2 filters (:338-356) -- in ONE launch: descs[0..n_phases) share the
@@ -169,6 +170,29 @@ int mr_conv2d_nhwc_tc(const mr_conv_desc* desc, int n_pad, int k_pad, int round_
  * (anything else: MR_EINVAL).  Tiles are ordered (spatial tile, phase), so the phases of a tile run side by side and the input is
  * read from HBM once instead of once per phase.  n_phases = 1 is mr_conv2d_nhwc_tc. */
 int mr_conv2d_nhwc_tc_phases(const mr_conv_desc* descs, int n_phases, int n_pad, int k_pad, int round_out, void* stream);
+/* The kernel mr_conv2d_nhwc_tc_phases(descs, n_phases, n_pad, k_pad, ...) launches for these arguments, and the inputs of that
+ * choice.  The descriptors are validated as for a launch; nothing is launched and no tensor is touched (fake pointers are fine).
+ * The launch path runs exactly this plan.  Needs a current CUDA device (register occupancy, SM count). */
+#define MR_TC_KERNEL_TAP 0           /* tap-refetch kernel: one input box and one weight slice per (tap, K chunk) */
+#define MR_TC_KERNEL_HALO 1          /* halo kernel, the layer's weights resident in shared memory */
+#define MR_TC_KERNEL_HALO_STREAM 2   /* halo kernel, the weights streamed through a ring of b_stream stages */
+typedef struct mr_tc_plan {
+    int kernel;                      /* MR_TC_KERNEL_* */
+    int n_pad;                       /* MMA N */
+    int kc;                          /* channels per K chunk */
+    int row_bytes;                   /* bytes of one K chunk row in shared memory (swizzle span): 128, or 64 */
+    int ctas_per_sm;
+    int stages;                      /* pipeline stages: input box + weight slice (tap) / input box (halo) */
+    int b_stream;                    /* weight ring stages of MR_TC_KERNEL_HALO_STREAM, else 0 */
+    int grid;                        /* CTAs launched; each loops over tiles grid apart */
+    int total_tiles;                 /* output tiles x batch x phases */
+    int tiles_x;                     /* output tiles per row (8 px wide on the halo kernel, 16 on the tap kernel) */
+    int smem_bytes;                  /* dynamic shared memory per CTA */
+    int halo_pitch;                  /* halo kernel: pixels per row of the input box, else 0 */
+    int tap_reg_ctas, halo_reg_ctas; /* CTAs per SM the registers of the two kernels for this n_pad allow */
+    int halo_shape;                  /* 1: one phase, stride 1, kh <= 7, kw <= 9 and the tuning switches admit the halo kernel */
+} mr_tc_plan;
+int mr_conv2d_nhwc_tc_plan(const mr_conv_desc* descs, int n_phases, int n_pad, int k_pad, mr_tc_plan* out);
 /* Host-side weight packing for mr_conv2d_nhwc_tc (pure host code, callable without a GPU).
  *   mr_pack_conv_weights_bytes: size of the packed tensor and its n_pad / k_pad for a correlation kernel (Cout, sum src_c, kh, kw)
  *     whose input channels are the concatenation of n_src sources; dtype MR_DT_F32 (TF32-rounded fp32) or MR_DT_F16.

@@ -61,6 +61,21 @@ class ConvDesc(ctypes.Structure):
                 ("act", c_int), ("act_a", c_float), ("act_b", c_float), ("src_dtype", c_int), ("dst_dtype", c_int)]
 
 
+TC_KERNEL_TAP, TC_KERNEL_HALO, TC_KERNEL_HALO_STREAM = 0, 1, 2
+TC_KERNEL_NAMES = {TC_KERNEL_TAP: "tap", TC_KERNEL_HALO: "halo", TC_KERNEL_HALO_STREAM: "halo-stream"}
+
+
+class TcPlan(ctypes.Structure):
+    """Mirror of `struct mr_tc_plan` (include/monorec_b200.h): the kernel a tensor-core launch runs and why."""
+    _fields_ = [("kernel", c_int), ("n_pad", c_int), ("kc", c_int), ("row_bytes", c_int), ("ctas_per_sm", c_int),
+                ("stages", c_int), ("b_stream", c_int), ("grid", c_int), ("total_tiles", c_int), ("tiles_x", c_int),
+                ("smem_bytes", c_int), ("halo_pitch", c_int), ("tap_reg_ctas", c_int), ("halo_reg_ctas", c_int),
+                ("halo_shape", c_int)]
+
+    def as_dict(self):
+        return {name: getattr(self, name) for name, _ in self._fields_}
+
+
 def same_pad_before(n, k, s):
     """Leading zero padding of PadSameConv2d (model/layers.py:249-251); the trailing part is implicit (zero fill)."""
     total = s * (math.ceil(n / s) - 1) + k - n
@@ -344,21 +359,51 @@ def conv2d_tc(srcs, L, out=None, out_hw=None, round_out=True, half=False, out_f3
     """Tensor-core launch (csrc/conv_tc.cu) of a PackedConv."""
     lib = _lib.load()
     x0 = srcs[0]
-    B, Hs, Ws, _ = x0.shape
-    sy, sx = L.stride
-    pad = L.pad if L.pad is not None else (same_pad_before(Hs, L.kh, sy), same_pad_before(Ws, L.kw, sx))
-    if out_hw is None:
-        out_hw = (math.ceil(Hs / sy), math.ceil(Ws / sx))
-    Ho, Wo = out_hw
+    B = x0.shape[0]
+    Ho, Wo = _tc_out_hw(srcs, L, out_hw)
     if out is None:
         out = torch.empty(B, Ho * L.out_step[0], Wo * L.out_step[1], L.cout, device=x0.device,
                           dtype=torch.float16 if (half and not out_f32) else torch.float32)
     wtc, n_pad, k_pad = L.wtc(half)
     d = ConvDesc()
-    _fill_desc(d, srcs, L, out, (Ho, Wo), pad, wtc, half, out_coff)
+    _fill_desc(d, srcs, L, out, (Ho, Wo), _tc_pad(srcs, L), wtc, half, out_coff)
     with torch.cuda.device(x0.device):
         _lib.check(lib.mr_conv2d_nhwc_tc(ctypes.byref(d), n_pad, k_pad, int(round_out), _stream(x0)), "mr_conv2d_nhwc_tc")
     return out
+
+
+def _tc_out_hw(srcs, L, out_hw):
+    if out_hw is not None:
+        return tuple(out_hw)
+    Hs, Ws = srcs[0].shape[1:3]
+    return math.ceil(Hs / L.stride[0]), math.ceil(Ws / L.stride[1])
+
+
+def _tc_pad(srcs, L):
+    if L.pad is not None:
+        return L.pad
+    Hs, Ws = srcs[0].shape[1:3]
+    return same_pad_before(Hs, L.kh, L.stride[0]), same_pad_before(Ws, L.kw, L.stride[1])
+
+
+def tc_plan(srcs, subs, out, out_hw=None, half=False, out_coff=0):
+    """The kernel choice (include/monorec_b200.h: mr_conv2d_nhwc_tc_plan) of conv2d_tc(srcs, subs[0], out, ...) or, for several
+    PackedConv, conv2d_tc_phases(srcs, subs, out, ...) with the same arguments; a dict of the mr_tc_plan fields.  Launches
+    nothing."""
+    lib = _lib.load()
+    out_hw = _tc_out_hw(srcs, subs[0], out_hw)
+    descs = (ConvDesc * len(subs))()
+    n_pad = k_pad = None
+    for d, L in zip(descs, subs):
+        wtc, n_pad_i, k_pad_i = L.wtc(half)
+        assert n_pad in (None, n_pad_i) and k_pad in (None, k_pad_i)
+        n_pad, k_pad = n_pad_i, k_pad_i
+        _fill_desc(d, srcs, L, out, out_hw, _tc_pad(srcs, L), wtc, half, out_coff)
+        d.bias = subs[0].bias.data_ptr() if subs[0].bias is not None else None
+    plan = TcPlan()
+    with torch.cuda.device(srcs[0].device):
+        _lib.check(lib.mr_conv2d_nhwc_tc_plan(descs, len(subs), n_pad, k_pad, ctypes.byref(plan)), "mr_conv2d_nhwc_tc_plan")
+    return plan.as_dict()
 
 
 def _fill_desc(d, srcs, L, out, out_hw, pad, wtc, half, out_coff=0):

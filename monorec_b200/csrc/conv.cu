@@ -304,6 +304,7 @@ extern "C" int mr_conv2d_nhwc(const mr_conv_desc* desc, void* stream) {
     MR_REQUIRE(d.kh >= 1 && d.kw >= 1 && d.sy >= 1 && d.sx >= 1 && d.oy_step >= 1 && d.ox_step >= 1,
                "mr_conv2d_nhwc: bad kernel/stride");
     MR_REQUIRE(d.dst_coff >= 0 && d.dst_coff + d.Cout <= d.dst_c, "mr_conv2d_nhwc: channel slice out of range");
+    MR_REQUIRE(d.oy_off >= 0 && d.ox_off >= 0, "mr_conv2d_nhwc: oy_off=%d / ox_off=%d must be >= 0", d.oy_off, d.ox_off);
     MR_REQUIRE((d.Ho - 1) * d.oy_step + d.oy_off < d.dst_H && (d.Wo - 1) * d.ox_step + d.ox_off < d.dst_W,
                "mr_conv2d_nhwc: output placement out of range");
     MR_REQUIRE(d.act >= MR_ACT_NONE && d.act <= MR_ACT_ABSTANH, "mr_conv2d_nhwc: unknown activation %d", d.act);

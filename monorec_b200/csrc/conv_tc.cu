@@ -695,12 +695,16 @@ int resident_ctas(const void* kernel) {
     return n > 0 ? n : 1;
 }
 
-}  // namespace
+// bytes of one input stage of the halo kernel: a box of (16 + kh - 1) rows x pitch pixels of one K chunk, rounded up to 1 KB
+size_t halo_box_bytes(int kh, int pitch, int row_bytes) { return ((size_t)(16 + kh - 1) * pitch * row_bytes + 1023) & ~size_t(1023); }
 
-static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad, int k_pad, int round_out, void* stream) {
+// Every argument check of mr_conv2d_nhwc_tc / _phases / _plan.  Makes no CUDA call, so a bad descriptor is rejected the same
+// way with or without a GPU.  *kc_out: channels per K chunk (32 or 64), derived from k_pad.
+int tc_validate(const mr_conv_desc* desc, int n_phases, int n_pad, int k_pad, int* kc_out) {
     MR_REQUIRE(desc != nullptr, "mr_conv2d_nhwc_tc: null descriptor");
     MR_REQUIRE(n_phases >= 1 && n_phases <= 4, "mr_conv2d_nhwc_tc_phases: 1..4 phases (got %d)", n_phases);
     const mr_conv_desc& d = desc[0];
+    MR_REQUIRE(d.n_src >= 1 && d.n_src <= MR_CONV_MAX_SRC, "mr_conv2d_nhwc_tc: n_src=%d out of range", d.n_src);
     for (int p = 1; p < n_phases; ++p) {   // phases share everything but the filter (size, padding, weights) and the output offset
         const mr_conv_desc& e = desc[p];
         bool same = e.n_src == d.n_src && e.B == d.B && e.Hs == d.Hs && e.Ws == d.Ws && e.upsample2 == d.upsample2 && e.sy == d.sy &&
@@ -710,30 +714,35 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
                     e.src_dtype == d.src_dtype && e.dst_dtype == d.dst_dtype;
         for (int s = 0; same && s < d.n_src; ++s) same = e.src[s] == d.src[s] && e.src_c[s] == d.src_c[s];
         MR_REQUIRE(same, "mr_conv2d_nhwc_tc_phases: phase %d differs from phase 0 in more than filter size, padding, weights and output offset", p);
-        MR_REQUIRE(e.weight && e.kh >= 1 && e.kw >= 1 && (e.Ho - 1) * e.oy_step + e.oy_off < e.dst_H && (e.Wo - 1) * e.ox_step + e.ox_off < e.dst_W,
-                   "mr_conv2d_nhwc_tc_phases: phase %d: bad filter / output placement", p);
-        MR_REQUIRE((reinterpret_cast<uintptr_t>(e.weight) & 15) == 0, "mr_conv2d_nhwc_tc_phases: weights are not 16-byte aligned");
     }
-    MR_REQUIRE(d.n_src >= 1 && d.n_src <= MR_CONV_MAX_SRC, "mr_conv2d_nhwc_tc: n_src=%d out of range", d.n_src);
-    MR_REQUIRE(d.upsample2 == 0, "mr_conv2d_nhwc_tc: upsample-on-read is expressed as sub-pixel convolutions on this path");
-    MR_REQUIRE(d.weight && d.dst, "mr_conv2d_nhwc_tc: null weight/dst");
+    MR_REQUIRE(d.upsample2 == 0, "mr_conv2d_nhwc_tc: upsample2: upsample-on-read is expressed as sub-pixel convolutions on this path");
+    MR_REQUIRE(d.dst != nullptr, "mr_conv2d_nhwc_tc: null dst");
+    MR_REQUIRE(d.src_dtype == MR_DT_F32 || d.src_dtype == MR_DT_F16, "mr_conv2d_nhwc_tc: bad src_dtype %d", d.src_dtype);
+    MR_REQUIRE(d.dst_dtype == MR_DT_F32 || d.dst_dtype == MR_DT_F16, "mr_conv2d_nhwc_tc: bad dst_dtype %d", d.dst_dtype);
     MR_REQUIRE(d.Cout >= 1 && d.Cout <= 256 && n_pad >= d.Cout && n_pad <= 256 && (n_pad % 16) == 0,
                "mr_conv2d_nhwc_tc: Cout=%d n_pad=%d unsupported (Cout <= 256, n_pad multiple of 16)", d.Cout, n_pad);
     MR_REQUIRE(d.B >= 1 && d.B <= 65535 && d.Hs >= 1 && d.Ws >= 1 && d.Ho >= 1 && d.Wo >= 1, "mr_conv2d_nhwc_tc: bad shape");
-    MR_REQUIRE(d.kh >= 1 && d.kw >= 1 && d.sy >= 1 && d.sx >= 1 && d.sy <= 4 && d.sx <= 4, "mr_conv2d_nhwc_tc: bad kernel/stride");
-    MR_REQUIRE(d.dst_coff >= 0 && d.dst_coff + d.Cout <= d.dst_c, "mr_conv2d_nhwc_tc: channel slice out of range");
-    MR_REQUIRE((d.Ho - 1) * d.oy_step + d.oy_off < d.dst_H && (d.Wo - 1) * d.ox_step + d.ox_off < d.dst_W,
-               "mr_conv2d_nhwc_tc: output placement out of range");
-    EncodeTiledFn encode = get_encode_fn();
-    if (encode == nullptr) {
-        mr::set_error("mr_conv2d_nhwc_tc: cuTensorMapEncodeTiled is not available from this driver");
-        return MR_ENOSUPPORT;
+    MR_REQUIRE(d.sy >= 1 && d.sx >= 1 && d.sy <= 4 && d.sx <= 4, "mr_conv2d_nhwc_tc: stride sy=%d sx=%d out of 1..4", d.sy, d.sx);
+    MR_REQUIRE(d.oy_step >= 1 && d.ox_step >= 1, "mr_conv2d_nhwc_tc: oy_step=%d / ox_step=%d must be >= 1", d.oy_step, d.ox_step);
+    MR_REQUIRE(d.act >= MR_ACT_NONE && d.act <= MR_ACT_ABSTANH, "mr_conv2d_nhwc_tc: unknown act %d", d.act);
+    MR_REQUIRE(d.dst_coff >= 0 && d.dst_coff + d.Cout <= d.dst_c, "mr_conv2d_nhwc_tc: channel slice dst_coff=%d + Cout=%d out of dst_c=%d",
+               d.dst_coff, d.Cout, d.dst_c);
+    for (int p = 0; p < n_phases; ++p) {
+        const mr_conv_desc& e = desc[p];
+        MR_REQUIRE(e.weight != nullptr && (reinterpret_cast<uintptr_t>(e.weight) & 15) == 0,
+                   "mr_conv2d_nhwc_tc: phase %d: weight is null or not 16-byte aligned", p);
+        MR_REQUIRE(e.kh >= 1 && e.kw >= 1, "mr_conv2d_nhwc_tc: phase %d: bad filter size kh=%d kw=%d", p, e.kh, e.kw);
+        MR_REQUIRE(e.oy_off >= 0 && e.ox_off >= 0, "mr_conv2d_nhwc_tc: phase %d: oy_off=%d / ox_off=%d must be >= 0", p, e.oy_off, e.ox_off);
+        MR_REQUIRE((e.Ho - 1) * e.oy_step + e.oy_off < e.dst_H && (e.Wo - 1) * e.ox_step + e.ox_off < e.dst_W,
+                   "mr_conv2d_nhwc_tc: phase %d: output placement out of range (dst_H=%d dst_W=%d)", p, e.dst_H, e.dst_W);
     }
-    TcArgs a{};
-    a.n_src = d.n_src;
-    MR_REQUIRE(d.src_dtype == MR_DT_F32 || d.src_dtype == MR_DT_F16, "mr_conv2d_nhwc_tc: bad src_dtype %d", d.src_dtype);
-    MR_REQUIRE(d.dst_dtype == MR_DT_F32 || d.dst_dtype == MR_DT_F16, "mr_conv2d_nhwc_tc: bad dst_dtype %d", d.dst_dtype);
     const bool f16 = d.src_dtype == MR_DT_F16;
+    const int cmult = f16 ? 8 : 4;            // pixel stride must be a multiple of 16 bytes for TMA
+    for (int s = 0; s < d.n_src; ++s) {
+        MR_REQUIRE(d.src[s] != nullptr && d.src_c[s] >= cmult && (d.src_c[s] % cmult) == 0,
+                   "mr_conv2d_nhwc_tc: source %d needs src_c a multiple of %d (got %d)", s, cmult, d.src_c[s]);
+        MR_REQUIRE((reinterpret_cast<uintptr_t>(d.src[s]) & 15) == 0, "mr_conv2d_nhwc_tc: source %d is not 16-byte aligned", s);
+    }
     // K chunk = one swizzle row of channels: 32 fp32 or 64 half (128 bytes).  Half sources whose channel counts waste less
     // with 32-channel chunks (32, 96, ... channels) are packed that way by the caller (k_pad tells): 64-byte rows, SWIZZLE_64B,
     // so that neither TMA nor the MMA spends time on the zero half of a 128-byte row.
@@ -743,16 +752,24 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
         for (int s = 0; s < d.n_src; ++s) { k64 += (d.src_c[s] + 63) / 64 * 64; k32 += (d.src_c[s] + 31) / 32 * 32; }
         if (k_pad != k64 && k_pad == k32) kc = 32;
     }
-    const int esize = f16 ? 2 : 4;
-    const int cmult = f16 ? 8 : 4;            // pixel stride must be a multiple of 16 bytes for TMA
-    a.row_bytes = kc * (f16 ? 2 : 4);
-    a.kc = kc; a.out_f16 = (d.dst_dtype == MR_DT_F16) ? 1 : 0;
-    const TcKernels kern = tc_kernels(n_pad, f16);
     int ksum = 0;
+    for (int s = 0; s < d.n_src; ++s) ksum += (d.src_c[s] + kc - 1) / kc * kc;
+    MR_REQUIRE(ksum == k_pad, "mr_conv2d_nhwc_tc: packed weight k_pad (%d) does not match the sources (%d)", k_pad, ksum);
+    *kc_out = kc;
+    return MR_OK;
+}
+
+// The kernel choice for a validated descriptor: tap-refetch or halo kernel, resident or streamed weights, CTAs per SM,
+// stages, grid.  The launch below runs exactly this plan; mr_conv2d_nhwc_tc_plan reports it.
+int tc_plan(const mr_conv_desc* desc, int n_phases, int n_pad, int kc, mr_tc_plan* out) {
+    const mr_conv_desc& d = desc[0];
+    const bool f16 = d.src_dtype == MR_DT_F16;
+    const int row_bytes = kc * (f16 ? 2 : 4);
+    const TcKernels kern = tc_kernels(n_pad, f16);
     // "halo" variant (one input box per tile, resident weights): stride 1, taps reach at most 8 px to the right, weights fit
     int chunks_all = 0;
     for (int s = 0; s < d.n_src; ++s) chunks_all += (d.src_c[s] + kc - 1) / kc;
-    const size_t bres = (size_t)d.kh * d.kw * chunks_all * n_pad * a.row_bytes;
+    const size_t bres = (size_t)d.kh * d.kw * chunks_all * n_pad * row_bytes;
     // MONOREC_B200_TC_HALO: unset = automatic, 0 = never, n = 1..4: at most n CTAs per SM (1: also layers that only fit once).
     // Box rows are 8 + kw - 1 px, so a box holds exactly the pixels the taps touch and the 48-channel full-resolution layers
     // fit twice per SM next to their weights.
@@ -762,7 +779,7 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     // MONOREC_B200_TC_HALO_PITCH=16: fixed 16-px box rows (A/B measurements)
     static const int pitch_env = getenv("MONOREC_B200_TC_HALO_PITCH") ? atoi(getenv("MONOREC_B200_TC_HALO_PITCH")) : 0;
     const int halo_pitch = (pitch_env >= 8 + d.kw - 1) ? pitch_env : 8 + d.kw - 1;
-    const size_t halo_a_bytes = ((size_t)(16 + d.kh - 1) * halo_pitch * a.row_bytes + 1023) & ~size_t(1023);
+    const size_t halo_a_bytes = halo_box_bytes(d.kh, halo_pitch, row_bytes);
     const size_t bres_al = (bres + 1023) & ~size_t(1023);
     // CTAs per SM the accumulator registers allow (the wider N, the more registers per consumer thread)
     const int halo_reg_ctas = resident_ctas(kern.halo);
@@ -775,8 +792,9 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     };
     // CTAs per SM: up to three, each with at least two input stages (up to 4).
     // MONOREC_B200_TC_HALO=n (1..4) caps / forces the count for measurements (1: also layers that only fit once).
+    const bool halo_shape = n_phases == 1 && halo_env != 0 && (!f16 || halo_f16) && d.sy == 1 && d.sx == 1 && d.kw <= 9 && d.kh <= 7;
     int halo_ctas = 0;
-    if (n_phases == 1 && halo_env != 0 && (!f16 || halo_f16) && d.sy == 1 && d.sx == 1 && d.kw <= 9 && d.kh <= 7) {
+    if (halo_shape) {
         const int cap = (halo_env >= 1 && halo_env <= 4) ? halo_env : 3;
         for (int c = cap; c >= (halo_env == 1 ? 1 : 2) && halo_ctas == 0; --c)
             if (halo_fit(c) >= 2) halo_ctas = c;
@@ -787,9 +805,8 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     // multi-source decoder layers.  MONOREC_B200_TC_STREAM=0 disables it (A/B).
     static const bool stream_on = getenv("MONOREC_B200_TC_STREAM") ? (atoi(getenv("MONOREC_B200_TC_STREAM")) != 0) : true;
     int b_stream = 0, stream_stages = 0;
-    const size_t b_slice = (size_t)n_pad * a.row_bytes;
-    if (halo_ctas == 0 && stream_on && n_phases == 1 && halo_env != 0 && (!f16 || halo_f16) && d.sy == 1 && d.sx == 1 && d.kw <= 9 &&
-        d.kh <= 7 && d.kh * d.kw > 1 && halo_reg_ctas >= 2) {
+    const size_t b_slice = (size_t)n_pad * row_bytes;
+    if (halo_ctas == 0 && stream_on && halo_shape && d.kh * d.kw > 1 && halo_reg_ctas >= 2) {
         const size_t budget = (size_t)228 * 1024 / 2 - (1 + 1 + 1) * 1024 - 512 - 1024;
         if (budget > 2 * halo_a_bytes + 3 * b_slice) {
             int nb = (int)((budget - 2 * halo_a_bytes) / b_slice);
@@ -801,22 +818,88 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
         }
     }
     const bool halo = halo_ctas > 0;
-    const int halo_stages = b_stream ? stream_stages : (halo ? halo_fit(halo_ctas) : 0);
-    const size_t halo_front = b_stream ? (size_t)b_stream * b_slice : bres_al;   // bytes in front of the input stages
+    const int tiles_x = halo ? (d.Wo + 7) / 8 : (d.Wo + kTileW - 1) / kTileW;
+    const int tiles = tiles_x * (halo ? (d.Ho + 15) / 16 : (d.Ho + kTileH - 1) / kTileH);
+    const int total_tiles = tiles * d.B * n_phases;
+    // persistent grid over the SMs of the current device
+    int dev = 0, sms = 0;
+    MR_CUDA(cudaGetDevice(&dev));
+    MR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    static const int kForceCtas = getenv("MONOREC_B200_TC_CTAS") ? atoi(getenv("MONOREC_B200_TC_CTAS")) : 0;   // tuning knob
+    // resident CTAs per SM: bounded by the accumulator registers and capped at 4; with MMA N = 32..64 one CTA cannot keep the
+    // tensor pipe busy, so several CTAs interleave their MMA chains
+    const int reg_ctas = resident_ctas(kern.tap);
+    mr_tc_plan p{};
+    p.n_pad = n_pad; p.kc = kc; p.row_bytes = row_bytes;
+    p.total_tiles = total_tiles; p.tiles_x = tiles_x;
+    p.tap_reg_ctas = reg_ctas; p.halo_reg_ctas = halo_reg_ctas; p.halo_shape = halo_shape ? 1 : 0;
+    if (halo) {
+        p.kernel = b_stream ? MR_TC_KERNEL_HALO_STREAM : MR_TC_KERNEL_HALO;
+        p.ctas_per_sm = halo_ctas;
+        p.stages = b_stream ? stream_stages : halo_fit(halo_ctas);
+        p.b_stream = b_stream;
+        p.halo_pitch = halo_pitch;
+        const size_t halo_front = b_stream ? (size_t)b_stream * b_slice : bres_al;   // bytes in front of the input stages
+        p.smem_bytes = (int)(halo_front + (size_t)p.stages * halo_a_bytes + 1024);
+    } else {
+        int ctas_per_sm = reg_ctas > 4 ? 4 : reg_ctas;
+        if (kForceCtas > 0 && kForceCtas <= reg_ctas) ctas_per_sm = kForceCtas;
+        const size_t stage_bytes = (size_t)(128 + n_pad) * row_bytes;
+        const size_t budget = (size_t)(200 * 1024) / ctas_per_sm - 2 * 1024;
+        int stages = (int)(budget / stage_bytes);
+        if (stages > 8) stages = 8;
+        if (stages < 2) stages = 2;
+        p.kernel = MR_TC_KERNEL_TAP;
+        p.ctas_per_sm = ctas_per_sm;
+        p.stages = stages;
+        p.smem_bytes = (int)((size_t)stages * stage_bytes + 1024);
+    }
+    p.grid = sms * p.ctas_per_sm;
+    if (p.grid > total_tiles) p.grid = total_tiles;
+    *out = p;
+    return MR_OK;
+}
+
+}  // namespace
+
+extern "C" int mr_conv2d_nhwc_tc_plan(const mr_conv_desc* descs, int n_phases, int n_pad, int k_pad, mr_tc_plan* out) {
+    MR_REQUIRE(out != nullptr, "mr_conv2d_nhwc_tc_plan: null out");
+    int kc = 0;
+    const int rc = tc_validate(descs, n_phases, n_pad, k_pad, &kc);
+    if (rc != MR_OK) return rc;
+    return tc_plan(descs, n_phases, n_pad, kc, out);
+}
+
+static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad, int k_pad, int round_out, void* stream) {
+    int kc = 0;
+    int rc = tc_validate(desc, n_phases, n_pad, k_pad, &kc);
+    if (rc != MR_OK) return rc;
+    EncodeTiledFn encode = get_encode_fn();
+    if (encode == nullptr) {
+        mr::set_error("mr_conv2d_nhwc_tc: cuTensorMapEncodeTiled is not available from this driver");
+        return MR_ENOSUPPORT;
+    }
+    mr_tc_plan plan;
+    rc = tc_plan(desc, n_phases, n_pad, kc, &plan);
+    if (rc != MR_OK) return rc;
+    const mr_conv_desc& d = desc[0];
+    const bool f16 = d.src_dtype == MR_DT_F16;
+    const bool halo = plan.kernel != MR_TC_KERNEL_TAP;
+    const int esize = f16 ? 2 : 4;
+    TcArgs a{};
+    a.n_src = d.n_src;
+    a.row_bytes = plan.row_bytes;
+    a.kc = kc; a.out_f16 = (d.dst_dtype == MR_DT_F16) ? 1 : 0;
     CUtensorMap tmA[MR_CONV_MAX_SRC];
     for (int s = 0; s < d.n_src; ++s) {
         const int C = d.src_c[s];
-        MR_REQUIRE(d.src[s] != nullptr && C >= cmult && (C % cmult) == 0,
-                   "mr_conv2d_nhwc_tc: source %d needs a channel count that is a multiple of %d (got %d)", s, cmult, C);
-        MR_REQUIRE((reinterpret_cast<uintptr_t>(d.src[s]) & 15) == 0, "mr_conv2d_nhwc_tc: source %d is not 16-byte aligned", s);
         a.chunks[s] = (C + kc - 1) / kc;
         a.tail_ksteps[s] = ((C - (a.chunks[s] - 1) * kc) * esize + 31) / 32;
-        ksum += a.chunks[s] * kc;
         const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)d.Ws, (cuuint64_t)d.Hs, (cuuint64_t)d.B};
         const cuuint64_t gstr[3] = {(cuuint64_t)C * esize, (cuuint64_t)d.Ws * C * esize, (cuuint64_t)d.Hs * d.Ws * C * esize};
         // with a traversal stride s the box spans box/s loaded elements: 16 (8) output pixels need a span of 16*s (8*s)
         cuuint32_t box[4] = {(cuuint32_t)kc, (cuuint32_t)(kTileW * d.sx), (cuuint32_t)(kTileH * d.sy), 1};
-        if (halo) { box[1] = (cuuint32_t)halo_pitch; box[2] = (cuuint32_t)(16 + d.kh - 1); }
+        if (halo) { box[1] = (cuuint32_t)plan.halo_pitch; box[2] = (cuuint32_t)(16 + d.kh - 1); }
         const cuuint32_t estr[4] = {1, (cuuint32_t)d.sx, (cuuint32_t)d.sy, 1};
         CUresult r = encode(&tmA[s], f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(d.src[s]), gdim, gstr, box, estr,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, a.row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
@@ -827,8 +910,6 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
         }
     }
     for (int s = d.n_src; s < MR_CONV_MAX_SRC; ++s) tmA[s] = tmA[0];
-    MR_REQUIRE(ksum == k_pad, "mr_conv2d_nhwc_tc: packed weight K (%d) does not match the sources (%d)", k_pad, ksum);
-    MR_REQUIRE((reinterpret_cast<uintptr_t>(d.weight) & 15) == 0, "mr_conv2d_nhwc_tc: weights are not 16-byte aligned");
     CUtensorMap tmBs[4];
     for (int p = 0; p < n_phases; ++p) {
         const mr_conv_desc& e = desc[p];
@@ -845,7 +926,6 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
         }
     }
     for (int p = n_phases; p < 4; ++p) tmBs[p] = tmBs[0];
-    const CUtensorMap& tmB = tmBs[0];
     a.n_phase = n_phases;
     for (int p = 0; p < 4; ++p) {
         const mr_conv_desc& e = desc[p < n_phases ? p : 0];
@@ -853,50 +933,28 @@ static int conv2d_nhwc_tc_impl(const mr_conv_desc* desc, int n_phases, int n_pad
     }
     a.kh = d.kh; a.kw = d.kw; a.sy = d.sy; a.sx = d.sx; a.pad_t = d.pad_t; a.pad_l = d.pad_l;
     a.Ho = d.Ho; a.Wo = d.Wo; a.Cout = d.Cout; a.n_pad = n_pad;
-    a.tiles_x = halo ? (d.Wo + 7) / 8 : (d.Wo + kTileW - 1) / kTileW;
-    const int tiles = a.tiles_x * (halo ? (d.Ho + 15) / 16 : (d.Ho + kTileH - 1) / kTileH);
-    const size_t stage_bytes = (size_t)(128 + n_pad) * a.row_bytes;
-    a.tiles_per_img = tiles;
-    a.total_tiles = tiles * d.B * n_phases;
-    // persistent grid over the SMs of the current device
-    int dev = 0, sms = 0;
-    MR_CUDA(cudaGetDevice(&dev));
-    MR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    static const int kForceCtas = getenv("MONOREC_B200_TC_CTAS") ? atoi(getenv("MONOREC_B200_TC_CTAS")) : 0;   // tuning knob
-    // resident CTAs per SM: bounded by the accumulator registers and capped at 4; with MMA N = 32..64 one CTA cannot keep the
-    // tensor pipe busy, so several CTAs interleave their MMA chains
-    const int reg_ctas = resident_ctas(kern.tap);
-    int ctas_per_sm = reg_ctas > 4 ? 4 : reg_ctas;
-    if (kForceCtas > 0 && kForceCtas <= reg_ctas) ctas_per_sm = kForceCtas;
-    const size_t budget = (size_t)(200 * 1024) / ctas_per_sm - 2 * 1024;
-    int stages = (int)(budget / stage_bytes);
-    if (stages > 8) stages = 8;
-    if (stages < 2) stages = 2;
-    a.stages = stages;
+    a.tiles_x = plan.tiles_x;
+    a.tiles_per_img = plan.total_tiles / (d.B * n_phases);
+    a.total_tiles = plan.total_tiles;
+    a.stages = plan.stages;
     a.bias = d.bias; a.dst = d.dst;
     a.dst_H = d.dst_H; a.dst_W = d.dst_W; a.dst_c = d.dst_c; a.dst_coff = d.dst_coff;
     a.oy_step = d.oy_step; a.ox_step = d.ox_step; a.oy_off = d.oy_off; a.ox_off = d.ox_off;
     a.act = d.act; a.act_a = d.act_a; a.act_b = d.act_b; a.round_out = round_out;
+    const TcKernels kern = tc_kernels(n_pad, f16);
     if (halo) {
-        a.stages = halo_stages;
-        a.halo_pitch = halo_pitch;
-        a.halo_a_bytes = (uint32_t)halo_a_bytes;
-        a.b_stream = b_stream;
-        const size_t smem = halo_front + (size_t)halo_stages * halo_a_bytes + 1024;
-        int grid = sms * halo_ctas;
-        if (grid > a.total_tiles) grid = a.total_tiles;
-        void* args[] = {&tmA[0], &tmA[1], &tmA[2], const_cast<CUtensorMap*>(&tmB), &a};
+        a.halo_pitch = plan.halo_pitch;
+        a.halo_a_bytes = (uint32_t)halo_box_bytes(d.kh, plan.halo_pitch, plan.row_bytes);
+        a.b_stream = plan.b_stream;
+        void* args[] = {&tmA[0], &tmA[1], &tmA[2], &tmBs[0], &a};
         MR_CUDA(cudaFuncSetAttribute(kern.halo, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(212 * 1024)));
-        MR_CUDA(cudaLaunchKernel(kern.halo, dim3(grid), dim3(kTcThreads), args, smem, (cudaStream_t)stream));
+        MR_CUDA(cudaLaunchKernel(kern.halo, dim3(plan.grid), dim3(kTcThreads), args, (size_t)plan.smem_bytes, (cudaStream_t)stream));
         MR_LAUNCH_CHECK("conv_tc_halo_kernel");
         return MR_OK;
     }
-    const size_t smem = (size_t)stages * stage_bytes + 1024;
-    int grid = sms * ctas_per_sm;
-    if (grid > a.total_tiles) grid = a.total_tiles;
     void* args[] = {&tmA[0], &tmA[1], &tmA[2], &tmBs[0], &tmBs[1], &tmBs[2], &tmBs[3], &a};
     MR_CUDA(cudaFuncSetAttribute(kern.tap, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(212 * 1024)));
-    MR_CUDA(cudaLaunchKernel(kern.tap, dim3(grid), dim3(kTcThreads), args, smem, (cudaStream_t)stream));
+    MR_CUDA(cudaLaunchKernel(kern.tap, dim3(plan.grid), dim3(kTcThreads), args, (size_t)plan.smem_bytes, (cudaStream_t)stream));
     MR_LAUNCH_CHECK("conv_tc_kernel");
     return MR_OK;
 }

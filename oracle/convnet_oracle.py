@@ -122,6 +122,79 @@ def depth_module(sd, cost_volume, keyframe, image_features, prefix="depth_module
     return preds
 
 
+ACT_NONE, ACT_LEAKY, ACT_SIGMOID, ACT_ABSTANH = 0, 1, 2, 3    # include/monorec_b200.h MR_ACT_*
+
+
+def exact_grid_data(shape, lim, scale_log2, generator):
+    """Integers in [-lim, lim] times 2^-scale_log2 (float32).  With |i| <= 32 at 2^-3 for activations and |j| <= 8 at 2^-4 for
+    weights and biases every value lies on the TF32 and the half grid and every product is exact in fp32."""
+    i = torch.randint(-lim, lim + 1, shape, generator=generator, dtype=torch.int64)
+    return (i.to(torch.float64) * 2.0 ** -scale_log2).to(torch.float32)
+
+
+def round_tf32(x):
+    """The engine's round_out: (bits + 0x1000) & ~0x1FFF on float32 (round half away from zero onto 10 mantissa bits)."""
+    bits = x.contiguous().view(torch.int32)
+    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+def conv_engine_ref(srcs, w, bias, kh, kw, stride, pad, out_hw, out_step=(1, 1), out_off=(0, 0), act=ACT_NONE, act_a=0.0,
+                    act_b=1.0, round_out=False, out_dtype=torch.float32, upsample2=False, exact=True):
+    """Reference of one call of the convolution engine (include/monorec_b200.h, mr_conv_desc), in float64 on the CPU.
+
+    srcs: NHWC tensors [B, Hs, Ws, C_i] concatenated along C; w: correlation kernel (Cout, sum C_i, kh, kw); bias: (Cout,) or
+    None; pad = (pad_t, pad_l) leading zero padding, every tap outside the (optionally nearest-x2 upsampled) input reads 0;
+    out_hw = (Ho, Wo).  Returns (pre, out, ys, xs): pre = the float64 sum of products [B, Ho, Wo, Cout] (exact);
+    out = bias + activation + output rounding applied the way the kernels do it, in float32 (then out_dtype); output
+    pixel (oy, ox) belongs at destination row ys[oy], column xs[ox].
+
+    exact=True asserts that the data makes the engine's result exact whatever its accumulation order: every input a multiple
+    of 2^-3 and every weight / bias a multiple of 2^-4 (so every product and partial sum is a multiple of 2^-7), and the sum
+    of |products| + |bias| of every output below 2^17, so every partial sum fits the 24-bit fp32 significand."""
+    x = torch.cat([s.to(torch.float64) for s in srcs], 3).permute(0, 3, 1, 2)          # NCHW float64
+    if upsample2:
+        x = x.repeat_interleave(2, 2).repeat_interleave(2, 3)
+    Ho, Wo = out_hw
+    sy, sx = stride
+    pt, pl = pad
+    x = x[:, :, max(-pt, 0):, max(-pl, 0):]              # negative SAME padding (stride > kernel) crops, as PadSameConv2d does
+    pt, pl = max(pt, 0), max(pl, 0)
+    B, C, H, W = x.shape
+    need_h, need_w = (Ho - 1) * sy + kh, (Wo - 1) * sx + kw
+    xp = torch.zeros(B, C, max(need_h, pt + H), max(need_w, pl + W), dtype=torch.float64)
+    xp[:, :, pt:pt + H, pl:pl + W] = x
+    xp = xp[:, :, :need_h, :need_w]
+    w64 = w.to(torch.float64)
+    pre = F.conv2d(xp, w64, None, stride=stride)[:, :, :Ho, :Wo]
+    if exact:
+        assert torch.equal(torch.frac(x * 8), torch.zeros_like(x)), "inputs must be multiples of 2^-3"
+        assert torch.equal(torch.frac(w64 * 16), torch.zeros_like(w64)), "weights must be multiples of 2^-4"
+        mag = F.conv2d(xp.abs(), w64.abs(), None, stride=stride)[:, :, :Ho, :Wo]
+        if bias is not None:
+            b64 = bias.to(torch.float64)
+            assert torch.equal(torch.frac(b64 * 16), torch.zeros_like(b64)), "biases must be multiples of 2^-4"
+            mag = mag + b64.abs().view(1, -1, 1, 1)
+        assert float(mag.max()) < 2.0 ** 17, f"partial sums reach {float(mag.max())}: not exact in fp32"
+    pre = pre.permute(0, 2, 3, 1).contiguous()
+    v = pre.to(torch.float32)                                                            # exact (see above)
+    if bias is not None:
+        v = v + bias.to(torch.float32)
+    if act == ACT_LEAKY:
+        v = torch.where(v >= 0, v, torch.tensor(act_a, dtype=torch.float32) * v)
+    elif act == ACT_SIGMOID:
+        v = torch.sigmoid(v.to(torch.float64)).to(torch.float32)
+    elif act == ACT_ABSTANH:
+        v = (act_a + act_b * torch.tanh(v.to(torch.float64)).abs()).to(torch.float32)
+    else:
+        assert act == ACT_NONE, act
+    if round_out:
+        v = round_tf32(v)
+    out = v.to(out_dtype)
+    ys = torch.arange(Ho) * out_step[0] + out_off[0]
+    xs = torch.arange(Wo) * out_step[1] + out_off[1]
+    return pre, out, ys, xs
+
+
 def resnet_features(sd, keyframe_plus_half, prefix="_feature_extractor.encoder."):
     """ResnetEncoder.forward (monorec_model.py:118-129) on torchvision resnet18 weights held in `sd` (eval BN)."""
     import torchvision

@@ -270,18 +270,6 @@ def test_modules_tf32_vs_oracle(tf32_mode):
     assert em < 1e-2 and max(ed) < 1e-2
 
 
-def test_tc_halo_variant_in_subprocess():
-    """The opt-in halo-reuse kernel (MONOREC_B200_TC_HALO=1; one input box per tile, resident weights) computes the same
-    layers; the switch is read once per process, hence the subprocess."""
-    import os
-    import subprocess
-    import sys
-    env = dict(os.environ, MONOREC_B200_TC_HALO="1")
-    r = subprocess.run([sys.executable, "-m", "pytest", __file__, "-q", "-m", "gpu", "-k", "tc_conv_matches_torch or tc_concat"],
-                       env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:]
-
-
 def test_full_size_model_modes_and_graph_replay():
     """BASELINE config 3 shape (256x512, D=32, F=4): tensor-core vs CUDA-core arithmetic agree within the TF32 tolerance,
     and the CUDA-graph replay reproduces the eager forward bit for bit."""
