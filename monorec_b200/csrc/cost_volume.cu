@@ -134,16 +134,10 @@ __host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_
     return L;
 }
 
-// ---- fp32 pair helpers (a pair is either two columns or two samples).  sm_90a has no packed fp32x2 arithmetic, so each
-// helper is two scalar round-to-nearest operations; the _rn intrinsics keep ptxas from contracting them, so every result is
-// rounded exactly as a packed FADD2 / FMUL2 / FFMA2 would round it. ----------------------------------------------------
+// ---- fp32 pairs (a pair is either two columns or two samples of one lane).  sm_90a has no packed fp32x2 arithmetic: the
+// march is written per scalar.  Stage 2 uses an explicit fmaf wherever a product feeds an add; stage 1 rounds every sample
+// position and weight separately (see bilinear_weights). ---------------------------------------------------------------
 __device__ __forceinline__ float2 bc2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
-__device__ __forceinline__ float2 neg2(float2 a) { return make_float2(-a.x, -a.y); }
 
 // single MUFU.RCP (flush-to-zero variant: no denormal pre/post-scaling code; operands here are never denormal)
 __device__ __forceinline__ float fast_rcp(float x) {
@@ -243,12 +237,22 @@ struct Stage1Ctx {
 
 __device__ __forceinline__ void setup_stage1(Stage1Ctx& c, const float* m, float z, float2 fu2) {
     // projection c = M [u v 1]^T z + p split into a per-lane column part and a per-row part
-    c.pzx = mul2(mul2(bc2(m[0]), fu2), bc2(z));
-    c.pzy = mul2(mul2(bc2(m[4]), fu2), bc2(z));
-    c.pzz = mul2(mul2(bc2(m[8]), fu2), bc2(z));
+    c.pzx = make_float2(__fmul_rn(m[0] * fu2.x, z), __fmul_rn(m[0] * fu2.y, z));
+    c.pzy = make_float2(__fmul_rn(m[4] * fu2.x, z), __fmul_rn(m[4] * fu2.y, z));
+    c.pzz = make_float2(__fmul_rn(m[8] * fu2.x, z), __fmul_rn(m[8] * fu2.y, z));
     c.rax = m[1] * z; c.rbx = fmaf(m[2], z, m[3]);
     c.ray = m[5] * z; c.rby = fmaf(m[6], z, m[7]);
     c.raz = m[9] * z; c.rbz = fmaf(m[10], z, m[11]);
+}
+
+// Bilinear weights of one sample at u = cx / cz (sample position + 0.5) with tap origin x0f, y0f.  Stage 1 rounds every
+// position and weight separately (the _rn intrinsics keep ptxas from contracting them): the SSIM of low-variance windows
+// amplifies a last-bit move of the sample position far more than any other rounding of the march.
+__device__ __forceinline__ void bilinear_weights(float ux, float uy, float x0f, float y0f, float& w00, float& w01, float& w10,
+                                                 float& w11) {
+    const float wx1 = __fadd_rn(__fadd_rn(ux, -0.5f), -x0f), wy1 = __fadd_rn(__fadd_rn(uy, -0.5f), -y0f);
+    const float wx0 = __fadd_rn(1.0f, -wx1), wy0 = __fadd_rn(1.0f, -wy1);
+    w00 = __fmul_rn(wx0, wy0); w01 = __fmul_rn(wx1, wy0); w10 = __fmul_rn(wx0, wy1); w11 = __fmul_rn(wx1, wy1);
 }
 
 struct Taps {                            // the 24 taps and 4 weight pairs of one row step (two samples per lane)
@@ -262,32 +266,34 @@ struct Taps {                            // the 24 taps and 4 weight pairs of on
 template <int MODE>
 __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float fv, Taps& t) {
     const float rcx = fmaf(c.rax, fv, c.rbx), rcy = fmaf(c.ray, fv, c.rby), rcz = fmaf(c.raz, fv, c.rbz);
-    const float2 cx = add2(c.pzx, bc2(rcx)), cy = add2(c.pzy, bc2(rcy)), cz = add2(c.pzz, bc2(rcz));
-    const float2 inv = make_float2(fast_rcp(cz.x), fast_rcp(cz.y));
-    float2 ux = mul2(cx, inv), uy = mul2(cy, inv);   // sample position + 0.5
-    if (MODE <= 1) {
+    const float inv[2] = {fast_rcp(__fadd_rn(c.pzz.x, rcz)), fast_rcp(__fadd_rn(c.pzz.y, rcz))};
+    // sample position + 0.5
+    float ux[2] = {__fmul_rn(__fadd_rn(c.pzx.x, rcx), inv[0]), __fmul_rn(__fadd_rn(c.pzx.y, rcx), inv[1])};
+    float uy[2] = {__fmul_rn(__fadd_rn(c.pzy.x, rcy), inv[0]), __fmul_rn(__fadd_rn(c.pzy.y, rcy), inv[1])};
+    // floor by magic-number rounding: rn(s - 0.5) differs from floor(s) only for integral s, where the interpolated value
+    // is the same (weight 1 on the tap both conventions share)
+    float tx[2], ty[2];
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
         if (MODE == 1) {   // == .clamp(-2, 2) of the normalised grid (monorec_model.py:208); also maps NaN to the low bound
-            ux.x = fminf(fmaxf(ux.x, c.sx_lo), c.sx_hi); ux.y = fminf(fmaxf(ux.y, c.sx_lo), c.sx_hi);
-            uy.x = fminf(fmaxf(uy.x, c.sy_lo), c.sy_hi); uy.y = fminf(fmaxf(uy.y, c.sy_lo), c.sy_hi);
+            ux[k] = fminf(fmaxf(ux[k], c.sx_lo), c.sx_hi); uy[k] = fminf(fmaxf(uy[k], c.sy_lo), c.sy_hi);
         }
-        // floor by magic-number rounding: rn(s - 0.5) differs from floor(s) only for integral s, where the interpolated value
-        // is the same (weight 1 on the tap both conventions share)
-        const float2 tx = add2(ux, bc2(kMagic - 1.0f)), ty = add2(uy, bc2(kMagic - 1.0f));
-        const float2 x0f = add2(tx, bc2(-kMagic)), y0f = add2(ty, bc2(-kMagic));
-        const float2 wx1 = add2(add2(ux, bc2(-0.5f)), neg2(x0f)), wy1 = add2(add2(uy, bc2(-0.5f)), neg2(y0f));
-        const float2 wx0 = add2(bc2(1.0f), neg2(wx1)), wy0 = add2(bc2(1.0f), neg2(wy1));
-        t.w00 = mul2(wx0, wy0); t.w01 = mul2(wx1, wy0); t.w10 = mul2(wx0, wy1); t.w11 = mul2(wx1, wy1);
+        tx[k] = __fadd_rn(ux[k], kMagic - 1.0f); ty[k] = __fadd_rn(uy[k], kMagic - 1.0f);
+    }
+    if (MODE <= 1) {
+        bilinear_weights(ux[0], uy[0], tx[0] - kMagic, ty[0] - kMagic, t.w00.x, t.w01.x, t.w10.x, t.w11.x);
+        bilinear_weights(ux[1], uy[1], tx[1] - kMagic, ty[1] - kMagic, t.w00.y, t.w01.y, t.w10.y, t.w11.y);
         uint32_t aa, ab;
         if (MODE == 0) {
             // address = window + 4 ((y0 - wy0) kPitch + x0 - wx0) with y0 = bits(ty) - kMagicBits: every constant is in kaddr
-            aa = ((((uint32_t)__float_as_int(ty.x) << 7) + (uint32_t)__float_as_int(tx.x)) << 2) + c.kaddr;
-            ab = ((((uint32_t)__float_as_int(ty.y) << 7) + (uint32_t)__float_as_int(tx.y)) << 2) + c.kaddr;
+            aa = ((((uint32_t)__float_as_int(ty[0]) << 7) + (uint32_t)__float_as_int(tx[0])) << 2) + c.kaddr;
+            ab = ((((uint32_t)__float_as_int(ty[1]) << 7) + (uint32_t)__float_as_int(tx[1])) << 2) + c.kaddr;
         } else {
             // integer tap origin clamped to [-2, W] x [-2, H]: taps of the ring [-2,-1] / [W, W+1] are zero-filled by TMA
-            const int xa = min(max(__float_as_int(tx.x) - kMagicBits, -2), c.W);
-            const int xb = min(max(__float_as_int(tx.y) - kMagicBits, -2), c.W);
-            const int ya = min(max(__float_as_int(ty.x) - kMagicBits, -2), c.H);
-            const int yb = min(max(__float_as_int(ty.y) - kMagicBits, -2), c.H);
+            const int xa = min(max(__float_as_int(tx[0]) - kMagicBits, -2), c.W);
+            const int xb = min(max(__float_as_int(tx[1]) - kMagicBits, -2), c.W);
+            const int ya = min(max(__float_as_int(ty[0]) - kMagicBits, -2), c.H);
+            const int yb = min(max(__float_as_int(ty[1]) - kMagicBits, -2), c.H);
             aa = ((((uint32_t)ya << 7) + (uint32_t)xa) << 2) + c.kaddr;
             ab = ((((uint32_t)yb << 7) + (uint32_t)xb) << 2) + c.kaddr;
         }
@@ -310,17 +316,14 @@ __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float f
         }
     } else {
         const int W = c.W, H = c.H;
-        const float2 tx = add2(ux, bc2(kMagic - 1.0f)), ty = add2(uy, bc2(kMagic - 1.0f));
-        const int x0a = __float_as_int(tx.x) - kMagicBits, x0b = __float_as_int(tx.y) - kMagicBits;
-        const int y0a = __float_as_int(ty.x) - kMagicBits, y0b = __float_as_int(ty.y) - kMagicBits;
+        const int x0a = __float_as_int(tx[0]) - kMagicBits, x0b = __float_as_int(tx[1]) - kMagicBits;
+        const int y0a = __float_as_int(ty[0]) - kMagicBits, y0b = __float_as_int(ty[1]) - kMagicBits;
         const bool inb = ((unsigned)x0a <= (unsigned)(W - 2)) && ((unsigned)x0b <= (unsigned)(W - 2)) &&
                          ((unsigned)y0a <= (unsigned)(H - 2)) && ((unsigned)y0b <= (unsigned)(H - 2));
         int oa, ob, dxa, dxb, dya, dyb;
         if (__all_sync(0xffffffffu, inb)) {
-            const float2 x0f = add2(tx, bc2(-kMagic)), y0f = add2(ty, bc2(-kMagic));
-            const float2 wx1 = add2(add2(ux, bc2(-0.5f)), neg2(x0f)), wy1 = add2(add2(uy, bc2(-0.5f)), neg2(y0f));
-            const float2 wx0 = add2(bc2(1.0f), neg2(wx1)), wy0 = add2(bc2(1.0f), neg2(wy1));
-            t.w00 = mul2(wx0, wy0); t.w01 = mul2(wx1, wy0); t.w10 = mul2(wx0, wy1); t.w11 = mul2(wx1, wy1);
+            bilinear_weights(ux[0], uy[0], tx[0] - kMagic, ty[0] - kMagic, t.w00.x, t.w01.x, t.w10.x, t.w11.x);
+            bilinear_weights(ux[1], uy[1], tx[1] - kMagic, ty[1] - kMagic, t.w00.y, t.w01.y, t.w10.y, t.w11.y);
             oa = y0a * W + x0a; ob = y0b * W + x0b;
             dxa = dxb = 1; dya = dyb = W;
         } else {
@@ -330,9 +333,8 @@ __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float f
             int os[2], dxs[2], dys[2];
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
-                float sxk = (k ? ux.y : ux.x), syk = (k ? uy.y : uy.x);
-                sxk = fminf(fmaxf(sxk, c.sx_lo), c.sx_hi) - 0.5f;
-                syk = fminf(fmaxf(syk, c.sy_lo), c.sy_hi) - 0.5f;
+                const float sxk = fminf(fmaxf(ux[k], c.sx_lo), c.sx_hi) - 0.5f;
+                const float syk = fminf(fmaxf(uy[k], c.sy_lo), c.sy_hi) - 0.5f;
                 const float x0f = floorf(sxk), y0f = floorf(syk);
                 float wx1 = sxk - x0f, wy1 = syk - y0f;
                 float wx0 = (x0f + 1.0f) - sxk, wy0 = (y0f + 1.0f) - syk;
@@ -346,9 +348,8 @@ __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float f
                 wx0s[k] = wx0; wx1s[k] = wx1; wy0s[k] = wy0; wy1s[k] = wy1;
                 os[k] = ya * W + xa; dxs[k] = xb - xa; dys[k] = (yb - ya) * W;
             }
-            const float2 wx0 = make_float2(wx0s[0], wx0s[1]), wx1 = make_float2(wx1s[0], wx1s[1]);
-            const float2 wy0 = make_float2(wy0s[0], wy0s[1]), wy1 = make_float2(wy1s[0], wy1s[1]);
-            t.w00 = mul2(wx0, wy0); t.w01 = mul2(wx1, wy0); t.w10 = mul2(wx0, wy1); t.w11 = mul2(wx1, wy1);
+            t.w00 = make_float2(wx0s[0] * wy0s[0], wx0s[1] * wy0s[1]); t.w01 = make_float2(wx1s[0] * wy0s[0], wx1s[1] * wy0s[1]);
+            t.w10 = make_float2(wx0s[0] * wy1s[0], wx0s[1] * wy1s[1]); t.w11 = make_float2(wx1s[0] * wy1s[0], wx1s[1] * wy1s[1]);
             oa = os[0]; ob = os[1]; dxa = dxs[0]; dxb = dxs[1]; dya = dys[0]; dyb = dys[1];
         }
 #pragma unroll
@@ -382,7 +383,7 @@ __device__ __forceinline__ void warp_row_finish(const Taps& t, const uint32_t xw
 struct Stage2Ctx {
     float2 cw0, cw1, cw2;    // channel weights / 9
     int pairflag;            // 1: both columns of this lane are output pixels and W is even (one 8-byte store)
-    bool st0, st1;
+    bool st0, st1;           // otherwise: column 2l / 2l+1 is an output pixel (one 4-byte store each)
     uint64_t pol_keep;
 };
 
@@ -418,50 +419,53 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
     yl[1] = lds64<kRowStride * 4>(yr);     yrr[1] = lds64<kRowStride * 4 + 8>(yr);
     yl[2] = lds64<2 * kRowStride * 4>(yr); yrr[2] = lds64<2 * kRowStride * 4 + 8>(yr);
     k4[0] = lds128<0>(cr); k4[1] = lds128<512>(cr); k4[2] = lds128<1024>(cr);
+    // horizontal 3-sums of X, X^2, XY: the middle pair (columns 2l, 2l+1) is shared by both columns of the lane, and every
+    // product is folded into an FFMA of its sum
     float2 h1[3], hx[3], hy[3];
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-        const float2 xxl = mul2(xl[ch], xl[ch]), xxr = mul2(xrr[ch], xrr[ch]), xyl = mul2(xl[ch], yl[ch]), xyr = mul2(xrr[ch], yrr[ch]);
-        const float m1 = xl[ch].y + xrr[ch].x, mx = xxl.y + xxr.x, my = xyl.y + xyr.x;
-        h1[ch] = make_float2(xl[ch].x + m1, m1 + xrr[ch].y);
-        hx[ch] = make_float2(xxl.x + mx, mx + xxr.y);
-        hy[ch] = make_float2(xyl.x + my, my + xyr.y);
+        const float2 l = xl[ch], r = xrr[ch], ly = yl[ch], ry = yrr[ch];
+        const float m1 = l.y + r.x, mx = fmaf(l.y, l.y, r.x * r.x), my = fmaf(l.y, ly.y, r.x * ry.x);
+        h1[ch] = make_float2(l.x + m1, m1 + r.y);
+        hx[ch] = make_float2(fmaf(l.x, l.x, mx), fmaf(r.y, r.y, mx));
+        hy[ch] = make_float2(fmaf(l.x, ly.x, my), fmaf(r.y, ry.y, my));
     }
-    float2 e[3];
+    float e[3][2];
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
         // SSIM with every factor scaled by 81 (layers.py:123-137 through 3x3 box sums s = sum x, sxx, sxy; Y = 9 mu_y,
         // Sg = 81 (sigma_y + C2) hoisted):  n/d = (2 s Y + 81 C1)(2 (9 sxy - s Y) + 81 C2) / ((s^2 + Y^2 + 81 C1)(9 sxx - s^2 + Sg))
-        const float2 Y = make_float2(k4[ch].x, k4[ch].y), Sg = make_float2(k4[ch].z, k4[ch].w);
-        const float2 s = add2(add2(st.hs1[P1][ch], st.hs1[P2][ch]), h1[ch]);
-        const float2 sxx = add2(add2(st.hsx[P1][ch], st.hsx[P2][ch]), hx[ch]);
-        const float2 sxy = add2(add2(st.hsy[P1][ch], st.hsy[P2][ch]), hy[ch]);
-        const float2 p = mul2(s, Y), q = mul2(s, s);
-        const float2 n1h = add2(neg2(p), bc2(-40.5f * kC1));                 // -(N1 / 2)
-        const float2 n2 = fma2(bc2(2.0f), fma2(bc2(9.0f), sxy, neg2(p)), bc2(81.0f * kC2));
-        const float2 d1 = add2(q, fma2(Y, Y, bc2(81.0f * kC1)));
-        const float2 d2 = add2(fma2(bc2(9.0f), sxx, Sg), neg2(q));
-        const float2 num = mul2(n1h, n2), den = mul2(d1, d2);
-        // clamp((1 - n/d) / 2, 0, 1)   (layers.py:137)
-        e[ch] = make_float2(__saturatef(fmaf(num.x, fast_rcp(den.x), 0.5f)), __saturatef(fmaf(num.y, fast_rcp(den.y), 0.5f)));
+        const float Y[2] = {k4[ch].x, k4[ch].y}, Sg[2] = {k4[ch].z, k4[ch].w};
+        const float h1c[2] = {h1[ch].x, h1[ch].y}, hxc[2] = {hx[ch].x, hx[ch].y}, hyc[2] = {hy[ch].x, hy[ch].y};
+        const float a1[2] = {st.hs1[P1][ch].x, st.hs1[P1][ch].y}, b1[2] = {st.hs1[P2][ch].x, st.hs1[P2][ch].y};
+        const float ax[2] = {st.hsx[P1][ch].x, st.hsx[P1][ch].y}, bx[2] = {st.hsx[P2][ch].x, st.hsx[P2][ch].y};
+        const float ay[2] = {st.hsy[P1][ch].x, st.hsy[P1][ch].y}, by[2] = {st.hsy[P2][ch].x, st.hsy[P2][ch].y};
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const float s = (a1[k] + b1[k]) + h1c[k], sxx = (ax[k] + bx[k]) + hxc[k], sxy = (ay[k] + by[k]) + hyc[k];
+            const float p = s * Y[k];
+            const float n1h = -p - 40.5f * kC1;                                // -(N1 / 2)
+            const float n2 = fmaf(2.0f, fmaf(9.0f, sxy, -p), 81.0f * kC2);
+            const float d1 = fmaf(s, s, fmaf(Y[k], Y[k], 81.0f * kC1));        // s^2 + Y^2 + 81 C1
+            const float d2 = fmaf(-s, s, fmaf(9.0f, sxx, Sg[k]));              // 9 sxx - s^2 + Sg
+            // clamp((1 - n/d) / 2, 0, 1)   (layers.py:137)
+            e[ch][k] = __saturatef(fmaf(n1h * n2, fast_rcp(d1 * d2), 0.5f));
+        }
     }
-    const float2 E = fma2(c.cw2, e[2], fma2(c.cw1, e[1], mul2(c.cw0, e[0])));
+    const float2 E = make_float2(fmaf(c.cw2.x, e[2][0], fmaf(c.cw1.x, e[1][0], c.cw0.x * e[0][0])),
+                                 fmaf(c.cw2.y, e[2][1], fmaf(c.cw1.y, e[1][1], c.cw0.y * e[0][1])));
     const float eL = __shfl_up_sync(0xffffffffu, E.y, 1);
     const float eR = __shfl_down_sync(0xffffffffu, E.x, 1);
     const float mid = E.x + E.y;
     const float2 hEc = make_float2(eL + mid, mid + eR);
     // single-frame volume 1 - 2 sad (monorec_model.py:251) straight to HBM; the validity mask is applied by the
     // per-pixel phase (which zeroes invalid pixels) once all planes are known
-    const float2 sad = add2(add2(st.hE[P1], st.hE[P2]), hEc);
-    const float2 sv = fma2(bc2(-2.0f), sad, bc2(1.0f));
-    if (store) {
-        if (c.pairflag) {
-            st_hint_f2(out, sv, c.pol_keep);
-        } else {
-            if (c.st0) st_hint_f1(out, sv.x, c.pol_keep);
-            if (c.st1) st_hint_f1(out + 1, sv.y, c.pol_keep);
-        }
-    }
+    const float2 sv = make_float2(fmaf(-2.0f, (st.hE[P1].x + st.hE[P2].x) + hEc.x, 1.0f),
+                                  fmaf(-2.0f, (st.hE[P1].y + st.hE[P2].y) + hEc.y, 1.0f));
+    // predicated stores (no divergent branch in the row loop): the lane's pair as one 8-byte store, or its single column
+    if (store && c.pairflag) st_hint_f2(out, sv, c.pol_keep);
+    if (store && c.st0) st_hint_f1(out, sv.x, c.pol_keep);
+    if (store && c.st1) st_hint_f1(out + 1, sv.y, c.pol_keep);
     st.hE[P] = hEc;
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) { st.hs1[P][ch] = h1[ch]; st.hsx[P][ch] = hx[ch]; st.hsy[P][ch] = hy[ch]; }
@@ -536,8 +540,12 @@ struct PixelPhase {
 };
 
 template <int T>
-__device__ __forceinline__ void pixel_phase(const PixelPhase& c, const int tid) {
+__device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
     constexpr int kSlots = 32 / T;                       // pixels per warp iteration
+    // the thread index is read again here (volatile: not merged with the kernel's own read) instead of being kept live in a
+    // register across the march, where ptxas spilled it and reloaded it on every pixel iteration
+    int tid;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
     const int lane = tid & 31, warp = tid >> 5;
     const int sub = lane % kSlots, chunk = lane / kSlots;
     const int D = c.D, F = c.F, TH = c.TH;
@@ -557,12 +565,35 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c, const int tid) 
         // addresses advance by pointer increments (one 64-bit add per access; an index expression costs a wide multiply each)
         char* cv_out = reinterpret_cast<char*>(c.cv + ((size_t)c.b * D + d_lo) * plane + pix);
         char* sf = reinterpret_cast<char*>(c.sfcv + ((size_t)c.b * D + d_lo) * plane + pix);       // frame f: + f * fstride
-        float acc[kChunk], vv[kChunk];
+        float acc[kChunk], vv[kChunk], nv[kChunk];
 #pragma unroll
         for (int j = 0; j < kChunk; ++j) acc[j] = 0.f;
         float wsum = 0.f;
+        // this lane's planes of frame f -> nv (-2 for planes >= D and invalid pixels).  With T == 1 the loads of frame f + 1
+        // are issued before frame f is reduced, so one frame's memory round trip overlaps the arithmetic of the previous one
+        auto fetch = [&](const int f, const char* q) {
+            if (own && (c.vmask[f * vstride + p] != 0)) {
+                if (D == T * kChunk) {                   // 32 / 64 / 128 planes: no per-plane predicates
+#pragma unroll
+                    for (int j = 0; j < kChunk; ++j, q += pstride) nv[j] = __ldcg(reinterpret_cast<const float*>(q));
+                } else {
+#pragma unroll
+                    for (int j = 0; j < kChunk; ++j, q += pstride) nv[j] = (d_lo + j < D) ? __ldcg(reinterpret_cast<const float*>(q)) : -2.0f;
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < kChunk; ++j) nv[j] = -2.0f;
+            }
+        };
+        // (T == 1 only: with T > 1 a lane's chunk is a quarter or half of the pixel's planes, and a second chunk of registers
+        // would spill)
+        if (T == 1) fetch(0, sf);
         for (int f = 0; f < F; ++f, sf += fstride) {
             const bool valid = own && (c.vmask[f * vstride + p] != 0);
+            if (T > 1) fetch(f, sf);
+#pragma unroll
+            for (int j = 0; j < kChunk; ++j) vv[j] = nv[j];
+            if (T == 1 && f + 1 < F) fetch(f + 1, sf + fstride);
             char* nh = nullptr;                          // this pixel's D channels of frame f in the NHWC copy (T == 1 only)
             if (T == 1 && c.sf_nhwc != nullptr)
                 nh = static_cast<char*>(c.sf_nhwc) + (((size_t)f * c.B + c.b) * plane + pix) * D * (c.sf_nhwc_half ? 2 : 4);
@@ -575,18 +606,6 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c, const int tid) 
                     for (int o = 0; o < D * (c.sf_nhwc_half ? 2 : 4); o += 16) *reinterpret_cast<uint4*>(nh + o) = make_uint4(0, 0, 0, 0);
             }
             if (T == 1 && !valid) continue;
-            if (valid) {
-                if (D == T * kChunk) {                   // 32 / 64 / 128 planes: no per-plane predicates
-#pragma unroll
-                    for (int j = 0; j < kChunk; ++j, q += pstride) vv[j] = __ldcg(reinterpret_cast<const float*>(q));
-                } else {
-#pragma unroll
-                    for (int j = 0; j < kChunk; ++j, q += pstride) vv[j] = (d_lo + j < D) ? __ldcg(reinterpret_cast<const float*>(q)) : -2.0f;
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < kChunk; ++j) vv[j] = -2.0f;
-            }
             float m4[4] = {-2.0f, -2.0f, -2.0f, -2.0f};
 #pragma unroll
             for (int j = 0; j < kChunk; ++j) m4[j & 3] = fmaxf(m4[j & 3], vv[j]);
@@ -874,7 +893,8 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     // ---- march over the F*D (frame, plane) units; no CTA-wide barrier in here ------------------------------------
     Stage2Ctx c2;
     c2.cw0 = bc2(a.cw0); c2.cw1 = bc2(a.cw1); c2.cw2 = bc2(a.cw2);
-    c2.st0 = st0; c2.st1 = st1; c2.pairflag = (st0 && st1 && ((W & 1) == 0)) ? 1 : 0; c2.pol_keep = pol_keep;
+    c2.pairflag = (st0 && st1 && ((W & 1) == 0)) ? 1 : 0;
+    c2.st0 = st0 && !c2.pairflag; c2.st1 = st1 && !c2.pairflag; c2.pol_keep = pol_keep;
     Stage1Ctx c1;
     c1.W = W; c1.H = H; c1.planei = planei;
     c1.sx_lo = sx_lo; c1.sx_hi = sx_hi; c1.sy_lo = sy_lo; c1.sy_hi = sy_hi;
@@ -953,9 +973,9 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     pp.kq = 0.5f * sqrtf(a.alpha * 1.4426950408889634f);
     pp.pol_stream = pol_stream;
     if (MR_CV_SKIP != 2) {
-        if (D <= kChunk) pixel_phase<1>(pp, tid);
-        else if (D <= 2 * kChunk) pixel_phase<2>(pp, tid);
-        else pixel_phase<4>(pp, tid);
+        if (D <= kChunk) pixel_phase<1>(pp);
+        else if (D <= 2 * kChunk) pixel_phase<2>(pp);
+        else pixel_phase<4>(pp);
     }
 }
 
