@@ -93,6 +93,22 @@ int mr_cost_volume_fwd_nhwc(const float* keyframe, const float* const* frames, c
                             int B, int F, int D, int H, int W,
                             float alpha, const float* chan_w, void* stream);
 
+/* mr_cost_volume_fwd on per-pixel depth hypotheses (data_dict["cv_depths"], monorec_model.py:181-182, :194-201):
+ *   pixel_depths  [B,D,H,W] fp32, 4-byte aligned: the depth of plane d at keyframe pixel (y, x); any order along d, and
+ *                 D need not be the model's cv_depth_steps (the view weight uses this D)
+ *   proj          [B,F,3,4] from mr_projection_tables(..., depths = NULL, ...)
+ *   out_sfcv_nhwc NULL, or [F,B,H,W,D] as in mr_cost_volume_fwd_nhwc (needs D <= 32, D % 8 == 0); nhwc_dtype MR_DT_F32 or
+ *                 MR_DT_F16 either way
+ * A pixel with a hypothesis that is not finite or <= 0 is invalid for every frame, and one whose nearest / farthest hypothesis
+ * projects behind a source camera is invalid for that frame (single-frame volume and view weight 0).  The TMA windows / gather choice is made as in
+ * mr_cost_volume_fwd; a depth map that repeats one depth per plane gives mr_cost_volume_fwd's results bit for bit.
+ * Constraints as mr_cost_volume_fwd.  All arguments are checked before the first CUDA call. */
+int mr_cost_volume_fwd_depthmap(const float* keyframe, const float* const* frames, const float* proj,
+                                const float* pixel_depths, float* out_cv, float* out_sfcv,
+                                void* out_sfcv_nhwc, int nhwc_dtype,
+                                int B, int F, int D, int H, int W,
+                                float alpha, const float* chan_w, void* stream);
+
 /* Same path with HOST buffers (pinned or pageable): uploads the images and matrices, runs
  * mr_projection_tables + mr_cost_volume_fwd and downloads both volumes; batch elements are pipelined on
  * internal streams so copies overlap the kernel.  This is the end-to-end entry bench.py times as `e2e`.

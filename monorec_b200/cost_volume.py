@@ -60,12 +60,18 @@ class CostVolumeModule(nn.Module):
 
     @torch.no_grad()
     def forward(self, data_dict):
+        """data_dict["cv_depths"], when present, gives the depth hypotheses per pixel as in the reference (:181-182): a
+        (B, D, H, W) tensor on the keyframe's device with 2 <= D <= 128, any order along D.  It replaces the uniform
+        inverse-depth planes, and its D is the one of the view weight.  It is read as contiguous fp32: other dtypes and
+        expanded or strided views (such as a broadcast of per-plane depths) are materialised first.
+        """
         start_time = time.time()
         keyframe = _as_f32c(data_dict["keyframe"])
         if not keyframe.is_cuda:
             raise _lib.MonorecLibraryError("monorec_b200.CostVolumeModule needs CUDA tensors (no CPU fallback)")
+        pixel_depths = None
         if "cv_depths" in data_dict:
-            raise NotImplementedError("monorec_b200: per-pixel cv_depths hypotheses are not implemented")
+            pixel_depths = self._check_cv_depths(data_dict["cv_depths"], keyframe)
         lib = _lib.load()
         frames, intrinsics, poses = self._gather(data_dict)
         frames = [_as_f32c(f) for f in frames]
@@ -77,26 +83,41 @@ class CostVolumeModule(nn.Module):
         F = len(frames)
         if C != 3:
             raise NotImplementedError("monorec_b200: 3-channel images only")
-        # .item()-free: the ranges are python floats on the model, mirrored into the dict as 1-element tensors
-        lo, hi, D = self._plane_range(data_dict)
+        if pixel_depths is not None:
+            lo, hi, D = 0.0, 0.0, pixel_depths.shape[1]
+        else:
+            # .item()-free: the ranges are python floats on the model, mirrored into the dict as 1-element tensors
+            lo, hi, D = self._plane_range(data_dict)
         dev = keyframe.device
         stream = torch.cuda.current_stream(dev).cuda_stream
         with torch.cuda.device(dev):
             proj = torch.empty(B, F, 3, 4, device=dev, dtype=torch.float32)
-            depths = torch.empty(D, device=dev, dtype=torch.float32)
+            depths = torch.empty(D, device=dev, dtype=torch.float32) if pixel_depths is None else None
             cv = torch.empty(B, D, H, W, device=dev, dtype=torch.float32)
             sfcv = torch.empty(F, B, D, H, W, device=dev, dtype=torch.float32)
             _lib.check(lib.mr_projection_tables(kpose.data_ptr(), kK.data_ptr(), _lib.ptr_array(poses),
                                                 _lib.ptr_array(intrinsics), B, F, H, W, proj.data_ptr(),
-                                                depths.data_ptr(), D, lo, hi, stream), "mr_projection_tables")
+                                                None if depths is None else depths.data_ptr(), D, lo, hi, stream),
+                       "mr_projection_tables")
             cw = None
             if self.channel_weights is not None:
                 cw = (_lib.c_float * 3)(*self.channel_weights)
             else:
                 cw = (_lib.c_float * 3)(1 / 3, 1 / 3, 1 / 3)  # monorec_model.py:174-177
             nhwc = data_dict.get("_sfcv_nhwc")   # MonoRecModel: the MaskModule's input buffer [F*B,H,W,D], filled by the kernel
-            if nhwc is not None and self.tma_windows and D <= 32 and D % 8 == 0 and tuple(nhwc.shape) == (F * B, H, W, D) \
-                    and nhwc.is_contiguous() and nhwc.dtype in (torch.float32, torch.float16):
+            fill_nhwc = nhwc is not None and self.tma_windows and D <= 32 and D % 8 == 0 \
+                and tuple(nhwc.shape) == (F * B, H, W, D) and nhwc.is_contiguous() \
+                and nhwc.dtype in (torch.float32, torch.float16)
+            if pixel_depths is not None:
+                # (one entry: it chooses TMA windows or the gather itself, like mr_cost_volume_fwd)
+                _lib.check(lib.mr_cost_volume_fwd_depthmap(
+                    keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), pixel_depths.data_ptr(), cv.data_ptr(),
+                    sfcv.data_ptr(), nhwc.data_ptr() if fill_nhwc else None,
+                    1 if fill_nhwc and nhwc.dtype == torch.float16 else 0, B, F, D, H, W, float(self.alpha), cw, stream),
+                    "mr_cost_volume_fwd_depthmap")
+                if fill_nhwc:
+                    data_dict["_sfcv_nhwc_filled"] = True
+            elif fill_nhwc:
                 _lib.check(lib.mr_cost_volume_fwd_nhwc(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
                                                        depths.data_ptr(), cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr(),
                                                        1 if nhwc.dtype == torch.float16 else 0, B, F, D, H, W,
@@ -111,6 +132,22 @@ class CostVolumeModule(nn.Module):
         # host-side issue time (the reference's number includes its device work only because it synchronises implicitly)
         data_dict["cv_module_time"] = torch.full((1,), time.time() - start_time, device=dev, dtype=torch.float32)
         return data_dict
+
+    @staticmethod
+    def _check_cv_depths(z, keyframe):
+        """(B, D, H, W) per-pixel hypotheses as contiguous fp32 on the keyframe's device; ValueError before any launch."""
+        B, _, H, W = keyframe.shape
+        if not torch.is_tensor(z):
+            raise ValueError(f"cv_depths must be a tensor, got {type(z).__name__}")
+        if z.device != keyframe.device:
+            raise ValueError(f"cv_depths is on {z.device}, the keyframe on {keyframe.device}")
+        if z.dim() != 4 or z.shape[0] != B or z.shape[2] != H or z.shape[3] != W:
+            raise ValueError(f"cv_depths must be shaped (B, D, H, W) = ({B}, D, {H}, {W}), got {tuple(z.shape)}")
+        if not 2 <= z.shape[1] <= 128:
+            raise ValueError(f"cv_depths needs 2 <= D <= 128 hypotheses per pixel, got D = {z.shape[1]}")
+        if z.is_complex():
+            raise ValueError("cv_depths must be real")
+        return _as_f32c(z)
 
     @staticmethod
     def _plane_range(data_dict):

@@ -107,10 +107,13 @@ struct GroupInfo {                       // one window (a run of consecutive pla
 };
 
 struct SmemLayout {
-    int win, ytile, cst, xbuf, pjs, zs, vmask, rowrng, bbox, gid, uflag, ginfo, seq2g, nwin, bars, ctr, total;  // byte offsets
+    int win, ytile, cst, xbuf, pjs, zs, vmask, rowrng, bbox, gid, uflag, ginfo, seq2g, nwin, bars, ctr;  // byte offsets
+    int zpix, zrow;      // per-pixel depths only: [TH][kTileCols] and [D][TH+4] float2 (min, max) depth tables
+    int total;
 };
 
-__host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_tma) {
+// pix: the per-pixel depth source (cv_depths) appends its two depth tables; the plane layout is unchanged
+__host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_tma, bool pix = false) {
     SmemLayout L;
     int off = 0;
     auto take = [&](int bytes, int align) { off = (off + align - 1) / align * align; int o = off; off += bytes; return o; };
@@ -130,6 +133,12 @@ __host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_
     L.nwin = take(MR_MAX_FRAMES * 4, 4);
     L.bars = take(kBuf * 8, 8);
     L.ctr = take((2 + 2 * kBuf) * 4, 4);
+    if (pix) {
+        L.zpix = take(TH * kTileCols * 8, 16);
+        L.zrow = take(D * (TH + 4) * 8, 16);
+    } else {
+        L.zpix = L.zrow = 0;
+    }
     L.total = off;
     return L;
 }
@@ -233,6 +242,11 @@ struct Stage1Ctx {
     const float* img;                    // global mode: source frame of this batch element, [3][H][W]
     int W, H, planei;
     float sx_lo, sx_hi, sy_lo, sy_hi;    // == grid clamp(-2, 2) + 0.5, monorec_model.py:208
+    // per-pixel depths only: the depth changes from sample to sample, so setup_stage1's products are formed per sample
+    float2 mu0, mu4, mu8;                // rn(m0 u), rn(m4 u), rn(m8 u) of the lane's two columns
+    float m1, m2, m3, m5, m6, m7, m9, m10, m11;
+    const float* zp;                     // the unit's depth plane cv_depths[b, d], [H][W]
+    int zc0, zc1;                        // the lane's two columns clamped into the image
 };
 
 __device__ __forceinline__ void setup_stage1(Stage1Ctx& c, const float* m, float z, float2 fu2) {
@@ -243,6 +257,24 @@ __device__ __forceinline__ void setup_stage1(Stage1Ctx& c, const float* m, float
     c.rax = m[1] * z; c.rbx = fmaf(m[2], z, m[3]);
     c.ray = m[5] * z; c.rby = fmaf(m[6], z, m[7]);
     c.raz = m[9] * z; c.rbz = fmaf(m[10], z, m[11]);
+}
+
+// The per-pixel counterpart: only the depth-free factors are kept; warp_row_issue<MODE, true> rounds every product of
+// setup_stage1 per sample in the same order, so a depth map that repeats one depth per plane gives the plane path's bits.
+__device__ __forceinline__ void setup_stage1_pix(Stage1Ctx& c, const float* m, float2 fu2, const float* zp) {
+    c.mu0 = make_float2(__fmul_rn(m[0], fu2.x), __fmul_rn(m[0], fu2.y));
+    c.mu4 = make_float2(__fmul_rn(m[4], fu2.x), __fmul_rn(m[4], fu2.y));
+    c.mu8 = make_float2(__fmul_rn(m[8], fu2.x), __fmul_rn(m[8], fu2.y));
+    c.m1 = m[1]; c.m2 = m[2]; c.m3 = m[3];
+    c.m5 = m[5]; c.m6 = m[6]; c.m7 = m[7];
+    c.m9 = m[9]; c.m10 = m[10]; c.m11 = m[11];
+    c.zp = zp;
+}
+
+// depth of the lane's two columns in image row v (clamped into the image: halo rows only feed invalid outputs)
+__device__ __forceinline__ float2 load_row_depths(const Stage1Ctx& c, const int v) {
+    const int o = min(max(v, 0), c.H - 1) * c.W;
+    return make_float2(__ldg(c.zp + (o + c.zc0)), __ldg(c.zp + (o + c.zc1)));
 }
 
 // Bilinear weights of one sample at u = cx / cz (sample position + 0.5) with tap origin x0f, y0f.  Stage 1 rounds every
@@ -263,13 +295,29 @@ struct Taps {                            // the 24 taps and 4 weight pairs of on
 // MODE 0: taps from the window, every sample of the unit strictly inside the image (decided by the plan): no clamps
 // MODE 1: taps from the window, coordinates clamped to the 2-px zero ring (== zero padding of F.grid_sample)
 // MODE 2: taps from global memory with per-tap zero padding
-template <int MODE>
-__device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float fv, Taps& t) {
-    const float rcx = fmaf(c.rax, fv, c.rbx), rcy = fmaf(c.ray, fv, c.rby), rcz = fmaf(c.raz, fv, c.rbz);
-    const float inv[2] = {fast_rcp(__fadd_rn(c.pzz.x, rcz)), fast_rcp(__fadd_rn(c.pzz.y, rcz))};
-    // sample position + 0.5
-    float ux[2] = {__fmul_rn(__fadd_rn(c.pzx.x, rcx), inv[0]), __fmul_rn(__fadd_rn(c.pzx.y, rcx), inv[1])};
-    float uy[2] = {__fmul_rn(__fadd_rn(c.pzy.x, rcy), inv[0]), __fmul_rn(__fadd_rn(c.pzy.y, rcy), inv[1])};
+// PIX: z = the depths of the lane's two samples in this row (per-pixel depth source); unused for the plane table
+template <int MODE, bool PIX = false>
+__device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float fv, Taps& t, const float2 z = float2{}) {
+    float inv[2], ux[2], uy[2];
+    if constexpr (!PIX) {
+        const float rcx = fmaf(c.rax, fv, c.rbx), rcy = fmaf(c.ray, fv, c.rby), rcz = fmaf(c.raz, fv, c.rbz);
+        inv[0] = fast_rcp(__fadd_rn(c.pzz.x, rcz)); inv[1] = fast_rcp(__fadd_rn(c.pzz.y, rcz));
+        // sample position + 0.5
+        ux[0] = __fmul_rn(__fadd_rn(c.pzx.x, rcx), inv[0]); ux[1] = __fmul_rn(__fadd_rn(c.pzx.y, rcx), inv[1]);
+        uy[0] = __fmul_rn(__fadd_rn(c.pzy.x, rcy), inv[0]); uy[1] = __fmul_rn(__fadd_rn(c.pzy.y, rcy), inv[1]);
+    } else {
+        // setup_stage1 and the row part above, per sample: rn(rn(m0 u) z) + fma(rn(m1 z), v, fma(m2, z, m3)), ...
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const float zk = k ? z.y : z.x;
+            const float rcx = fmaf(__fmul_rn(c.m1, zk), fv, fmaf(c.m2, zk, c.m3));
+            const float rcy = fmaf(__fmul_rn(c.m5, zk), fv, fmaf(c.m6, zk, c.m7));
+            const float rcz = fmaf(__fmul_rn(c.m9, zk), fv, fmaf(c.m10, zk, c.m11));
+            inv[k] = fast_rcp(__fadd_rn(__fmul_rn(k ? c.mu8.y : c.mu8.x, zk), rcz));
+            ux[k] = __fmul_rn(__fadd_rn(__fmul_rn(k ? c.mu0.y : c.mu0.x, zk), rcx), inv[k]);
+            uy[k] = __fmul_rn(__fadd_rn(__fmul_rn(k ? c.mu4.y : c.mu4.x, zk), rcy), inv[k]);
+        }
+    }
     // floor by magic-number rounding: rn(s - 0.5) differs from floor(s) only for integral s, where the interpolated value
     // is the same (weight 1 on the tap both conventions share)
     float tx[2], ty[2];
@@ -480,18 +528,28 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
 // a triple (the rolling state is symmetric under rotation of its slots).
 //   xb: shared address of this warp's two row buffers; yr / cr: keyframe row rlo-2 / table row rlo-2 (lane columns);
 //   out: single-frame volume at output row rlo - 4 (advanced every step, stored from the fifth step on); wstride = W
-template <int MODE>
+//   PIX: per-pixel depths, read from image row v0 (= fv0) on; each row's depths are loaded one row step before they are used
+template <int MODE, bool PIX = false>
 __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx& c2, const uint32_t xb, const int lane,
                                            const float fv0, const int nsteps, uint32_t yr, uint32_t cr, float* out,
-                                           const int wstride) {
+                                           const int wstride, const int v0 = 0) {
     Stage2State st;
     st.clear();
     float fv = fv0;
     uint32_t off = 0;                      // byte offset of the row buffer stage 2 reads next
     const uint32_t xw = xb + 4 * (lane + 1), xr = xb + 8 * lane;
+    int zv = v0 + 1;                       // PIX: image row of the depths in flight (zn)
+    float2 zn{};
+    if constexpr (PIX) zn = load_row_depths(c1, v0);
     {
         Taps t;
-        warp_row_issue<MODE>(c1, fv, t);
+        if constexpr (PIX) {
+            const float2 zc = zn;
+            zn = load_row_depths(c1, zv);
+            warp_row_issue<MODE, true>(c1, fv, t, zc);
+        } else {
+            warp_row_issue<MODE>(c1, fv, t);
+        }
         warp_row_finish(t, xw);
     }
     __syncwarp();
@@ -501,7 +559,13 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
     auto both = [&](auto tag) {
         fv += 1.0f;
         Taps tp;
-        if (MR_CV_SKIP != 4) warp_row_issue<MODE>(c1, fv, tp);
+        if constexpr (PIX) {
+            const float2 zc = zn;
+            zn = load_row_depths(c1, ++zv);
+            if (MR_CV_SKIP != 4) warp_row_issue<MODE, true>(c1, fv, tp, zc);
+        } else {
+            if (MR_CV_SKIP != 4) warp_row_issue<MODE>(c1, fv, tp);
+        }
         if (MR_CV_ORDER == 0 && MR_CV_SKIP != 4) warp_row_finish(tp, xw + (kXbBytes - off));
         if (MR_CV_SKIP != 3) ssim_row<decltype(tag)::value>(st, c2, xr + off, yr, cr, out, done >= 4);
         if (MR_CV_ORDER != 0 && MR_CV_SKIP != 4) warp_row_finish(tp, xw + (kXbBytes - off));
@@ -659,10 +723,13 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
     }
 }
 
+// PIX selects the depth source: false = one depth per plane (a.depths = zs[D], the default linspace planes), true = one depth
+// per plane and pixel (a.depths = cv_depths [B,D,H,W]).
+template <bool PIX>
 __global__ void __launch_bounds__(kThreads, MR_CV_MINBLOCKS)
 cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     extern __shared__ __align__(128) unsigned char smem[];
-    const SmemLayout L = make_layout(a.D, a.TH, a.F, a.use_tma);
+    const SmemLayout L = make_layout(a.D, a.TH, a.F, a.use_tma, PIX);
     float* win = reinterpret_cast<float*>(smem + L.win);
     float* ytile = reinterpret_cast<float*>(smem + L.ytile);
     float* cst = reinterpret_cast<float*>(smem + L.cst);
@@ -706,7 +773,50 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             ytile[line * kRowStride + idx] = val;
         }
     }
-    for (int i = tid; i < D; i += kThreads) zs[i] = __ldg(a.depths + i);
+    if constexpr (!PIX) {
+        for (int i = tid; i < D; i += kThreads) zs[i] = __ldg(a.depths + i);
+    } else {
+        // Depth extremes.  fminf / fmaxf drop NaN, so a hypothesis that is not finite is recorded explicitly: it turns the
+        // entry into (NaN, NaN), which fails every comparison of the validity pre-pass and of the plan.
+        const float* zb = a.depths + (size_t)b * D * plane;
+        const float kFinite = 3.40282347e38f;
+        // per output pixel, over its own D hypotheses (validity pre-pass); only pixels that can be valid are evaluated.  A
+        // hypothesis <= 0 is no point in front of the keyframe camera: like a non-finite one, it makes the pixel invalid.
+        float2* zpix = reinterpret_cast<float2*>(smem + L.zpix);
+        for (int p = tid; p < TH * kTileCols; p += kThreads) {
+            const int r = p >> 6, bc = p & 63;
+            const int u = u0 + bc, v = v0 + r;
+            float lo = __int_as_float(0x7fc00000), hi = lo;
+            if (bc >= 2 && bc < 2 + kOutCols && u >= 2 && u < W - 2 && v >= 2 && v < H - 2) {
+                const float* q = zb + (size_t)v * W + u;
+                lo = 3.0e38f; hi = -3.0e38f;
+                bool bad = false;
+                for (int d = 0; d < D; ++d, q += plane) {
+                    const float z = __ldg(q);
+                    bad = bad || !(z > 0.f && z <= kFinite);
+                    lo = fminf(lo, z); hi = fmaxf(hi, z);
+                }
+                if (bad) lo = hi = __int_as_float(0x7fc00000);
+            }
+            zpix[p] = make_float2(lo, hi);
+        }
+        // per plane and tile row -2 .. TH+1, over the 64 buffer columns, rows and columns clamped into the image as stage 1
+        // reads them (the plan reduces the rows each frame's march touches)
+        float2* zrow = reinterpret_cast<float2*>(smem + L.zrow);
+        for (int line = warp; line < D * (TH + 4); line += kWarps) {
+            const int d = line / (TH + 4), rr = line - d * (TH + 4);
+            const float* q = zb + (size_t)d * plane + (size_t)min(max(v0 - 2 + rr, 0), H - 1) * W;
+            const float z0 = __ldg(q + min(max(u0 + lane, 0), W - 1)), z1 = __ldg(q + min(max(u0 + lane + 32, 0), W - 1));
+            const bool bad = __any_sync(0xffffffffu, !(fabsf(z0) <= kFinite) || !(fabsf(z1) <= kFinite));
+            float lo = fminf(z0, z1), hi = fmaxf(z0, z1);
+#pragma unroll
+            for (int s = 16; s >= 1; s >>= 1) {
+                lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, s));
+                hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, s));
+            }
+            if (lane == 0) zrow[line] = bad ? make_float2(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000)) : make_float2(lo, hi);
+        }
+    }
     if (lane < 6) {   // columns -1 and 64 of both row buffers stay zero
         const int rb = lane / 3, ch = lane % 3;
         xbuf[(rb * 3 + ch) * kRowStride] = 0.f;
@@ -764,7 +874,13 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             const float m03 = m[3], m13 = m[7], m23 = m[11];
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
-                const float z = zs[k ? D - 1 : 0];
+                float z;
+                if constexpr (PIX) {   // the pixel's own nearest and farthest hypothesis (NaN: one is not finite)
+                    const float2 e = reinterpret_cast<const float2*>(smem + L.zpix)[r * kTileCols + bc];
+                    z = k ? e.y : e.x;
+                } else {
+                    z = zs[k ? D - 1 : 0];
+                }
                 const float den = fmaf(az, z, m23);
                 const float inv = fast_rcp(den);
                 const float sx = fmaf(fmaf(ax, z, m03), inv, -0.5f);
@@ -787,13 +903,31 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
         unsigned char fl = 0;          // bit 0: footprint usable for a window, bit 1: strictly inside the image
         if (rhi >= rlo && a.use_tma) {
             const float* m = pjs + 12 * f;
-            const float z = zs[d];
-            float xmin = 3.0e38f, xmax = -3.0e38f, ymin = 3.0e38f, ymax = -3.0e38f;
+            float zlo, zhi = 0.f;
             bool good = true;
+            if constexpr (PIX) {
+                // depth interval of plane d over the rows rlo-2 .. rhi+2 this frame's march touches.  The unit's samples lie
+                // in the hull of the 8 points (tile corner, zlo / zhi) and the denominator is affine in that point, so while
+                // it is > 0 at the 8 corners their projections bound every sample.  Not finite, or far beyond any scene
+                // depth (where the products of stage 1 could overflow): the unit gathers with clamped taps.
+                const float2* zrow = reinterpret_cast<const float2*>(smem + L.zrow) + d * (TH + 4);
+                zlo = zrow[rlo].x; zhi = zrow[rlo].y;
+                bool finite = (zlo == zlo) && (zhi == zhi);
+                for (int rr = rlo + 1; rr <= rhi + 4; ++rr) {
+                    const float2 e = zrow[rr];
+                    finite = finite && (e.x == e.x) && (e.y == e.y);
+                    zlo = fminf(zlo, e.x); zhi = fmaxf(zhi, e.y);
+                }
+                good = finite && fmaxf(-zlo, zhi) < 1.0e20f;
+            } else {
+                zlo = zs[d];
+            }
+            float xmin = 3.0e38f, xmax = -3.0e38f, ymin = 3.0e38f, ymax = -3.0e38f;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
+            for (int k = 0; k < (PIX ? 8 : 4); ++k) {
                 const float fu = (float)(u0 + ((k & 1) ? kTileCols - 1 : 0));
                 const float fv = (float)(v0 + ((k & 2) ? rhi + 2 : rlo - 2));
+                const float z = (PIX && (k & 4)) ? zhi : zlo;
                 const float cx = fmaf(fmaf(m[0], fu, fmaf(m[1], fv, m[2])), z, m[3]);
                 const float cy = fmaf(fmaf(m[4], fu, fmaf(m[5], fv, m[6])), z, m[7]);
                 const float cz = fmaf(fmaf(m[8], fu, fmaf(m[9], fv, m[10])), z, m[11]);
@@ -898,6 +1032,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     Stage1Ctx c1;
     c1.W = W; c1.H = H; c1.planei = planei;
     c1.sx_lo = sx_lo; c1.sx_hi = sx_hi; c1.sy_lo = sy_lo; c1.sy_hi = sy_hi;
+    if constexpr (PIX) { c1.zc0 = min(max(u0 + lane, 0), W - 1); c1.zc1 = min(max(u0 + lane + 32, 0), W - 1); }
     // per-lane shared addresses for stage 2 (columns 2l-1 .. 2l+2 live at float index 2l .. 2l+3 of a row)
     const uint32_t xb_s = smem_u32(xbuf);
     const uint32_t ys_s = smem_u32(ytile) + 8 * lane;
@@ -911,7 +1046,8 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
         const int f = unit / D, d = unit - f * D;
         const int rlo = rowrng[2 * f], rhi = rowrng[2 * f + 1];
         if (rhi < rlo) continue;  // no valid pixel of this tile for frame f: the per-pixel phase zero-fills
-        setup_stage1(c1, pjs + 12 * f, zs[d], fu2);
+        if constexpr (PIX) setup_stage1_pix(c1, pjs + 12 * f, fu2, a.depths + ((size_t)b * D + d) * plane);
+        else setup_stage1(c1, pjs + 12 * f, zs[d], fu2);
         const int nsteps = rhi - rlo + 5;
         const float fv0 = (float)(v0 + rlo - 2);
         const uint32_t yr = ys_s + rlo * kYRowBytes;          // tile row rlo-2 is keyframe-tile row rlo
@@ -936,10 +1072,10 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             if (uflag[unit] & 2) {
                 // tap address = wb + 4 ((bits(ty) - kMagicBits - wy0) kPitch + bits(tx) - kMagicBits - wx0), mod 2^32
                 c1.kaddr = wb - 4u * ((uint32_t)(kMagicBits + gi.wy0) * kPitch + (uint32_t)(kMagicBits + gi.wx0));
-                march_unit<0>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W);
+                march_unit<0, PIX>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
             } else {
                 c1.kaddr = wb - 4u * ((uint32_t)(int)gi.wy0 * kPitch + (uint32_t)(int)gi.wx0);
-                march_unit<1>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W);
+                march_unit<1, PIX>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
             }
             // hand the buffer on: the last unit of the window re-arms it with the window after next
             if (lane == 0) {
@@ -957,7 +1093,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             __syncwarp();
         } else {
             c1.img = a.frames[f] + (size_t)b * 3 * plane;
-            march_unit<2>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W);
+            march_unit<2, PIX>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
         }
     }
     __syncthreads();  // the marching warps' global stores are visible to the whole CTA from here on
@@ -1056,11 +1192,23 @@ __global__ void projection_tables_kernel(const float* kf_pose, const float* kf_K
     }
 }
 
-int pick_tile_rows(int D, int F, int use_tma) {
+int pick_tile_rows(int D, int F, int use_tma, bool pix) {
     const int limit = 227 * 1024;
     for (int th = MR_CV_TILE_ROWS; th >= 2; th >>= 1)
-        if (make_layout(D, th, F, use_tma).total <= limit) return th;
+        if (make_layout(D, th, F, use_tma, pix).total <= limit) return th;
     return 0;
+}
+
+template <bool PIX>
+int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
+    static int smem_set = 0;   // the attribute is per function and per device context; setting it again is harmless
+    if (smem_set < smem) {
+        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        smem_set = 227 * 1024;
+    }
+    cost_volume_kernel<PIX><<<grid, kThreads, smem, stream>>>(a, maps);
+    MR_LAUNCH_CHECK("cost_volume_kernel");
+    return MR_OK;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1105,7 +1253,7 @@ extern "C" int mr_projection_tables(const float* keyframe_pose, const float* key
 int mr::launch_cost_volume(const float* keyframe, const float* const* frames, const float* proj,
                            const float* depths, float* out_cv, float* out_sfcv, int B, int F, int D, int H, int W,
                            float alpha, const float* chan_w, int b_begin, int b_count, int gather_only,
-                           cudaStream_t stream, void* sf_nhwc, int sf_nhwc_dtype) {
+                           cudaStream_t stream, void* sf_nhwc, int sf_nhwc_dtype, int per_pixel_depths) {
     MR_REQUIRE(keyframe && frames && proj && depths && out_cv && out_sfcv, "mr_cost_volume_fwd: null pointer");
     MR_REQUIRE(b_begin >= 0 && b_count >= 1 && b_begin + b_count <= B, "mr_cost_volume_fwd: bad batch range");
     MR_REQUIRE(B >= 1 && B <= 21845, "mr_cost_volume_fwd: batch %d out of range", B);
@@ -1147,23 +1295,17 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
             a.use_tma = 1;
         }
     }
-    a.TH = pick_tile_rows(D, F, a.use_tma);
+    const bool pix = per_pixel_depths != 0;
+    a.TH = pick_tile_rows(D, F, a.use_tma, pix);
     MR_REQUIRE(a.TH > 0, "mr_cost_volume_fwd: no tile height fits shared memory for D=%d F=%d", D, F);
     a.alpha = alpha;
     a.inv_dm1 = (float)(1.0 / (double)(D - 1));
     const float def_w[3] = {5.f / 32.f, 16.f / 32.f, 11.f / 32.f};  // monorec_model.py:133
     const float* cw = chan_w ? chan_w : def_w;
     a.cw0 = cw[0] / 9.f; a.cw1 = cw[1] / 9.f; a.cw2 = cw[2] / 9.f;  // monorec_model.py:141 (weights / patch_size^2)
-    const SmemLayout L = make_layout(D, a.TH, F, a.use_tma);
+    const SmemLayout L = make_layout(D, a.TH, F, a.use_tma, pix);
     dim3 grid((W + kOutCols - 1) / kOutCols, (H + a.TH - 1) / a.TH, b_count);
-    static int smem_set = 0;   // the attribute is per function and per device context; setting it again is harmless
-    if (smem_set < L.total) {
-        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        smem_set = 227 * 1024;
-    }
-    cost_volume_kernel<<<grid, kThreads, L.total, stream>>>(a, local);
-    MR_LAUNCH_CHECK("cost_volume_kernel");
-    return MR_OK;
+    return pix ? launch_kernel<true>(grid, L.total, stream, a, local) : launch_kernel<false>(grid, L.total, stream, a, local);
 }
 
 extern "C" int mr_cost_volume_fwd(const float* keyframe, const float* const* frames, const float* proj,
@@ -1186,4 +1328,19 @@ extern "C" int mr_cost_volume_fwd_nhwc(const float* keyframe, const float* const
     MR_REQUIRE(out_sfcv_nhwc != nullptr, "mr_cost_volume_fwd_nhwc: null NHWC buffer");
     return mr::launch_cost_volume(keyframe, frames, proj, depths, out_cv, out_sfcv, B, F, D, H, W, alpha, chan_w, 0, B, 0,
                                   (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype);
+}
+
+extern "C" int mr_cost_volume_fwd_depthmap(const float* keyframe, const float* const* frames, const float* proj,
+                                           const float* pixel_depths, float* out_cv, float* out_sfcv, void* out_sfcv_nhwc,
+                                           int nhwc_dtype, int B, int F, int D, int H, int W, float alpha,
+                                           const float* chan_w, void* stream) {
+    MR_REQUIRE(pixel_depths != nullptr, "mr_cost_volume_fwd_depthmap: null pixel_depths");
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(pixel_depths) & 3) == 0,
+               "mr_cost_volume_fwd_depthmap: pixel_depths must be 4-byte aligned");
+    MR_REQUIRE(D >= 2 && D <= 128, "mr_cost_volume_fwd_depthmap: 2 <= D <= 128 required (got D=%d)", D);
+    MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "mr_cost_volume_fwd_depthmap: 1 <= F <= %d required (got F=%d)", MR_MAX_FRAMES, F);
+    MR_REQUIRE(nhwc_dtype == MR_DT_F32 || nhwc_dtype == MR_DT_F16,
+               "mr_cost_volume_fwd_depthmap: nhwc_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", nhwc_dtype);
+    return mr::launch_cost_volume(keyframe, frames, proj, pixel_depths, out_cv, out_sfcv, B, F, D, H, W, alpha, chan_w, 0, B,
+                                  0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, 1);
 }

@@ -6,7 +6,8 @@ Compiles cost_volume.cu (default: the package's) for sm_90a with the library's f
 it with line information and finds the loops of cost_volume_kernel (backward branches).  A loop is attributed to a
 call site of march_unit<MODE> or pixel_phase<T> when the inlining chains of its instructions reach that call's source
 line.  For each march mode it prints the largest such loop, the row loop (three row steps per body), and for the
-per-pixel phase its loops; counts are per row step for the march and per loop iteration otherwise.
+per-pixel phase its loops; counts are per row step for the march and per loop iteration otherwise.  The plane-depth
+instantiation cost_volume_kernel<false> is reported first, the per-pixel-depth one (cv_depths) after it.
 """
 import collections
 import re
@@ -47,12 +48,19 @@ def disassemble(src):
                               capture_output=True, text=True).stdout
 
 
-def kernel_instructions(dis):
-    """[(addr, opcode, text, source lines of the inlining chain)] and {label: addr} of cost_volume_kernel."""
+INSTANTIATIONS = [  # (label, mangled template argument of cost_volume_kernel<PIX>)
+    ("plane depths (cost_volume_kernel<false>)", "cost_volume_kernelILb0E"),
+    ("per-pixel depths (cost_volume_kernel<true>)", "cost_volume_kernelILb1E"),
+]
+
+
+def kernel_instructions(dis, name="cost_volume_kernelILb0E"):
+    """[(addr, opcode, text, source lines of the inlining chain)] and {label: addr} of the kernel whose .text section
+    name contains `name` (default: the plane instantiation)."""
     ins, labels, cur, inside, pending = [], {}, [], False, []
     for line in dis.splitlines():
         if line.startswith(".text."):
-            inside = "cost_volume_kernel" in line
+            inside = name in line
             continue
         if not inside:
             continue
@@ -80,10 +88,21 @@ def main():
     text = src.read_text().splitlines()
     sites = {}
     for i, l in enumerate(text, 1):
-        m = re.search(r"\b(march_unit|pixel_phase)<(\d)>\(", l)
+        m = re.search(r"\b(march_unit|pixel_phase)<(\d)(?:, PIX)?>\(", l)
         if m and "__device__" not in l and "void" not in l:
             sites[f"{m.group(1)}<{m.group(2)}>"] = i
-    ins, labels = kernel_instructions(disassemble(src))
+    dis = disassemble(src)
+    for k, (title, name) in enumerate(INSTANTIATIONS):
+        if name not in dis:      # (a source from before the depth source became a template parameter)
+            if k == 0:
+                report(src, "cost_volume_kernel", *kernel_instructions(dis, "cost_volume_kernel"), sites)
+            continue
+        if k:
+            print("\n" + "=" * 100)
+        report(src, title, *kernel_instructions(dis, name), sites)
+
+
+def report(src, title, ins, labels, sites):
     index = {a: k for k, (a, *_r) in enumerate(ins)}
     loops = []
     for k, (addr, op, body, _l) in enumerate(ins):
@@ -91,7 +110,7 @@ def main():
             tgt = re.search(r"(\.L_x_\d+)", body)
             if tgt and labels.get(tgt.group(1), addr + 1) <= addr:
                 loops.append((index[labels[tgt.group(1)]], k))
-    print(f"{src.name}: cost_volume_kernel, {len(ins)} instructions, {len(loops)} loops")
+    print(f"{src.name}: {title}, {len(ins)} instructions, {len(loops)} loops")
     for name, site in sorted(sites.items(), key=lambda kv: kv[1]):
         mine = []
         for lo, hi in loops:
