@@ -177,8 +177,9 @@ int mr_conv2d_nhwc(const mr_conv_desc* desc, void* stream);
  * 32 channels (64-byte swizzle rows); the MMA is f16; dst_dtype selects half or float output.
  * Stride-1 layers whose packed weights fit in shared memory twice per SM run on the "halo" variant of the kernel (same
  * results); larger weights stream through it, and everything else runs on the tap-refetch kernel (mr_conv2d_nhwc_tc_plan
- * tells which).  Tuning switches (environment, read once): MONOREC_B200_TC_HALO=0|1..4, MONOREC_B200_TC_STREAM=0|1,
- * MONOREC_B200_TC_HALO_F16=0|1, MONOREC_B200_TC_CTAS=n. */
+ * tells which).  Test levers (environment, read once) that force the kernels tests could not reach otherwise:
+ * MONOREC_B200_TC_HALO=0 (never the halo kernel) | 1..4 (at most n CTAs per SM; 1 also admits layers that only fit once),
+ * MONOREC_B200_TC_STREAM=0 (no streamed weights). */
 int mr_conv2d_nhwc_tc(const mr_conv_desc* desc, int n_pad, int k_pad, int round_out, void* stream);
 /* The sub-pixel convolutions of one layer -- Refine's ConvTranspose2d(k4,s2)+crop = four 2x2 filters (model/layers.py:380-400),
  * Upconv's nearest-x2 + pad + 2x2 conv = 1x1 / 1x2 / 2x1 / 2x2 filters (:338-356) -- in ONE launch: descs[0..n_phases) share the

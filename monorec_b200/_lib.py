@@ -9,7 +9,7 @@ from pathlib import Path
 import os
 
 _PKG = Path(__file__).resolve().parent
-# MONOREC_B200_LIB: load another build of the library (kernel-variant experiments: tools/build_variant.py)
+# MONOREC_B200_LIB: load another build of the library (kernel-variant experiments: tools/build_variant_src.py)
 LIB_PATH = Path(os.environ["MONOREC_B200_LIB"]) if os.environ.get("MONOREC_B200_LIB") else _PKG / "libmonorec_b200.so"
 _lib = None
 

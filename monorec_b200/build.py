@@ -14,9 +14,6 @@ LIB = PKG / "libmonorec_b200.so"
 STAMP = PKG / ".libmonorec_b200.stamp"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17"]
-for _knob in ("MR_CV_THREADS", "MR_CV_MINBLOCKS", "MR_CV_TILE_ROWS", "MR_CV_SKIP"):   # tuning knobs of the cost-volume kernel
-    if os.environ.get(_knob):
-        FLAGS.append(f"-D{_knob}=" + os.environ[_knob])
 
 
 def sources():

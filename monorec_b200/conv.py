@@ -17,19 +17,11 @@ import os
 MAX_SRC = 3
 ACT_NONE, ACT_LEAKY, ACT_SIGMOID, ACT_ABSTANH = 0, 1, 2, 3
 LEAKY_SLOPE = 0.1  # model/layers.py:290, 318, 381
-KC = 32            # channels per K chunk of the tensor-core kernel (csrc/conv_tc.cu)
 
 # Arithmetic of the dense-contraction layers: "tf32" = wgmma tensor cores (tf32, fp32 accumulate, fp32 storage),
 # "f16" = wgmma f16 with half NHWC activations and weights (fp32 accumulate; BASELINE config 3),
-# "fp32" = CUDA-core FMA kernel (bit-level parity path).  1-channel heads always use the CUDA-core dot-product kernel.
+# "fp32" = CUDA-core FMA kernel (bit-level parity path).
 MODE = os.environ.get("MONOREC_B200_CONV", "tf32").lower()
-# half sources of <= 32 channels: 32-channel K chunks (SWIZZLE_64B rows), in the tap-refetch kernel and inside the halo box alike
-# (round 2: 429 -> 203 us on the 32->32 3x3 layer over the single-frame volumes).
-K32 = os.environ.get("MONOREC_B200_TC_K32", "1") != "0"
-HALO_F16 = os.environ.get("MONOREC_B200_TC_HALO_F16", "1") != "0" and os.environ.get("MONOREC_B200_TC_HALO", "") != "0"
-# the single-channel layers (1x1 mask classifier, the four 3x3 depth heads) run on the tensor cores too in the tf32 / f16
-# modes (Cout padded to 16): 5.93 -> 5.83 ms per half-mode forward at B=8 against the CUDA-core per-pixel kernel (round 2)
-TC_HEADS = True
 DT_F32, DT_F16 = 0, 1
 FLOPS = None       # set to [0] to count the conv stacks' flops during a forward (bench.py's tensor roofline)
 
@@ -91,24 +83,6 @@ def pack_conv_weight(w):
     return w.detach().to(torch.float32).permute(2, 3, 1, 0).contiguous()
 
 
-def pack_convT_k4s2(w):
-    """nn.ConvTranspose2d(k=4, s=2) weight (Cin, Cout, 4, 4) -> four sub-pixel 2x2 kernels [py][px] -> [2][2][Cin][Cout].
-
-    With the reference's centre crop of one pixel (model/layers.py:269-286, oversize = -2) output pixel (Y, X) of the
-    cropped 2H x 2W map receives input rows i with 2 i + ky = Y + 1:
-        Y even (py = 0): (i, ky) = (Y/2 - 1, 3), (Y/2, 1)          Y odd (py = 1): (i, ky) = ((Y-1)/2, 2), ((Y+1)/2, 0)
-    i.e. a 2-tap filter along each axis on the input grid with taps ordered by increasing i.
-    """
-    w = w.detach().to(torch.float32)
-    taps = {0: (3, 1), 1: (2, 0)}
-    out = {}
-    for py in (0, 1):
-        for px in (0, 1):
-            sub = w[:, :, list(taps[py]), :][:, :, :, list(taps[px])]      # (Cin, Cout, 2, 2)
-            out[(py, px)] = sub.permute(2, 3, 0, 1).contiguous()           # [2][2][Cin][Cout]
-    return out
-
-
 def conv2d(srcs, weight, bias, kh, kw, stride=(1, 1), act=ACT_NONE, act_a=0.0, act_b=1.0, upsample2=False,
            out=None, out_coff=0, pad=None, out_hw=None, out_step=(1, 1), out_off=(0, 0)):
     """One fused convolution launch.
@@ -151,19 +125,6 @@ def conv2d(srcs, weight, bias, kh, kw, stride=(1, 1), act=ACT_NONE, act_a=0.0, a
     d.src_dtype, d.dst_dtype = _dt(x0), _dt(out)
     with torch.cuda.device(x0.device):
         _lib.check(lib.mr_conv2d_nhwc(ctypes.byref(d), _stream(x0)), "mr_conv2d_nhwc")
-    return out
-
-
-def conv_transpose_k4s2_crop(srcs, sub_weights, bias, act=ACT_LEAKY, act_a=LEAKY_SLOPE):
-    """Refine (model/layers.py:380-400): ConvTranspose2d(k4, s2) + LeakyReLU + centre crop, as 4 sub-pixel 2x2 convs."""
-    x0 = srcs[0]
-    B, Hs, Ws, _ = x0.shape
-    Cout = sub_weights[(0, 0)].shape[-1]
-    out = torch.empty(B, 2 * Hs, 2 * Ws, Cout, device=x0.device, dtype=torch.float32)
-    for py in (0, 1):
-        for px in (0, 1):
-            conv2d(srcs, sub_weights[(py, px)], bias, 2, 2, act=act, act_a=act_a, out=out,
-                   pad=(1 - py, 1 - px), out_hw=(Hs, Ws), out_step=(2, 2), out_off=(py, px))
     return out
 
 
@@ -268,23 +229,14 @@ def mask_volume(volume, mask):
 # --------------------------------------------------------------------------------------------------------------------
 # layer objects: weights packed once for both kernels, dispatch by MODE
 # --------------------------------------------------------------------------------------------------------------------
-def _round_tf32(w):
-    """Round-to-nearest onto the TF32 grid (10 explicit mantissa bits); the tensor core truncates the rest."""
-    bits = w.contiguous().view(torch.int32)
-    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
-
-
-def pack_tc_weight(w, src_c, half=False, allow_k32=True):
+def pack_tc_weight(w, src_c, half=False):
     """Correlation kernel (Cout, Cin, kh, kw) -> [kh*kw][n_pad][k_pad] K-major through the library's host-side packer
     (include/monorec_b200.h: mr_pack_conv_weights): every source padded to a whole number of K chunks (32 fp32 / 64 half
-    channels = one 128-byte swizzle row, or 32 half channels = one 64-byte row when every source has <= 32 channels; zero
-    rows), Cout padded to a multiple of 16; values rounded to TF32 (fp32 storage) or converted to half.
-    allow_k32=False / MONOREC_B200_TC_K32=0 (experiments) force 64-channel chunks by packing in torch instead."""
-    import ctypes
+    channels = one 128-byte swizzle row, or 32 half channels = one 64-byte row when every source has <= 32 channels, which
+    took the 32->32 3x3 layer over the single-frame volumes from 429 to 203 us; zero rows), Cout padded to a multiple of 16;
+    values rounded to TF32 (fp32 storage) or converted to half."""
     Cout, Cin, kh, kw = w.shape
     assert sum(src_c) == Cin
-    if half and not (K32 and allow_k32) and all(c <= 32 for c in src_c):
-        return _pack_tc_weight_torch(w, src_c, half, kc=64)
     lib = _lib.load()
     wc = w.detach().to("cpu", torch.float32).contiguous()
     sc = (ctypes.c_int * len(src_c))(*[int(c) for c in src_c])
@@ -297,28 +249,11 @@ def pack_tc_weight(w, src_c, half=False, allow_k32=True):
     return out.to(w.device), n_pad.value, k_pad.value
 
 
-def _pack_tc_weight_torch(w, src_c, half, kc=None):
-    """The same layout written with torch ops (the packer's restatement: tests compare the two)."""
-    Cout, Cin, kh, kw = w.shape
-    if kc is None:
-        kc = (32 if all(c <= 32 for c in src_c) else 64) if half else KC
-    n_pad = ((Cout + 15) // 16) * 16
-    k_pad = sum(((c + kc - 1) // kc) * kc for c in src_c)
-    out = torch.zeros(kh * kw, n_pad, k_pad, device=w.device, dtype=torch.float32)
-    wt = w.detach().to(torch.float32).permute(2, 3, 0, 1).reshape(kh * kw, Cout, Cin)
-    ci = ko = 0
-    for c in src_c:
-        out[:, :Cout, ko:ko + c] = wt[:, :, ci:ci + c]
-        ci += c
-        ko += ((c + kc - 1) // kc) * kc
-    return (out.to(torch.float16).contiguous() if half else _round_tf32(out)), n_pad, k_pad
-
-
 class PackedConv:
     """One convolution of the engine with its weights in both kernel layouts."""
 
     def __init__(self, weight, bias, src_c, stride=(1, 1), act=ACT_NONE, act_a=0.0, act_b=1.0, pad=None, out_step=(1, 1),
-                 out_off=(0, 0), allow_tc=True):
+                 out_off=(0, 0)):
         w = weight.detach().to(torch.float32)
         self.cout, self.cin, self.kh, self.kw = w.shape
         self.src_c = tuple(int(c) for c in src_c)
@@ -326,14 +261,16 @@ class PackedConv:
         self.act, self.act_a, self.act_b = act, act_a, act_b
         self.bias = None if bias is None else bias.detach().to(torch.float32).contiguous()
         self.w32 = pack_conv_weight(w)
-        self.tc_ok = (allow_tc or TC_HEADS) and self.cout <= 256 and (self.cout >= 8 or TC_HEADS) and all(c % 4 == 0 for c in self.src_c)
+        # single-channel layers (the 1x1 mask classifier, the four 3x3 depth heads) run on the tensor cores too, Cout padded
+        # to 16: 5.93 -> 5.83 ms per half-mode forward at B=8 against the CUDA-core per-pixel kernel
+        self.tc_ok = self.cout <= 256 and all(c % 4 == 0 for c in self.src_c)
         self.tc_ok_f16 = self.tc_ok and all(c % 8 == 0 for c in self.src_c)
         self._wtc = {}
         self._w_src = w
 
     def wtc(self, half=False):
         if half not in self._wtc:
-            self._wtc[half] = pack_tc_weight(self._w_src, self.src_c, half=half, allow_k32=True)
+            self._wtc[half] = pack_tc_weight(self._w_src, self.src_c, half=half)
         return self._wtc[half]
 
     def __call__(self, srcs, out=None, out_hw=None, final=False, out_coff=0):
@@ -450,10 +387,6 @@ def conv2d_tc_phases(srcs, subs, out, out_hw, round_out=True, half=False):
     return out
 
 
-# MONOREC_B200_SUBPIXEL_ONE_LAUNCH=0: one launch per sub-pixel phase (A/B measurements)
-SUBPIXEL_ONE_LAUNCH = os.environ.get("MONOREC_B200_SUBPIXEL_ONE_LAUNCH", "1") != "0"
-
-
 class PackedSubpixel:
     """Four sub-pixel convolutions writing the (2H, 2W) output with step 2: Refine's ConvTranspose2d(k4, s2) + crop
     (model/layers.py:380-400) and Upconv's nearest-x2 + pad(0,1,0,1) + 2x2 conv (:338-356)."""
@@ -467,7 +400,7 @@ class PackedSubpixel:
         out = torch.empty(B, 2 * Hs, 2 * Ws, self.subs[0].cout, device=x0.device, dtype=x0.dtype)
         L0 = self.subs[0]
         half = MODE == "f16" and x0.dtype == torch.float16 and L0.tc_ok_f16
-        if SUBPIXEL_ONE_LAUNCH and (half or (MODE == "tf32" and L0.tc_ok)) and all(L.pad is not None for L in self.subs):
+        if (half or (MODE == "tf32" and L0.tc_ok)) and all(L.pad is not None for L in self.subs):
             if FLOPS is not None:
                 FLOPS[0] += sum(2 * B * Hs * Ws * L.cout * sum(L.src_c) * L.kh * L.kw for L in self.subs)
             return conv2d_tc_phases(srcs, self.subs, out, (Hs, Ws), round_out=not half, half=half)
@@ -477,25 +410,33 @@ class PackedSubpixel:
 
 
 def refine_layer(conv2d_t, src_c, act=ACT_LEAKY, act_a=LEAKY_SLOPE):
-    w = conv2d_t.weight.detach().to(torch.float32)       # (Cin, Cout, 4, 4)
-    taps = {0: (3, 1), 1: (2, 0)}                        # see pack_convT_k4s2
+    """Refine's ConvTranspose2d(k4, s2) + crop as four 2x2 phase convolutions, decomposed by the library's host-side
+    mr_subpixel_convt_k4s2 (include/monorec_b200.h)."""
+    lib = _lib.load()
+    w = conv2d_t.weight.detach().to("cpu", torch.float32).contiguous()     # (Cin, Cout, 4, 4)
+    cin, cout = w.shape[:2]
     subs = []
     for py in (0, 1):
         for px in (0, 1):
-            sub = w[:, :, list(taps[py]), :][:, :, :, list(taps[px])].permute(1, 0, 2, 3).contiguous()  # (Cout,Cin,2,2)
-            subs.append(PackedConv(sub, conv2d_t.bias, src_c, act=act, act_a=act_a, pad=(1 - py, 1 - px),
-                                   out_step=(2, 2), out_off=(py, px)))
+            sub = torch.empty(cout, cin, 2, 2)
+            pad_t, pad_l = c_int(0), c_int(0)
+            _lib.check(lib.mr_subpixel_convt_k4s2(w.data_ptr(), cin, cout, py, px, sub.data_ptr(), ctypes.byref(pad_t),
+                                                  ctypes.byref(pad_l)), "mr_subpixel_convt_k4s2")
+            subs.append(PackedConv(sub.to(conv2d_t.weight.device), conv2d_t.bias, src_c, act=act, act_a=act_a,
+                                   pad=(pad_t.value, pad_l.value), out_step=(2, 2), out_off=(py, px)))
     return PackedSubpixel(subs)
 
 
 def upconv_layer(conv, src_c):
-    """out[2oy+py, 2ox+px] of nearest-x2 + 2x2 conv: even phases see both taps on the same input pixel (weights add up),
-    odd phases see input pixels o and o+1 (zero beyond the border = the reference's trailing pad)."""
-    w = conv.weight.detach().to(torch.float32)           # (Cout, Cin, 2, 2)
+    """Upconv's nearest-x2 + pad + 2x2 conv as four phase convolutions of 1x1 / 1x2 / 2x1 / 2x2 taps, decomposed by the
+    library's host-side mr_subpixel_upconv2 (include/monorec_b200.h)."""
+    lib = _lib.load()
+    w = conv.weight.detach().to("cpu", torch.float32).contiguous()         # (Cout, Cin, 2, 2)
+    cout, cin = w.shape[:2]
     subs = []
     for py in (0, 1):
-        wy = w if py == 1 else w.sum(2, keepdim=True)
         for px in (0, 1):
-            wyx = wy if px == 1 else wy.sum(3, keepdim=True)
-            subs.append(PackedConv(wyx.contiguous(), conv.bias, src_c, pad=(0, 0), out_step=(2, 2), out_off=(py, px)))
+            sub = torch.empty(cout, cin, 1 + py, 1 + px)
+            _lib.check(lib.mr_subpixel_upconv2(w.data_ptr(), cout, cin, py, px, sub.data_ptr(), None, None), "mr_subpixel_upconv2")
+            subs.append(PackedConv(sub.to(conv.weight.device), conv.bias, src_c, pad=(0, 0), out_step=(2, 2), out_off=(py, px)))
     return PackedSubpixel(subs)

@@ -3,7 +3,6 @@
 Same constructor arguments, same data_dict keys in and out; the arithmetic runs in the fused sm_90a kernel of
 libmonorec_b200.so (csrc/cost_volume.cu) through the C ABI.  No torch fallback.
 """
-import os
 import time
 
 import torch
@@ -39,8 +38,6 @@ class CostVolumeModule(nn.Module):
         self.alpha = alpha
         self.not_center_cv = not_center_cv
         self.sfcv_mult_mask = sfcv_mult_mask
-        # False: bilinear taps straight from global memory instead of TMA-staged shared-memory windows (tests, A/B timing)
-        self.tma_windows = os.environ.get("MONOREC_B200_CV_TMA", "1") != "0"
         if not (use_ssim is True or use_ssim == 1) or isinstance(use_ssim, float):
             raise NotImplementedError("monorec_b200: only use_ssim=True is implemented (reference default)")
         if patch_size != 3 or not_center_cv or not sfcv_mult_mask:
@@ -105,7 +102,7 @@ class CostVolumeModule(nn.Module):
             else:
                 cw = (_lib.c_float * 3)(1 / 3, 1 / 3, 1 / 3)  # monorec_model.py:174-177
             nhwc = data_dict.get("_sfcv_nhwc")   # MonoRecModel: the MaskModule's input buffer [F*B,H,W,D], filled by the kernel
-            fill_nhwc = nhwc is not None and self.tma_windows and D <= 32 and D % 8 == 0 \
+            fill_nhwc = nhwc is not None and D <= 32 and D % 8 == 0 \
                 and tuple(nhwc.shape) == (F * B, H, W, D) and nhwc.is_contiguous() \
                 and nhwc.dtype in (torch.float32, torch.float16)
             if pixel_depths is not None:
@@ -124,9 +121,9 @@ class CostVolumeModule(nn.Module):
                                                        float(self.alpha), cw, stream), "mr_cost_volume_fwd_nhwc")
                 data_dict["_sfcv_nhwc_filled"] = True
             else:
-                fwd = lib.mr_cost_volume_fwd if self.tma_windows else lib.mr_cost_volume_fwd_gather
-                _lib.check(fwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), depths.data_ptr(), cv.data_ptr(),
-                               sfcv.data_ptr(), B, F, D, H, W, float(self.alpha), cw, stream), "mr_cost_volume_fwd")
+                _lib.check(lib.mr_cost_volume_fwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), depths.data_ptr(),
+                                                  cv.data_ptr(), sfcv.data_ptr(), B, F, D, H, W, float(self.alpha), cw, stream),
+                           "mr_cost_volume_fwd")
         data_dict["cost_volume"] = cv
         data_dict["single_frame_cvs"] = [sfcv[f] for f in range(F)]
         # host-side issue time (the reference's number includes its device work only because it synchronises implicitly)

@@ -774,11 +774,8 @@ int tc_plan(const mr_conv_desc* desc, int n_phases, int n_pad, int kc, mr_tc_pla
     // Box rows are 8 + kw - 1 px, so a box holds exactly the pixels the taps touch and the 48-channel full-resolution layers
     // fit twice per SM next to their weights.
     static const int halo_env = getenv("MONOREC_B200_TC_HALO") ? atoi(getenv("MONOREC_B200_TC_HALO")) : -1;
-    static const bool halo_f16 = getenv("MONOREC_B200_TC_HALO_F16") ? (atoi(getenv("MONOREC_B200_TC_HALO_F16")) != 0) : true;
     // (64-byte rows are fine inside the halo box too: half sources of <= 32 channels packed with 32-channel chunks)
-    // MONOREC_B200_TC_HALO_PITCH=16: fixed 16-px box rows (A/B measurements)
-    static const int pitch_env = getenv("MONOREC_B200_TC_HALO_PITCH") ? atoi(getenv("MONOREC_B200_TC_HALO_PITCH")) : 0;
-    const int halo_pitch = (pitch_env >= 8 + d.kw - 1) ? pitch_env : 8 + d.kw - 1;
+    const int halo_pitch = 8 + d.kw - 1;
     const size_t halo_a_bytes = halo_box_bytes(d.kh, halo_pitch, row_bytes);
     const size_t bres_al = (bres + 1023) & ~size_t(1023);
     // CTAs per SM the accumulator registers allow (the wider N, the more registers per consumer thread)
@@ -791,8 +788,8 @@ int tc_plan(const mr_conv_desc* desc, int n_phases, int n_pad, int kc, mr_tc_pla
         return st > 4 ? 4 : st;
     };
     // CTAs per SM: up to three, each with at least two input stages (up to 4).
-    // MONOREC_B200_TC_HALO=n (1..4) caps / forces the count for measurements (1: also layers that only fit once).
-    const bool halo_shape = n_phases == 1 && halo_env != 0 && (!f16 || halo_f16) && d.sy == 1 && d.sx == 1 && d.kw <= 9 && d.kh <= 7;
+    // MONOREC_B200_TC_HALO=n (1..4) caps / forces the count (1: also layers that only fit once).
+    const bool halo_shape = n_phases == 1 && halo_env != 0 && d.sy == 1 && d.sx == 1 && d.kw <= 9 && d.kh <= 7;
     int halo_ctas = 0;
     if (halo_shape) {
         const int cap = (halo_env >= 1 && halo_env <= 4) ? halo_env : 3;
@@ -802,7 +799,7 @@ int tc_plan(const mr_conv_desc* desc, int n_phases, int n_pad, int kc, mr_tc_pla
     // Weights that do not fit next to two input stages stream instead: the [n_pad x chunk] slice of each (chunk, tap) goes through
     // a ring of 3..8 stages behind the chunk's input box.  Per tile that is all the weights once (L2 hits) plus ONE input box per
     // chunk, against kh*kw input boxes + the same weights in the tap-refetch kernel, whose L2->SM traffic bounds the
-    // multi-source decoder layers.  MONOREC_B200_TC_STREAM=0 disables it (A/B).
+    // multi-source decoder layers.  MONOREC_B200_TC_STREAM=0 disables it.
     static const bool stream_on = getenv("MONOREC_B200_TC_STREAM") ? (atoi(getenv("MONOREC_B200_TC_STREAM")) != 0) : true;
     int b_stream = 0, stream_stages = 0;
     const size_t b_slice = (size_t)n_pad * row_bytes;
@@ -825,7 +822,6 @@ int tc_plan(const mr_conv_desc* desc, int n_phases, int n_pad, int kc, mr_tc_pla
     int dev = 0, sms = 0;
     MR_CUDA(cudaGetDevice(&dev));
     MR_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    static const int kForceCtas = getenv("MONOREC_B200_TC_CTAS") ? atoi(getenv("MONOREC_B200_TC_CTAS")) : 0;   // tuning knob
     // resident CTAs per SM: bounded by the accumulator registers and capped at 4; with MMA N = 32..64 one CTA cannot keep the
     // tensor pipe busy, so several CTAs interleave their MMA chains
     const int reg_ctas = resident_ctas(kern.tap);
@@ -842,8 +838,7 @@ int tc_plan(const mr_conv_desc* desc, int n_phases, int n_pad, int kc, mr_tc_pla
         const size_t halo_front = b_stream ? (size_t)b_stream * b_slice : bres_al;   // bytes in front of the input stages
         p.smem_bytes = (int)(halo_front + (size_t)p.stages * halo_a_bytes + 1024);
     } else {
-        int ctas_per_sm = reg_ctas > 4 ? 4 : reg_ctas;
-        if (kForceCtas > 0 && kForceCtas <= reg_ctas) ctas_per_sm = kForceCtas;
+        const int ctas_per_sm = reg_ctas > 4 ? 4 : reg_ctas;
         const size_t stage_bytes = (size_t)(128 + n_pad) * row_bytes;
         const size_t budget = (size_t)(200 * 1024) / ctas_per_sm - 2 * 1024;
         int stages = (int)(budget / stage_bytes);

@@ -39,36 +39,17 @@ namespace {
 constexpr int kTileCols = 64;   // buffer columns per tile row (output columns + 2-px halo each side)
 constexpr int kOutCols = 60;    // output columns per tile
 constexpr int kRowStride = 68;  // floats per smem image row: column b lives at index b+1 (so [2l-1, 2l+2] is 8B aligned)
-#ifndef MR_CV_WARPS
-#define MR_CV_WARPS 16
-#endif
-#ifndef MR_CV_MINBLOCKS
-#define MR_CV_MINBLOCKS 1       // resident CTAs per SM the register allocator must leave room for
-#endif
-#ifndef MR_CV_NBUF
-#define MR_CV_NBUF 2            // source windows in flight per CTA
-#endif
-#ifndef MR_CV_WIN_ROWS
-#define MR_CV_WIN_ROWS 40       // rows per window (multiple of 8)
-#endif
-#ifndef MR_CV_MIN_GROUP
-#define MR_CV_MIN_GROUP 3       // plane groups smaller than this gather from global memory
-#endif
-#ifndef MR_CV_TILE_ROWS
-#define MR_CV_TILE_ROWS 16
-#endif
-#ifndef MR_CV_SKIP
-#define MR_CV_SKIP 0            // timing experiments only: 1 = no march, 2 = no per-pixel phase, 3 = march without stage 2, 4 = without stage 1
-#endif
-constexpr int kWarps = MR_CV_WARPS;
+constexpr int kWarps = 16;
 constexpr int kThreads = kWarps * 32;
-constexpr int kBuf = MR_CV_NBUF;
+constexpr int kMinBlocks = 1;                     // resident CTAs per SM the register allocator must leave room for
+constexpr int kBuf = 2;                           // source windows in flight per CTA
 constexpr int kPitch = 128;                       // pixels per window row (512 bytes)
-constexpr int kWinRows = MR_CV_WIN_ROWS;
+constexpr int kWinRows = 40;                      // rows per window (multiple of 8)
 constexpr int kChanStride = kWinRows * kPitch;    // floats between the channel planes of a window
 constexpr int kWinFloats = 3 * kChanStride;
 constexpr int kBoxRows = 8;                       // rows per TMA box
-constexpr int kMinGroup = MR_CV_MIN_GROUP;
+constexpr int kMinGroup = 3;                      // plane groups smaller than this gather from global memory
+constexpr int kTileRows = 16;                     // tile height when shared memory allows it (halved until it fits)
 static_assert(kWinRows % kBoxRows == 0, "window rows must be a multiple of the TMA box height");
 static_assert(MR_MAX_FRAMES <= kWarps, "the plan gives every source frame its own warp");
 
@@ -519,10 +500,6 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
     for (int ch = 0; ch < 3; ++ch) { st.hs1[P][ch] = h1[ch]; st.hsx[P][ch] = hx[ch]; st.hsy[P][ch] = hy[ch]; }
 }
 
-#ifndef MR_CV_ORDER
-#define MR_CV_ORDER 0     // 0: stage 1 of row t+1 completes, then stage 2 of row t (measured faster: 1.07 vs 1.12 ms); 1: taps stay in flight across stage 2
-#endif
-
 // The march of one unit over tile rows rlo-2 .. rhi+2 (nsteps = rhi - rlo + 5 >= 5 rows).  Stage 1 of the next row is
 // issued with stage 2 of the current one; the three-step loop body is entered at the slot that makes the last step end
 // a triple (the rolling state is symmetric under rotation of its slots).
@@ -562,13 +539,14 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
         if constexpr (PIX) {
             const float2 zc = zn;
             zn = load_row_depths(c1, ++zv);
-            if (MR_CV_SKIP != 4) warp_row_issue<MODE, true>(c1, fv, tp, zc);
+            warp_row_issue<MODE, true>(c1, fv, tp, zc);
         } else {
-            if (MR_CV_SKIP != 4) warp_row_issue<MODE>(c1, fv, tp);
+            warp_row_issue<MODE>(c1, fv, tp);
         }
-        if (MR_CV_ORDER == 0 && MR_CV_SKIP != 4) warp_row_finish(tp, xw + (kXbBytes - off));
-        if (MR_CV_SKIP != 3) ssim_row<decltype(tag)::value>(st, c2, xr + off, yr, cr, out, done >= 4);
-        if (MR_CV_ORDER != 0 && MR_CV_SKIP != 4) warp_row_finish(tp, xw + (kXbBytes - off));
+        // stage 1 of row t+1 completes before stage 2 of row t: measured faster than keeping the taps in flight across
+        // stage 2 (1.07 against 1.12 ms)
+        warp_row_finish(tp, xw + (kXbBytes - off));
+        ssim_row<decltype(tag)::value>(st, c2, xr + off, yr, cr, out, done >= 4);
         __syncwarp();
         off = kXbBytes - off;
         yr += kYRowBytes;
@@ -584,7 +562,7 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
         if (t + 1 >= 0) both(I1{});
         both(I2{});
     }
-    if (MR_CV_SKIP != 3) ssim_row<0>(st, c2, xr + off, yr, cr, out, true);
+    ssim_row<0>(st, c2, xr + off, yr, cr, out, true);
     __syncwarp();
 }
 
@@ -726,7 +704,7 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
 // PIX selects the depth source: false = one depth per plane (a.depths = zs[D], the default linspace planes), true = one depth
 // per plane and pixel (a.depths = cv_depths [B,D,H,W]).
 template <bool PIX>
-__global__ void __launch_bounds__(kThreads, MR_CV_MINBLOCKS)
+__global__ void __launch_bounds__(kThreads, kMinBlocks)
 cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     extern __shared__ __align__(128) unsigned char smem[];
     const SmemLayout L = make_layout(a.D, a.TH, a.F, a.use_tma, PIX);
@@ -940,7 +918,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             if (good) {
                 // one pixel of slack on every side for the rounding differences between this estimate and stage 1
                 // (the window origin is rounded down to a multiple of 4 pixels: TMA wants the innermost box coordinate
-                // 16-byte aligned -- measured: tools/experiments_r02/tma_probe.cu -- negative coordinates are fine)
+                // 16-byte aligned; negative coordinates are fine)
                 const int xl = (max((int)floorf(xmin) - 1, -2) >> 2) << 2, xh = min((int)floorf(xmax) + 2, W + 1);
                 const int yl = max((int)floorf(ymin) - 1, -2), yh = min((int)floorf(ymax) + 2, H + 1);
                 if (xh >= xl && yh >= yl && xh - xl < kPitch && yh - yl < kWinRows) {
@@ -1038,7 +1016,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     const uint32_t ys_s = smem_u32(ytile) + 8 * lane;
     const uint32_t cs_s = smem_u32(cst) + 16 * lane;
     const uint32_t win_s = smem_u32(win);
-    for (; MR_CV_SKIP != 1;) {
+    for (;;) {
         int unit = 0;
         if (lane == 0) unit = atomicAdd(&ctr[0], 1);
         unit = __shfl_sync(0xffffffffu, unit, 0);
@@ -1108,11 +1086,9 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     // exp(-alpha (sad - min sad)^2) with sad = (1 - sv) / 2 is ex2(-(k (max sv - sv))^2), k = sqrt(alpha log2(e)) / 2
     pp.kq = 0.5f * sqrtf(a.alpha * 1.4426950408889634f);
     pp.pol_stream = pol_stream;
-    if (MR_CV_SKIP != 2) {
-        if (D <= kChunk) pixel_phase<1>(pp);
-        else if (D <= 2 * kChunk) pixel_phase<2>(pp);
-        else pixel_phase<4>(pp);
-    }
+    if (D <= kChunk) pixel_phase<1>(pp);
+    else if (D <= 2 * kChunk) pixel_phase<2>(pp);
+    else pixel_phase<4>(pp);
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -1194,7 +1170,7 @@ __global__ void projection_tables_kernel(const float* kf_pose, const float* kf_K
 
 int pick_tile_rows(int D, int F, int use_tma, bool pix) {
     const int limit = 227 * 1024;
-    for (int th = MR_CV_TILE_ROWS; th >= 2; th >>= 1)
+    for (int th = kTileRows; th >= 2; th >>= 1)
         if (make_layout(D, th, F, use_tma, pix).total <= limit) return th;
     return 0;
 }

@@ -8,10 +8,10 @@ convolution engine) through the C ABI.  The ResNet-18 trunk stays on torchvision
 reference too; SURVEY.md §8f "next" row 1) with its eval-mode BatchNorms folded, in half precision in half mode.  (Round 2
 measured the trunk on the conv engine at 1.03 ms against cuDNN's 0.71 ms in half mode, so that variant was removed.)
 """
-import os
 import warnings
 
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 from . import conv as C
@@ -19,16 +19,7 @@ from .cost_volume import CostVolumeModule
 
 __all__ = ["MonoRecModel", "CostVolumeModule", "MaskModule", "DepthModule", "ResnetEncoder"]
 
-# in half mode the cuDNN trunk runs in half as well (folded weights and activations): its NHWC outputs feed the conv engine
-# without casts (0.82 -> 0.71 ms at B=8); MONOREC_B200_TRUNK=cudnn_f32 keeps it in fp32
-TRUNK_CUDNN_F16 = os.environ.get("MONOREC_B200_TRUNK", "cudnn_f16").lower() != "cudnn_f32"
-TRUNK_FUSED = os.environ.get("MONOREC_B200_TRUNK_FUSED", "1") != "0"
-# the trunk's 512-channel level (never consumed, see ResnetEncoder._forward_folded) on first use; 0: always computed
-# the trunk's 3x3 / stride-2 stem pool on the library's kernel; 0: ATen (A/B measurements)
-STEM_POOL = os.environ.get("MONOREC_B200_STEM_POOL", "1") != "0"
-# MaskModule encoder: 2x2 max-pool and max over the frames in one pass over a level's output; 0: two kernels (A/B measurements)
-FUSED_POOL = os.environ.get("MONOREC_B200_FUSED_POOL", "1") != "0"
-TRUNK_LAZY_LEVEL4 = os.environ.get("MONOREC_B200_TRUNK_LAZY_LEVEL4", "1") != "0"
+_CUDNN_FUSED = hasattr(torch, "cudnn_convolution_relu") and hasattr(torch, "cudnn_convolution_add_relu")
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -153,11 +144,34 @@ class ResnetEncoder(nn.Module):
             self._fold_cache, self._fold_sig = f, sig
         return self._fold_cache
 
+    # cuDNN's fused epilogues where the build offers them (conv + bias + ReLU, conv + residual + bias + ReLU: the ~24
+    # element-wise add / clamp launches of the trunk disappear); the folded trunk also runs on the CPU, on F.conv2d
+    @staticmethod
+    def _conv_relu(t, w, bias, stride, padding):
+        if t.is_cuda and _CUDNN_FUSED:
+            return torch.cudnn_convolution_relu(t, w, bias, list(stride), list(padding), [1, 1], 1)
+        return F.conv2d(t, w, bias, stride=stride, padding=padding).relu_()
+
+    @staticmethod
+    def _conv_add_relu(t, w, bias, z):
+        if t.is_cuda and _CUDNN_FUSED:
+            return torch.cudnn_convolution_add_relu(t, w, z, 1.0, bias, [1, 1], [1, 1], [1, 1], 1)
+        return F.conv2d(t, w, bias, padding=1).add_(z).relu_()
+
+    def _run_blocks(self, x, blocks):
+        """The residual blocks of one trunk level, on the folded weights `blocks` (an entry of `_folded()["blocks"]`)."""
+        for (w1, b1), stride, (w2, b2), down in blocks:
+            idt = x if down is None else F.conv2d(x, down[0], down[1], stride=down[2])
+            out = self._conv_relu(x, w1, b1, tuple(stride), (1, 1))
+            x = self._conv_add_relu(out, w2, b2, idt)
+        return x
+
     def _forward_folded(self, input_image):
-        import torch.nn.functional as F
         e, f = self.encoder, self._folded()
         x = (input_image - 0.45) / 0.225
-        if TRUNK_CUDNN_F16 and C.MODE == "f16" and x.is_cuda:
+        # in half mode the trunk runs in half as well (folded weights and activations): its NHWC outputs feed the conv engine
+        # without casts (0.82 -> 0.71 ms at B=8)
+        if C.MODE == "f16" and x.is_cuda:
             if getattr(self, "_fold_half_sig", None) != self._fold_sig:
                 conv = lambda wb: (wb[0].half().contiguous(memory_format=torch.channels_last), wb[1].half())   # noqa: E731
                 self._fold_half = {"stem": conv(f["stem"]),
@@ -166,46 +180,23 @@ class ResnetEncoder(nn.Module):
                 self._fold_half_sig = self._fold_sig
             f = self._fold_half
             x = x.half()
-        # cuDNN's fused epilogues where the build offers them (conv + bias + ReLU, conv + residual + bias + ReLU: the ~24
-        # element-wise add / clamp launches of the trunk disappear); MONOREC_B200_TRUNK_FUSED=0 keeps separate ATen ops
-        fused = TRUNK_FUSED and x.is_cuda and hasattr(torch, "cudnn_convolution_relu") and hasattr(torch, "cudnn_convolution_add_relu")
-
-        def conv_relu(t, w, bias, stride, padding):
-            if fused:
-                return torch.cudnn_convolution_relu(t, w, bias, list(stride), list(padding), [1, 1], 1)
-            return F.conv2d(t, w, bias, stride=stride, padding=padding).relu_()
-
-        def conv_add_relu(t, w, bias, z):
-            if fused:
-                return torch.cudnn_convolution_add_relu(t, w, z, 1.0, bias, [1, 1], [1, 1], [1, 1], 1)
-            return F.conv2d(t, w, bias, padding=1).add_(z).relu_()
-        def run_blocks(x, blocks):
-            for (w1, b1), stride, (w2, b2), down in blocks:
-                idt = x if down is None else F.conv2d(x, down[0], down[1], stride=down[2])
-                out = conv_relu(x, w1, b1, tuple(stride), (1, 1))
-                x = conv_add_relu(out, w2, b2, idt)
-            return x
-        x = conv_relu(x, f["stem"][0], f["stem"][1], tuple(e.conv1.stride), tuple(e.conv1.padding))
+        x = self._conv_relu(x, f["stem"][0], f["stem"][1], tuple(e.conv1.stride), tuple(e.conv1.padding))
         feats = [x]
         mp = e.maxpool
-        if (STEM_POOL and x.is_cuda and x.dtype in (torch.float16, torch.float32) and x.shape[1] % 8 == 0 and
+        if (x.is_cuda and x.dtype in (torch.float16, torch.float32) and x.shape[1] % 8 == 0 and
                 x.permute(0, 2, 3, 1).is_contiguous() and isinstance(mp, nn.MaxPool2d) and mp.kernel_size == 3 and mp.stride == 2 and
                 mp.padding == 1 and mp.dilation == 1 and not mp.ceil_mode):
             x = C.maxpool3s2_channels_last(x)            # (ATen's channels-last max-pool: 75 us for this 33 MB tensor)
         else:
             x = mp(x)
         for blocks in f["blocks"][:3]:
-            x = run_blocks(x, blocks)
+            x = self._run_blocks(x, blocks)
             feats.append(x)
         # The 512-channel level (layer4, 23 % of the trunk's multiply-adds) has no consumer: the MaskModule reads levels 0-3
         # (monorec_model.py:372-380), the DepthModule levels 0-2 (:545), and nothing else in the reference touches
         # data_dict["image_features"].  It is computed when somebody asks for it.
-        if TRUNK_LAZY_LEVEL4:
-            last = f["blocks"][3]
-            self.features = _TrunkFeatures(feats, lambda t: run_blocks(t, last))
-        else:
-            feats.append(run_blocks(x, f["blocks"][3]))
-            self.features = feats
+        last = f["blocks"][3]
+        self.features = _TrunkFeatures(feats, lambda t: self._run_blocks(t, last))
         return self.features
 
     def forward(self, input_image):
@@ -316,7 +307,7 @@ class MaskModule(nn.Module):
             p[f"dec{i}"] = [C.upconv_layer(seq[0].conv, up_src[i]), _leaky(seq[1].conv, cat_src[i]),
                             _leaky(seq[2].conv, (seq[2].conv.in_channels,))]
         cls = self.classifier[0]
-        p["cls"] = C.PackedConv(cls.weight, cls.bias, (cls.in_channels,), act=C.ACT_SIGMOID, allow_tc=False)
+        p["cls"] = C.PackedConv(cls.weight, cls.bias, (cls.in_channels,), act=C.ACT_SIGMOID)
         return p
 
     def forward(self, data_dict):
@@ -337,7 +328,7 @@ class MaskModule(nn.Module):
         if not self.use_cv:
             x.zero_()
         cv_feats = []
-        fused_pool = FUSED_POOL and nF > 1 and H % 16 == 0 and W % 16 == 0   # (one pass writes the pooled tensor and the frame maximum)
+        fused_pool = nF > 1 and H % 16 == 0 and W % 16 == 0   # (one pass writes the pooled tensor and the frame maximum)
         for lvl in range(5):
             for layer in P[f"enc{lvl}"]:
                 x = layer([x])
@@ -421,7 +412,7 @@ class DepthModule(nn.Module):
         p["dec2"] = (C.refine_layer(self.dec[2][0].conv2d_t, (e[2], fc[1], d[1])), cr2(self.dec[2][1], (d[2],)))
         p["dec3"] = C.refine_layer(self.dec[3].conv2d_t, (e[1], fc[0], d[2]))
         p["dec4"] = (cr2(self.dec[4][0], (e[0], d[3])), _leaky(self.dec[4][2], (d[4],)))
-        p["heads"] = [C.PackedConv(s[1].weight, s[1].bias, (s[1].in_channels,), act=C.ACT_ABSTANH, allow_tc=False)
+        p["heads"] = [C.PackedConv(s[1].weight, s[1].bias, (s[1].in_channels,), act=C.ACT_ABSTANH)
                       for s in self.predictors]
         return p
 

@@ -248,7 +248,7 @@ def test_tc_filter_size_limits_of_the_halo_kernel():
     for dt in ("tf32", "f16"):
         for name in ("k3x9_halo_limit", "k7x3_halo_limit"):
             p = _plan(by_name[name], dt)
-            assert p["halo_shape"] == (0 if HALO_ENV == "0" or (dt == "f16" and os.environ.get("MONOREC_B200_TC_HALO_F16") == "0") else 1)
+            assert p["halo_shape"] == (0 if HALO_ENV == "0" else 1)
         for name in ("k1x10_tap_fallback", "k8x1_tap_fallback"):
             p = _plan(by_name[name], dt)
             assert p["halo_shape"] == 0 and p["kernel"] == C.TC_KERNEL_TAP

@@ -38,7 +38,7 @@ def test_conv_same_padding_matches_torch(cin, cout, kh, kw, sy, sx, H, W):
     assert _rel(_nchw(out.cpu()), ref) < TOL
 
 
-def test_concat_sources_upconv_and_refine():
+def test_concat_sources_upconv_and_refine_layer_fp32(fp32_mode):
     from monorec_b200 import conv as C
     from oracle import convnet_oracle as CO
     g = torch.Generator().manual_seed(3)
@@ -56,11 +56,14 @@ def test_concat_sources_upconv_and_refine():
     ref = CO.upconv(sd, "u", cat)
     out = C.conv2d(srcs, C.pack_conv_weight(sd["u.conv.weight"]).to(DEV), sd["u.conv.bias"].to(DEV), 2, 2, upsample2=True)
     assert out.shape[1:3] == (16, 32) and _rel(_nchw(out.cpu()), ref) < TOL
-    # Refine (ConvTranspose2d k4 s2 + LReLU + crop)
+    # Refine (ConvTranspose2d k4 s2 + LReLU + crop): four sub-pixel phases on the CUDA-core kernel (fp32 mode)
     sd = {"r.conv2d_t.weight": torch.randn(259, 48, 4, 4, generator=g) / 32, "r.conv2d_t.bias": torch.randn(48, generator=g)}
     ref = CO.refine(sd, "r", cat)
-    sub = {k: v.to(DEV) for k, v in C.pack_convT_k4s2(sd["r.conv2d_t.weight"]).items()}
-    out = C.conv_transpose_k4s2_crop(srcs, sub, sd["r.conv2d_t.bias"].to(DEV))
+    ct = torch.nn.ConvTranspose2d(259, 48, 4, stride=2)
+    with torch.no_grad():
+        ct.weight.copy_(sd["r.conv2d_t.weight"])
+        ct.bias.copy_(sd["r.conv2d_t.bias"])
+    out = C.refine_layer(ct.to(DEV), (96, 128, 35))(srcs)
     assert out.shape[1:3] == (16, 32) and _rel(_nchw(out.cpu()), ref) < TOL
 
 
@@ -333,7 +336,7 @@ def test_f16_conv_matches_torch(f16_mode, cin, cout, kh, kw, sy, sx, H, W):
     assert _rel(_nchw(out.float().cpu()), ref) < TOL_F16
 
 
-def test_f16_helpers_and_subpixel(f16_mode):
+def test_f16_helpers_subpixel_and_tc_head(f16_mode):
     from monorec_b200 import conv as C
     from oracle import convnet_oracle as CO
     g = torch.Generator().manual_seed(8)
@@ -357,7 +360,7 @@ def test_f16_helpers_and_subpixel(f16_mode):
     assert out.dtype == torch.float16 and _rel(_nchw(out.float().cpu()), ref) < TOL_F16
     head = torch.nn.Conv2d(32, 1, 3)
     refh = torch.abs(torch.tanh(CO.conv_same(x, head.weight.detach(), head.bias.detach())))
-    outh = C.PackedConv(head.weight.to(DEV), head.bias.to(DEV), (32,), act=C.ACT_ABSTANH, act_a=0.0, act_b=1.0, allow_tc=False)([xh], final=True)
+    outh = C.PackedConv(head.weight.to(DEV), head.bias.to(DEV), (32,), act=C.ACT_ABSTANH, act_a=0.0, act_b=1.0)([xh], final=True)
     assert outh.dtype == torch.float32 and _rel(_nchw(outh.cpu()), refh) < TOL_F16
 
 

@@ -195,18 +195,28 @@ def test_hires_config_small_batch():
 def test_tma_windows_and_global_gather_agree(B, F, H, W):
     """mr_cost_volume_fwd (TMA-staged windows) == mr_cost_volume_fwd_gather (taps from global memory): same formula, same
     validity; the two interpolation code paths may differ in the last bits only."""
+    from monorec_b200 import _lib
     from monorec_b200.cost_volume import CostVolumeModule
     from monorec_b200.synthetic import make_inputs, to_device
-    data = make_inputs(B, F, H, W, seed=55)
+    D, dev = 32, "cuda:0"
+    d = to_device(make_inputs(B, F, H, W, seed=55), dev)
+    lib = _lib.load()
+    m = CostVolumeModule()
+    cw = (_lib.c_float * 3)(*m.channel_weights)
+    stream = torch.cuda.current_stream().cuda_stream
+    proj = torch.empty(B, F, 3, 4, device=dev)
+    depths = torch.empty(D, device=dev)
+    _lib.check(lib.mr_projection_tables(d["keyframe_pose"].data_ptr(), d["keyframe_intrinsics"].data_ptr(),
+                                        _lib.ptr_array(d["poses"]), _lib.ptr_array(d["intrinsics"]), B, F, H, W,
+                                        proj.data_ptr(), depths.data_ptr(), D, 0.0025, 0.33, stream), "mr_projection_tables")
     outs = []
-    for tma in (True, False):
-        d = to_device(data, "cuda:0")
-        d["_cv_range"] = (0.0025, 0.33, 32)
-        m = CostVolumeModule()
-        m.tma_windows = tma
-        o = m(d)
+    for name in ("mr_cost_volume_fwd", "mr_cost_volume_fwd_gather"):
+        cv = torch.full((B, D, H, W), float("nan"), device=dev)
+        sfcv = torch.full((F, B, D, H, W), float("nan"), device=dev)
+        _lib.check(getattr(lib, name)(d["keyframe"].data_ptr(), _lib.ptr_array(d["frames"]), proj.data_ptr(), depths.data_ptr(),
+                                      cv.data_ptr(), sfcv.data_ptr(), B, F, D, H, W, float(m.alpha), cw, stream), name)
         torch.cuda.synchronize()
-        outs.append((o["cost_volume"].cpu(), [s.cpu() for s in o["single_frame_cvs"]]))
+        outs.append((cv.cpu(), list(sfcv.cpu())))
     for a, b in zip(outs[0][1], outs[1][1]):
         assert torch.equal((a == 0).all(1), (b == 0).all(1))   # same validity (a plane stack that is exactly 0)
         d = (a - b).abs()

@@ -37,20 +37,30 @@ def test_conv_desc_abi_matches_library():
     assert ctypes.sizeof(ConvDesc) == _lib.load().mr_sizeof_conv_desc()
 
 
-def test_convT_subkernels_reproduce_conv_transpose():
-    """The four sub-pixel 2x2 kernels of pack_convT_k4s2 == ConvTranspose2d(k4,s2) + centre crop (layers.py:380-400)."""
+def test_refine_and_upconv_phases_reproduce_reference_layers():
+    """The phase convolutions refine_layer and upconv_layer build (packed weights, pad, out_off, activation) reproduce
+    ConvTranspose2d(k4, s2) + LeakyReLU + centre crop (Refine, layers.py:380-400) and Upsample(x2) + pad(0,1,0,1) +
+    Conv2d(k2) (Upconv, :338-356)."""
     import torch.nn.functional as F
-    from monorec_b200.conv import pack_convT_k4s2
+    from monorec_b200 import conv as C
     g = torch.Generator().manual_seed(0)
-    x = torch.randn(1, 5, 6, 7, generator=g)
-    w = torch.randn(5, 4, 4, 4, generator=g)
-    ref = F.conv_transpose2d(x, w, stride=2)[:, :, 1:-1, 1:-1]
-    out = torch.zeros_like(ref)
-    for (py, px), sub in pack_convT_k4s2(w).items():          # sub: [2][2][Cin][Cout]
-        wk = sub.permute(3, 2, 0, 1)                           # (Cout, Cin, 2, 2) correlation kernel
-        xp = F.pad(x, (1 - px, px, 1 - py, py))
-        out[:, :, py::2, px::2] = F.conv2d(xp, wk)
-    assert torch.allclose(out, ref, atol=1e-5)
+    x = torch.randn(1, 8, 6, 7, generator=g)
+    convt, conv = torch.nn.ConvTranspose2d(8, 4, 4, stride=2), torch.nn.Conv2d(8, 4, 2)
+    with torch.no_grad():
+        for p in list(convt.parameters()) + list(conv.parameters()):
+            p.copy_(torch.randn(p.shape, generator=g))
+        refine = F.leaky_relu(F.conv_transpose2d(x, convt.weight, convt.bias, stride=2)[:, :, 1:-1, 1:-1], C.LEAKY_SLOPE)
+        upconv = F.conv2d(F.pad(F.interpolate(x, scale_factor=2, mode="nearest"), (0, 1, 0, 1)), conv.weight, conv.bias)
+    for layer, ref in ((C.refine_layer(convt, (8,)), refine), (C.upconv_layer(conv, (8,)), upconv)):
+        assert len(layer.subs) == 4
+        out = torch.full_like(ref, float("nan"))
+        for L in layer.subs:
+            assert L.out_step == (2, 2)
+            (pt, pl), (oy, ox) = L.pad, L.out_off
+            xp = F.pad(x, (pl, L.kw - 1 - pl, pt, L.kh - 1 - pt))         # pixels beyond the trailing border are zero
+            y = F.conv2d(xp, L.w32.permute(3, 2, 0, 1), L.bias)           # w32: [kh][kw][Cin][Cout]
+            out[:, :, oy::2, ox::2] = F.leaky_relu(y, L.act_a) if L.act == C.ACT_LEAKY else y
+        assert torch.allclose(out, ref, atol=1e-5)
 
 
 def test_unsupported_reference_options_raise():
@@ -95,7 +105,7 @@ def test_trunk_batchnorm_folding_matches_unfolded_eval():
     assert float((out2 - ref2).abs().max()) < 1e-4 and float((out2 - out[0]).abs().max()) > 0.5
 
 
-def test_tc_weight_packing_chunk_widths():
+def test_tc_weight_packing_follows_source_chunk_widths():
     """Packed tensor-core weights: [taps][n_pad][k_pad], every source padded to whole K chunks; half sources of <= 32
     channels use 32-channel chunks (64-byte swizzle rows; the library derives the chunk width from k_pad:
     include/monorec_b200.h)."""
@@ -103,21 +113,42 @@ def test_tc_weight_packing_chunk_widths():
     w = torch.randn(24, 32, 3, 3)
     wt, n_pad, k_pad = C.pack_tc_weight(w, (32,), half=False)
     assert wt.dtype == torch.float32 and wt.shape == (9, 32, 32) and (n_pad, k_pad) == (32, 32)
-    assert torch.equal(wt[4, :24, :], C._round_tf32(w[:, :, 1, 1])) and float(wt[:, 24:].abs().max()) == 0.0
-    wt, n_pad, k_pad = C.pack_tc_weight(w, (32,), half=True, allow_k32=True)
-    assert wt.dtype == torch.float16 and k_pad == (32 if C.K32 else 64) and wt.shape == (9, 32, k_pad)
-    wt, n_pad, k_pad = C.pack_tc_weight(w, (32,), half=True, allow_k32=False)
-    assert k_pad == 64 and float(wt[:, :, 32:].abs().max()) == 0.0
+    assert torch.equal(wt[4, :24, :], _round_tf32(w[:, :, 1, 1])) and float(wt[:, 24:].abs().max()) == 0.0
+    wt, n_pad, k_pad = C.pack_tc_weight(w, (32,), half=True)
+    assert wt.dtype == torch.float16 and k_pad == 32 and wt.shape == (9, 32, k_pad)
     w2 = torch.randn(48, 96, 3, 3)
     wt, n_pad, k_pad = C.pack_tc_weight(w2, (32, 64), half=True)          # a 64-channel source keeps 64-channel chunks
     assert (n_pad, k_pad) == (48, 128) and torch.equal(wt[0, :, 64:128], w2[:, 32:, 0, 0].half())
     assert float(wt[:, :, 32:64].abs().max()) == 0.0
     s1 = C.PackedConv(w, None, (32,), stride=(1, 1))
     s2 = C.PackedConv(w, None, (32,), stride=(2, 1))
-    assert s1.wtc(True)[2] == (32 if C.K32 else 64) and s2.wtc(True)[2] == (32 if C.K32 else 64)
+    assert s1.wtc(True)[2] == 32 and s2.wtc(True)[2] == 32
 
 
-def test_c_packer_matches_torch_restatement():
+def _round_tf32(w):
+    """Round-to-nearest onto the TF32 grid (10 explicit mantissa bits); the tensor core truncates the rest."""
+    bits = w.contiguous().view(torch.int32)
+    return ((bits + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+def _pack_tc_weight_torch(w, src_c, half):
+    """The layout of mr_pack_conv_weights written with torch ops: [kh*kw][n_pad][k_pad], every source padded to whole K
+    chunks (32 fp32 channels; 64 half channels, or 32 when every source has <= 32 channels)."""
+    Cout, Cin, kh, kw = w.shape
+    kc = (32 if all(c <= 32 for c in src_c) else 64) if half else 32
+    n_pad = ((Cout + 15) // 16) * 16
+    k_pad = sum(((c + kc - 1) // kc) * kc for c in src_c)
+    out = torch.zeros(kh * kw, n_pad, k_pad, device=w.device, dtype=torch.float32)
+    wt = w.detach().to(torch.float32).permute(2, 3, 0, 1).reshape(kh * kw, Cout, Cin)
+    ci = ko = 0
+    for c in src_c:
+        out[:, :Cout, ko:ko + c] = wt[:, :, ci:ci + c]
+        ci += c
+        ko += ((c + kc - 1) // kc) * kc
+    return (out.to(torch.float16).contiguous() if half else _round_tf32(out)), n_pad, k_pad
+
+
+def test_c_packer_matches_layout_restatement():
     """mr_pack_conv_weights (host-side C, include/monorec_b200.h) == the torch restatement of the layout, fp32/TF32 and half,
     one to three concatenated sources, ragged channel counts; padding rows and columns are zero."""
     from monorec_b200 import conv as C
@@ -126,7 +157,7 @@ def test_c_packer_matches_torch_restatement():
         w = torch.randn(cout, sum(src_c), kh, kw, generator=g)
         for half in (False, True):
             got, n_pad, k_pad = C.pack_tc_weight(w, src_c, half=half)
-            ref, n_ref, k_ref = C._pack_tc_weight_torch(w, src_c, half)
+            ref, n_ref, k_ref = _pack_tc_weight_torch(w, src_c, half)
             assert (n_pad, k_pad) == (n_ref, k_ref) and got.dtype == ref.dtype and torch.equal(got, ref), (cout, src_c, half)
 
 
@@ -183,27 +214,22 @@ def test_integration_builds_from_reference_eval_config(golden_dir):
         assert tuple(model.inv_depth_min_max) == (0.33, 0.0025)
 
 
-def test_trunk_unused_level_is_lazy_and_identical():
+def test_trunk_level4_is_lazy_and_matches_run_blocks():
     """The 512-channel trunk level has no consumer in the reference (monorec_model.py:372-380, :545 read levels 0-3): it is
     evaluated on first use.  Slices / indices the Mask and Depth modules use do not trigger it; index 4, iteration and
     concatenation do, with the same values as the eager evaluation."""
     import monorec_b200.model as M
     enc = M.ResnetEncoder(18, pretrained=False).eval()
     x = torch.rand(2, 3, 64, 128)
-    old = M.TRUNK_LAZY_LEVEL4
-    try:
-        with torch.no_grad():
-            M.TRUNK_LAZY_LEVEL4 = False
-            eager = enc(x)
-            M.TRUNK_LAZY_LEVEL4 = True
-            lazy = enc(x)
-        assert type(eager) is list and isinstance(lazy, M._TrunkFeatures) and len(lazy) == 5
+    with torch.no_grad():
+        lazy = enc(x)
+        assert isinstance(lazy, M._TrunkFeatures) and len(lazy) == 5
         assert len(lazy[:4]) == 4 and lazy[3].shape[1] == 256 and list.__getitem__(lazy, 4) is None      # not evaluated yet
-        assert torch.equal(lazy[4], eager[4]) and torch.equal(lazy[-1], eager[4])
-        with torch.no_grad():
-            lazy2 = enc(x)
-        assert all(torch.equal(a, b) for a, b in zip(lazy2, eager))                                        # iteration evaluates
-        lazy2.reset_tail()
-        assert list.__getitem__(lazy2, 4) is None and torch.equal((lazy2 + [])[4], eager[4])
-    finally:
-        M.TRUNK_LAZY_LEVEL4 = old
+        eager = lazy[:4] + [enc._run_blocks(lazy[3], enc._folded()["blocks"][3])]
+    assert list.__getitem__(lazy, 4) is None
+    assert torch.equal(lazy[4], eager[4]) and torch.equal(lazy[-1], eager[4])
+    with torch.no_grad():
+        lazy2 = enc(x)
+    assert all(torch.equal(a, b) for a, b in zip(lazy2, eager))                                            # iteration evaluates
+    lazy2.reset_tail()
+    assert list.__getitem__(lazy2, 4) is None and torch.equal((lazy2 + [])[4], eager[4])
