@@ -109,6 +109,28 @@ int mr_cost_volume_fwd_depthmap(const float* keyframe, const float* const* frame
                                 int B, int F, int D, int H, int W,
                                 float alpha, const float* chan_w, void* stream);
 
+/* Error modes of the cost volume: the per-pixel, per-channel difference that the 3x3 patch cost sums
+ * (monorec_model.py:227-243).  The numbers are the reference's use_ssim values. */
+#define MR_CV_SSIM 1      /* use_ssim == True: SSIM error of w + .5, k + .5 (layers.py:119-139); every other entry uses it */
+#define MR_CV_SSIM_L1 2   /* use_ssim == 2: 0.85 SSIM + 0.15 |w - k| */
+#define MR_CV_BOX_L1 3    /* any other truthy use_ssim: avg_pool2d(|w - k|, 3, 1, padding=1) */
+
+/* The cost volume with any error mode and either depth source:
+ *   depths        [D] plane depths as in mr_cost_volume_fwd, or NULL
+ *   pixel_depths  [B,D,H,W] per-pixel hypotheses as in mr_cost_volume_fwd_depthmap, or NULL; exactly one of the two is given
+ *   out_sfcv_nhwc NULL, or [F,B,H,W,D] as in mr_cost_volume_fwd_nhwc; nhwc_dtype MR_DT_F32 or MR_DT_F16 either way
+ *   matching      MR_CV_SSIM, MR_CV_SSIM_L1 or MR_CV_BOX_L1.  0 (use_ssim falsy: plain |w - k|) is not implemented and
+ *                 returns MR_ENOSUPPORT; any other value MR_EINVAL
+ *   centered      1: out_cv = 1 - 2 sum_f w_f sad_f / sum_f w_f (every other entry); 0: out_cv = sum_f w_f sad_f / sum_f w_f
+ *                 (not_center_cv, monorec_model.py:267-269).  Either way 0 where sum_f w_f == 0, and out_sfcv = (1 - 2 sad) valid.
+ * With MR_CV_SSIM and centered = 1 the results are those of mr_cost_volume_fwd / mr_cost_volume_fwd_depthmap bit for bit.
+ * Constraints as mr_cost_volume_fwd.  All arguments are checked before the first CUDA call. */
+int mr_cost_volume_fwd_matching(const float* keyframe, const float* const* frames, const float* proj,
+                                const float* depths, const float* pixel_depths, float* out_cv, float* out_sfcv,
+                                void* out_sfcv_nhwc, int nhwc_dtype,
+                                int B, int F, int D, int H, int W,
+                                float alpha, const float* chan_w, int matching, int centered, void* stream);
+
 /* Same path with HOST buffers (pinned or pageable): uploads the images and matrices, runs
  * mr_projection_tables + mr_cost_volume_fwd and downloads both volumes; batch elements are pipelined on
  * internal streams so copies overlap the kernel.  This is the end-to-end entry bench.py times as `e2e`.

@@ -30,6 +30,9 @@ SIGNATURES = {
                                         c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_void_p]),
     "mr_cost_volume_fwd_depthmap": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_void_p]),
+    "mr_cost_volume_fwd_matching": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_int,
+                                            c_int, c_void_p]),
     "mr_cost_volume_host_workspace": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
     "mr_cost_volume_host_sfcv_offset": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
     "mr_cost_volume_host": (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_float] * 3 + [c_void_p, c_longlong]),

@@ -11,6 +11,24 @@ from torch import nn
 from . import _lib
 
 
+# error modes of the kernel (include/monorec_b200.h MR_CV_*): the numbers are the reference's use_ssim values
+CV_SSIM, CV_SSIM_L1, CV_BOX_L1 = 1, 2, 3
+
+
+def cv_matching_mode(use_ssim):
+    """The cost volume's difference for the reference's use_ssim, chosen with the reference's own comparisons in its order
+    (monorec_model.py:227-243): falsy -> |w - k| (not implemented: NotImplementedError), == True -> SSIM, == 2 -> 0.85 SSIM
+    + 0.15 |w - k|, anything else -> the 3x3 box average of |w - k|.  So 1.0 is SSIM, 2.0 is SSIM + L1, and 3, 0.5 or "sad"
+    are the box average."""
+    if not use_ssim:
+        raise NotImplementedError("monorec_b200: use_ssim falsy (the plain |w - k| difference) is not implemented")
+    if use_ssim == True:  # noqa: E712  (the reference's comparison: True, 1 and 1.0 all select SSIM)
+        return CV_SSIM
+    if use_ssim == 2:
+        return CV_SSIM_L1
+    return CV_BOX_L1
+
+
 def _as_f32c(t):
     if t.dtype != torch.float32 or not t.is_contiguous():
         t = t.to(torch.float32).contiguous()
@@ -20,10 +38,11 @@ def _as_f32c(t):
 class CostVolumeModule(nn.Module):
     """Drop-in for the reference class of the same name (monorec_model.py:132-148 for the ctor).
 
-    Supported configuration = the one every shipped config uses (SURVEY.md §8a): use_ssim=True (1), patch_size=3,
-    sfcv_mult_mask=True, not_center_cv=False; use_mono / use_stereo select the frame lists exactly like the
-    reference (:160-167).  Other ablation switches raise NotImplementedError instead of silently running something
-    else.
+    Every shipped config uses use_ssim=True, patch_size=3, sfcv_mult_mask=True, not_center_cv=False (SURVEY.md §8a).
+    use_ssim also takes the reference's other truthy values (see cv_matching_mode) and not_center_cv=True stores the
+    uncentred fused volume, as the reference does.  use_mono / use_stereo select the frame lists exactly like the reference
+    (:160-167).  use_ssim falsy, patch_size != 3 and sfcv_mult_mask=False raise NotImplementedError instead of silently
+    running something else.
     """
 
     def __init__(self, use_mono=True, use_stereo=False, use_ssim=True, patch_size=3,
@@ -38,10 +57,9 @@ class CostVolumeModule(nn.Module):
         self.alpha = alpha
         self.not_center_cv = not_center_cv
         self.sfcv_mult_mask = sfcv_mult_mask
-        if not (use_ssim is True or use_ssim == 1) or isinstance(use_ssim, float):
-            raise NotImplementedError("monorec_b200: only use_ssim=True is implemented (reference default)")
-        if patch_size != 3 or not_center_cv or not sfcv_mult_mask:
-            raise NotImplementedError("monorec_b200: only patch_size=3, not_center_cv=False, sfcv_mult_mask=True")
+        self.matching = cv_matching_mode(use_ssim)
+        if patch_size != 3 or not sfcv_mult_mask:
+            raise NotImplementedError("monorec_b200: only patch_size=3, sfcv_mult_mask=True")
 
     def _gather(self, data_dict):
         frames, intrinsics, poses = [], [], []
@@ -105,7 +123,17 @@ class CostVolumeModule(nn.Module):
             fill_nhwc = nhwc is not None and D <= 32 and D % 8 == 0 \
                 and tuple(nhwc.shape) == (F * B, H, W, D) and nhwc.is_contiguous() \
                 and nhwc.dtype in (torch.float32, torch.float16)
-            if pixel_depths is not None:
+            if self.matching != CV_SSIM or self.not_center_cv:
+                # the reference's non-default error modes and the uncentred volume, on either depth source
+                _lib.check(lib.mr_cost_volume_fwd_matching(
+                    keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
+                    None if depths is None else depths.data_ptr(), None if pixel_depths is None else pixel_depths.data_ptr(),
+                    cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if fill_nhwc else None,
+                    1 if fill_nhwc and nhwc.dtype == torch.float16 else 0, B, F, D, H, W, float(self.alpha), cw,
+                    self.matching, 0 if self.not_center_cv else 1, stream), "mr_cost_volume_fwd_matching")
+                if fill_nhwc:
+                    data_dict["_sfcv_nhwc_filled"] = True
+            elif pixel_depths is not None:
                 # (one entry: it chooses TMA windows or the gather itself, like mr_cost_volume_fwd)
                 _lib.check(lib.mr_cost_volume_fwd_depthmap(
                     keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), pixel_depths.data_ptr(), cv.data_ptr(),

@@ -25,6 +25,9 @@
 //           launches whose frames TMA cannot address (W % 4 != 0, unaligned base) gather from global memory instead.
 //   CTA phase 2 (thread = pixel): view weight from max_d / sum_d exp(..), zeroing of invalid pixels, fusion over
 //           frames from the L2-hot single-frame volumes.
+// Template parameters: the depth source (plane table / per-pixel cv_depths), the error mode of stage 2 (SSIM, SSIM + L1 or
+// the 3x3 box of L1: the reference's use_ssim, monorec_model.py:227-243) and the centring of the fused volume
+// (not_center_cv, :267-269).
 // Keyframe-only terms (9 mu_y, 81 (sigma_y + C2)) are hoisted into a smem table per tile; pixels whose reprojection leaves
 // the source for any plane (valid_f = 0) are found by a projection pre-pass over the two extreme planes (the samples of
 // one pixel lie on a line, monotone in depth, so the extremes decide) and whole row ranges / frames of a tile are skipped.
@@ -93,15 +96,20 @@ struct SmemLayout {
     int total;
 };
 
-// pix: the per-pixel depth source (cv_depths) appends its two depth tables; the plane layout is unchanged
-__host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_tma, bool pix = false) {
+constexpr int kXbWarpFloats = 2 * 3 * kRowStride;  // a warp's two warped-row buffers
+constexpr int kLSlotFloats = 3 * 64;              // kErrSsimL1: a warp's carried L1 terms, three float2 per lane (ssim_row)
+
+// pix: the per-pixel depth source (cv_depths) appends its two depth tables; the plane layout is unchanged.
+// err: the error mode (MR_CV_*).  MR_CV_SSIM_L1 warps keep kLSlotFloats behind their row buffers; MR_CV_BOX_L1 reads no
+// hoisted SSIM table, so its cst region is empty
+__host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_tma, bool pix = false, int err = MR_CV_SSIM) {
     SmemLayout L;
     int off = 0;
     auto take = [&](int bytes, int align) { off = (off + align - 1) / align * align; int o = off; off += bytes; return o; };
     L.win = take(use_tma ? kBuf * kWinFloats * 4 : 0, 128);
     L.ytile = take(3 * (TH + 4) * kRowStride * 4, 16);
-    L.cst = take(3 * (TH + 2) * kTileCols * 8, 16);
-    L.xbuf = take(kWarps * 2 * 3 * kRowStride * 4, 16);
+    L.cst = take(err == MR_CV_BOX_L1 ? 0 : 3 * (TH + 2) * kTileCols * 8, 16);
+    L.xbuf = take(kWarps * (kXbWarpFloats + (err == MR_CV_SSIM_L1 ? kLSlotFloats : 0)) * 4, 16);
     L.pjs = take(F * 12 * 4, 16);
     L.zs = take(((D + 3) / 4) * 16, 16);
     L.vmask = take(F * TH * kTileCols, 16);
@@ -209,6 +217,10 @@ __device__ __forceinline__ float4 lds128(uint32_t a) {
 template <int OFF>
 __device__ __forceinline__ void sts32(uint32_t a, float v) {
     asm volatile("st.shared.f32 [%0+%1], %2;" ::"r"(a), "n"(OFF), "f"(v) : "memory");
+}
+template <int OFF>
+__device__ __forceinline__ void sts64(uint32_t a, float2 v) {
+    asm volatile("st.shared.v2.f32 [%0+%1], {%2, %3};" ::"r"(a), "n"(OFF), "f"(v.x), "f"(v.y) : "memory");
 }
 
 constexpr int kXbBytes = 3 * kRowStride * 4;      // one warped-row buffer (3 channels)
@@ -409,15 +421,23 @@ __device__ __forceinline__ void warp_row_finish(const Taps& t, const uint32_t xw
 }
 
 // ---- stage 2 of the march: SSIM + patch cost of one row; lane owns buffer columns 2l, 2l+1 (a pair) ---------------------
+// Error modes: the per-pixel, per-channel difference that the 3x3 patch cost sums (monorec_model.py:227-243, chosen by
+// use_ssim; the values are the C ABI's MR_CV_*).  All three have the footprint of a 3x3 box around the pixel, so the tile,
+// its 2-px ring and the validity rule are the same for every mode.
+constexpr int kErrSsim = MR_CV_SSIM;      // SSIM error of w + .5, k + .5 (layers.py:119-137)
+constexpr int kErrSsimL1 = MR_CV_SSIM_L1; // 0.85 SSIM + 0.15 |w - k|
+constexpr int kErrBoxL1 = MR_CV_BOX_L1;   // avg_pool2d(|w - k|, 3, 1, padding=1): the 3x3 box sum of |w - k| / 9
+
 struct Stage2Ctx {
-    float2 cw0, cw1, cw2;    // channel weights / 9
+    float2 cw0, cw1, cw2;    // channel weights / 9 (kErrBoxL1: times 1/9, the box average)
     int pairflag;            // 1: both columns of this lane are output pixels and W is even (one 8-byte store)
     bool st0, st1;           // otherwise: column 2l / 2l+1 is an output pixel (one 4-byte store each)
     uint64_t pol_keep;
 };
 
 // rolling state: horizontal 3-sums of X, X^2, XY per channel for the last rows, indexed by (row step mod 3) so that no
-// register moves are needed
+// register moves are needed.  kErrBoxL1 keeps horizontal 3-sums of |X - Y| instead.
+template <int ERR>
 struct Stage2State {
     float2 hs1[3][3], hsx[3][3], hsy[3][3], hE[3];
     __device__ __forceinline__ void clear() {
@@ -429,15 +449,51 @@ struct Stage2State {
         }
     }
 };
+template <>
+struct Stage2State<kErrBoxL1> {
+    float2 hd[3][3], hE[3];
+    __device__ __forceinline__ void clear() {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            hE[i] = bc2(0.f);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) hd[i][c] = bc2(0.f);
+        }
+    }
+};
+
+// Patch cost of one row step, common to every error mode: E is the channel-weighted error of the lane's two columns in the
+// row whose error was just finished; its horizontal 3-sum joins the two rows before it in hE (rolling like Stage2State).
+template <int P>
+__device__ __forceinline__ void patch_cost_row(float2 (&hE)[3], const Stage2Ctx& c, const float2 E, float* out,
+                                               const bool store) {
+    constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
+    const float eL = __shfl_up_sync(0xffffffffu, E.y, 1);
+    const float eR = __shfl_down_sync(0xffffffffu, E.x, 1);
+    const float mid = E.x + E.y;
+    const float2 hEc = make_float2(eL + mid, mid + eR);
+    // single-frame volume 1 - 2 sad (monorec_model.py:251) straight to HBM; the validity mask is applied by the
+    // per-pixel phase (which zeroes invalid pixels) once all planes are known
+    const float2 sv = make_float2(fmaf(-2.0f, (hE[P1].x + hE[P2].x) + hEc.x, 1.0f),
+                                  fmaf(-2.0f, (hE[P1].y + hE[P2].y) + hEc.y, 1.0f));
+    // predicated stores (no divergent branch in the row loop): the lane's pair as one 8-byte store, or its single column
+    if (store && c.pairflag) st_hint_f2(out, sv, c.pol_keep);
+    if (store && c.st0) st_hint_f1(out, sv.x, c.pol_keep);
+    if (store && c.st1) st_hint_f1(out + 1, sv.y, c.pol_keep);
+    hE[P] = hEc;
+}
 
 // One row step: horizontal sums of the new warped row, SSIM error of the row above it (windows complete from the third
 // row of a unit on; earlier rows produce finite throw-away values from the zeroed state: 9 sxx >= s^2 for partial
 // windows too), patch cost of the row above that.  `store` is warp-uniform (false for the first four rows of a unit).
 //   xr: shared address of the warped row (this lane's columns 2l-1..2l+2); yr: keyframe tile row (+0.5), same columns;
 //   cr: hoisted (Y, Y, Sg, Sg) table row of the SSIM row; out: single-frame volume, output row of this step.
-template <int P>
-__device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
-                                         const uint32_t cr, float* out, const bool store) {
+// ERR: kErrSsim or kErrSsimL1 (kErrBoxL1 is box_l1_row below).  The row buffer and the keyframe tile both hold values
+// + 0.5, so the |X - Y| of kErrSsimL1 and kErrBoxL1 is |(w + .5) - (k + .5)|: it differs from the reference's |w - k| by the
+// rounding of the two additions (of order 1e-7).
+template <int P, int ERR>
+__device__ __forceinline__ void ssim_row(Stage2State<ERR>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
+                                         const uint32_t cr, float* out, const bool store, const uint32_t xb) {
     constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
     float2 xl[3], xrr[3], yl[3], yrr[3];
     float4 k4[3];
@@ -451,6 +507,7 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
     // horizontal 3-sums of X, X^2, XY: the middle pair (columns 2l, 2l+1) is shared by both columns of the lane, and every
     // product is folded into an FFMA of its sum
     float2 h1[3], hx[3], hy[3];
+    float2 L;   // kErrSsimL1: sum_c w_c |X - Y|_c of columns 2l, 2l+1, formed channel by channel while their values are loaded
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
         const float2 l = xl[ch], r = xrr[ch], ly = yl[ch], ry = yrr[ch];
@@ -458,6 +515,17 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
         h1[ch] = make_float2(l.x + m1, m1 + r.y);
         hx[ch] = make_float2(fmaf(l.x, l.x, mx), fmaf(r.y, r.y, mx));
         hy[ch] = make_float2(fmaf(l.x, ly.x, my), fmaf(r.y, ry.y, my));
+        if constexpr (ERR == kErrSsimL1) {
+            const float2 w = ch == 0 ? c.cw0 : ch == 1 ? c.cw1 : c.cw2;
+            const float2 d = make_float2(fabsf(l.y - ly.y), fabsf(r.x - ry.x));
+            L = ch == 0 ? make_float2(w.x * d.x, w.y * d.y) : make_float2(fmaf(w.x, d.x, L.x), fmaf(w.y, d.y, L.y));
+        }
+    }
+    if constexpr (ERR == kErrSsimL1) {
+        // kErrSsimL1: the row's 0.15 L waits one step in the lane's shared memory slot P behind the warp's row buffers,
+        // until this row's SSIM is finished.  (Carried in registers, or in one slot that is read before it is rewritten,
+        // it pushed the per-pixel gather march into local memory.)
+        sts64<2 * kXbBytes + 256 * P>(xb, make_float2(0.15f * L.x, 0.15f * L.y));
     }
     float e[3][2];
 #pragma unroll
@@ -481,23 +549,57 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
             e[ch][k] = __saturatef(fmaf(n1h * n2, fast_rcp(d1 * d2), 0.5f));
         }
     }
-    const float2 E = make_float2(fmaf(c.cw2.x, e[2][0], fmaf(c.cw1.x, e[1][0], c.cw0.x * e[0][0])),
-                                 fmaf(c.cw2.y, e[2][1], fmaf(c.cw1.y, e[1][1], c.cw0.y * e[0][1])));
-    const float eL = __shfl_up_sync(0xffffffffu, E.y, 1);
-    const float eR = __shfl_down_sync(0xffffffffu, E.x, 1);
-    const float mid = E.x + E.y;
-    const float2 hEc = make_float2(eL + mid, mid + eR);
-    // single-frame volume 1 - 2 sad (monorec_model.py:251) straight to HBM; the validity mask is applied by the
-    // per-pixel phase (which zeroes invalid pixels) once all planes are known
-    const float2 sv = make_float2(fmaf(-2.0f, (st.hE[P1].x + st.hE[P2].x) + hEc.x, 1.0f),
-                                  fmaf(-2.0f, (st.hE[P1].y + st.hE[P2].y) + hEc.y, 1.0f));
-    // predicated stores (no divergent branch in the row loop): the lane's pair as one 8-byte store, or its single column
-    if (store && c.pairflag) st_hint_f2(out, sv, c.pol_keep);
-    if (store && c.st0) st_hint_f1(out, sv.x, c.pol_keep);
-    if (store && c.st1) st_hint_f1(out + 1, sv.y, c.pol_keep);
-    st.hE[P] = hEc;
+    float2 E;
+    if constexpr (ERR == kErrSsimL1) {
+        // 0.85 SSIM + 0.15 |X - Y| per channel (monorec_model.py:237-241), channel-weighted as sums of their own; the L1
+        // sum of the SSIM row is the one the previous step stored
+        const float2 Lp = lds64<2 * kXbBytes + 256 * P2>(xb);
+        E = make_float2(fmaf(0.85f, fmaf(c.cw2.x, e[2][0], fmaf(c.cw1.x, e[1][0], c.cw0.x * e[0][0])), Lp.x),
+                        fmaf(0.85f, fmaf(c.cw2.y, e[2][1], fmaf(c.cw1.y, e[1][1], c.cw0.y * e[0][1])), Lp.y));
+    } else {
+        E = make_float2(fmaf(c.cw2.x, e[2][0], fmaf(c.cw1.x, e[1][0], c.cw0.x * e[0][0])),
+                        fmaf(c.cw2.y, e[2][1], fmaf(c.cw1.y, e[1][1], c.cw0.y * e[0][1])));
+    }
+    patch_cost_row<P>(st.hE, c, E, out, store);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) { st.hs1[P][ch] = h1[ch]; st.hsx[P][ch] = hx[ch]; st.hsy[P][ch] = hy[ch]; }
+}
+
+// kErrBoxL1: horizontal 3-sums of |X - Y| of the new row, their vertical 3-sum over the rolling rows (the 3x3 box of the
+// row above, at the step where the SSIM modes finish that row's SSIM), patch cost of the row above that
+template <int P>
+__device__ __forceinline__ void box_l1_row(Stage2State<kErrBoxL1>& st, const Stage2Ctx& c, const uint32_t xr,
+                                           const uint32_t yr, float* out, const bool store) {
+    constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
+    float2 xl[3], xrr[3], yl[3], yrr[3];
+    xl[0] = lds64<0>(xr);                  xrr[0] = lds64<8>(xr);
+    xl[1] = lds64<kRowStride * 4>(xr);     xrr[1] = lds64<kRowStride * 4 + 8>(xr);
+    xl[2] = lds64<2 * kRowStride * 4>(xr); xrr[2] = lds64<2 * kRowStride * 4 + 8>(xr);
+    yl[0] = lds64<0>(yr);                  yrr[0] = lds64<8>(yr);
+    yl[1] = lds64<kRowStride * 4>(yr);     yrr[1] = lds64<kRowStride * 4 + 8>(yr);
+    yl[2] = lds64<2 * kRowStride * 4>(yr); yrr[2] = lds64<2 * kRowStride * 4 + 8>(yr);
+    float2 hd[3], v[3];
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        const float2 l = xl[ch], r = xrr[ch], ly = yl[ch], ry = yrr[ch];
+        const float m = fabsf(l.y - ly.y) + fabsf(r.x - ry.x);
+        hd[ch] = make_float2(fabsf(l.x - ly.x) + m, m + fabsf(r.y - ry.y));
+        v[ch] = make_float2((st.hd[P1][ch].x + st.hd[P2][ch].x) + hd[ch].x, (st.hd[P1][ch].y + st.hd[P2][ch].y) + hd[ch].y);
+    }
+    // (the box's 1/9 is folded into the channel weights)
+    const float2 E = make_float2(fmaf(c.cw2.x, v[2].x, fmaf(c.cw1.x, v[1].x, c.cw0.x * v[0].x)),
+                                 fmaf(c.cw2.y, v[2].y, fmaf(c.cw1.y, v[1].y, c.cw0.y * v[0].y)));
+    patch_cost_row<P>(st.hE, c, E, out, store);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) st.hd[P][ch] = hd[ch];
+}
+
+// xb: the lane's address in the warp's first row buffer (xr without the buffer toggle)
+template <int P, int ERR>
+__device__ __forceinline__ void stage2_row(Stage2State<ERR>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
+                                           const uint32_t cr, float* out, const bool store, const uint32_t xb) {
+    if constexpr (ERR == kErrBoxL1) box_l1_row<P>(st, c, xr, yr, out, store);
+    else ssim_row<P, ERR>(st, c, xr, yr, cr, out, store, xb);
 }
 
 // The march of one unit over tile rows rlo-2 .. rhi+2 (nsteps = rhi - rlo + 5 >= 5 rows).  Stage 1 of the next row is
@@ -506,12 +608,18 @@ __device__ __forceinline__ void ssim_row(Stage2State& st, const Stage2Ctx& c, co
 //   xb: shared address of this warp's two row buffers; yr / cr: keyframe row rlo-2 / table row rlo-2 (lane columns);
 //   out: single-frame volume at output row rlo - 4 (advanced every step, stored from the fifth step on); wstride = W
 //   PIX: per-pixel depths, read from image row v0 (= fv0) on; each row's depths are loaded one row step before they are used
-template <int MODE, bool PIX = false>
+//   ERR: the error mode of stage 2
+template <int MODE, bool PIX, int ERR>
 __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx& c2, const uint32_t xb, const int lane,
                                            const float fv0, const int nsteps, uint32_t yr, uint32_t cr, float* out,
                                            const int wstride, const int v0 = 0) {
-    Stage2State st;
+    Stage2State<ERR> st;
     st.clear();
+    if constexpr (ERR == kErrSsimL1) {   // the L1 slots start at 0 like st
+        sts64<2 * kXbBytes>(xb + 8 * lane, bc2(0.f));
+        sts64<2 * kXbBytes + 256>(xb + 8 * lane, bc2(0.f));
+        sts64<2 * kXbBytes + 512>(xb + 8 * lane, bc2(0.f));
+    }
     float fv = fv0;
     uint32_t off = 0;                      // byte offset of the row buffer stage 2 reads next
     const uint32_t xw = xb + 4 * (lane + 1), xr = xb + 8 * lane;
@@ -546,12 +654,15 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
         // stage 1 of row t+1 completes before stage 2 of row t: measured faster than keeping the taps in flight across
         // stage 2 (1.07 against 1.12 ms)
         warp_row_finish(tp, xw + (kXbBytes - off));
-        ssim_row<decltype(tag)::value>(st, c2, xr + off, yr, cr, out, done >= 4);
+        stage2_row<decltype(tag)::value, ERR>(st, c2, xr + off, yr, cr, out, done >= 4, xr);
         __syncwarp();
         off = kXbBytes - off;
         yr += kYRowBytes;
         cr += kCRowBytes;
-        out += wstride;
+        // (kErrSsimL1: the stride as an unsigned step, whose high word is the constant 0: the signed step's high word held a
+        // register across the loop, and the per-pixel gather march spilled it)
+        if constexpr (ERR == kErrSsimL1) out += (size_t)(uint32_t)wstride;
+        else out += wstride;
         ++done;
     };
     using I0 = std::integral_constant<int, 0>;
@@ -562,7 +673,7 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
         if (t + 1 >= 0) both(I1{});
         both(I2{});
     }
-    ssim_row<0>(st, c2, xr + off, yr, cr, out, true);
+    stage2_row<0, ERR>(st, c2, xr + off, yr, cr, out, true, xr);
     __syncwarp();
 }
 
@@ -570,6 +681,8 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
 //      cv = sum_f w_f (1 - 2 sad_f) / sum_f w_f, 0 where sum_f w_f == 0 (:262-269).  T lanes share a pixel, each with a chunk of
 //      kChunk planes in registers (T = 1 for D <= 32, 2 for D <= 64, 4 for D <= 128): every (L2-hot) single-frame value is
 //      read back exactly once; max / sum over the planes are combined across the T lanes by shuffles.
+//      CENTER = false (not_center_cv, :267-269) stores the fused sad sum_f w_f sad_f / sum_f w_f = (1 - cv) / 2 instead,
+//      still 0 where sum_f w_f == 0.
 struct PixelPhase {
     float* cv;
     float* sfcv;
@@ -581,7 +694,7 @@ struct PixelPhase {
     uint64_t pol_stream;
 };
 
-template <int T>
+template <int T, bool CENTER>
 __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
     constexpr int kSlots = 32 / T;                       // pixels per warp iteration
     // the thread index is read again here (volatile: not merged with the kernel's own read) instead of being kept live in a
@@ -695,19 +808,27 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
         if (!own) continue;
         const float inv = (wsum == 0.f) ? 0.f : 1.0f / wsum;
         char* q = cv_out;
+        if constexpr (CENTER) {
 #pragma unroll
-        for (int j = 0; j < kChunk; ++j, q += pstride)
-            if (D == T * kChunk || d_lo + j < D) st_hint_f1(reinterpret_cast<float*>(q), acc[j] * inv, c.pol_stream);
+            for (int j = 0; j < kChunk; ++j, q += pstride)
+                if (D == T * kChunk || d_lo + j < D) st_hint_f1(reinterpret_cast<float*>(q), acc[j] * inv, c.pol_stream);
+        } else {
+            const float h = (wsum == 0.f) ? 0.f : 0.5f;
+#pragma unroll
+            for (int j = 0; j < kChunk; ++j, q += pstride)
+                if (D == T * kChunk || d_lo + j < D) st_hint_f1(reinterpret_cast<float*>(q), fmaf(-h, acc[j] * inv, h), c.pol_stream);
+        }
     }
 }
 
 // PIX selects the depth source: false = one depth per plane (a.depths = zs[D], the default linspace planes), true = one depth
-// per plane and pixel (a.depths = cv_depths [B,D,H,W]).
-template <bool PIX>
+// per plane and pixel (a.depths = cv_depths [B,D,H,W]).  ERR is the error mode of stage 2 (use_ssim), CENTER false stores the
+// uncentred fused volume (not_center_cv).
+template <bool PIX, int ERR, bool CENTER>
 __global__ void __launch_bounds__(kThreads, kMinBlocks)
 cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     extern __shared__ __align__(128) unsigned char smem[];
-    const SmemLayout L = make_layout(a.D, a.TH, a.F, a.use_tma, PIX);
+    const SmemLayout L = make_layout(a.D, a.TH, a.F, a.use_tma, PIX, ERR);
     float* win = reinterpret_cast<float*>(smem + L.win);
     float* ytile = reinterpret_cast<float*>(smem + L.ytile);
     float* cst = reinterpret_cast<float*>(smem + L.cst);
@@ -733,7 +854,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     const int v0 = blockIdx.y * TH;            // image row of tile row 0
     const size_t plane = (size_t)H * W;
     const int planei = H * W;
-    float* xbuf = reinterpret_cast<float*>(smem + L.xbuf) + warp * 2 * 3 * kRowStride;
+    float* xbuf = reinterpret_cast<float*>(smem + L.xbuf) + warp * (kXbWarpFloats + (ERR == kErrSsimL1 ? kLSlotFloats : 0));
 
     // ---- keyframe tile (+0.5, monorec_model.py:232) and hoisted SSIM terms -------------------------------------
     const float* key = a.key + (size_t)b * 3 * plane;
@@ -809,8 +930,8 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     }
     __syncthreads();
     // table entry for the column pair (2j, 2j+1) of e-row er, channel ch: (Y[2j], Y[2j+1], Sg[2j], Sg[2j+1]) with
-    // Y = 9 mu_y = sum y, Sg = 81 (sigma_y + C2) = 9 sum y^2 - Y^2 + 81 C2
-    for (int line = warp; line < 3 * (TH + 2); line += kWarps) {      // line = e-row * 3 + channel
+    // Y = 9 mu_y = sum y, Sg = 81 (sigma_y + C2) = 9 sum y^2 - Y^2 + 81 C2 (kErrBoxL1 reads no table)
+    for (int line = warp; line < (ERR == kErrBoxL1 ? 0 : 3 * (TH + 2)); line += kWarps) {      // line = e-row * 3 + channel
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
             const int bc = lane + 32 * k;
@@ -1004,7 +1125,11 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
 
     // ---- march over the F*D (frame, plane) units; no CTA-wide barrier in here ------------------------------------
     Stage2Ctx c2;
-    c2.cw0 = bc2(a.cw0); c2.cw1 = bc2(a.cw1); c2.cw2 = bc2(a.cw2);
+    if constexpr (ERR != kErrBoxL1) {
+        c2.cw0 = bc2(a.cw0); c2.cw1 = bc2(a.cw1); c2.cw2 = bc2(a.cw2);
+    } else {
+        c2.cw0 = bc2(a.cw0 / 9.0f); c2.cw1 = bc2(a.cw1 / 9.0f); c2.cw2 = bc2(a.cw2 / 9.0f);
+    }
     c2.pairflag = (st0 && st1 && ((W & 1) == 0)) ? 1 : 0;
     c2.st0 = st0 && !c2.pairflag; c2.st1 = st1 && !c2.pairflag; c2.pol_keep = pol_keep;
     Stage1Ctx c1;
@@ -1050,10 +1175,10 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             if (uflag[unit] & 2) {
                 // tap address = wb + 4 ((bits(ty) - kMagicBits - wy0) kPitch + bits(tx) - kMagicBits - wx0), mod 2^32
                 c1.kaddr = wb - 4u * ((uint32_t)(kMagicBits + gi.wy0) * kPitch + (uint32_t)(kMagicBits + gi.wx0));
-                march_unit<0, PIX>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
+                march_unit<0, PIX, ERR>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
             } else {
                 c1.kaddr = wb - 4u * ((uint32_t)(int)gi.wy0 * kPitch + (uint32_t)(int)gi.wx0);
-                march_unit<1, PIX>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
+                march_unit<1, PIX, ERR>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
             }
             // hand the buffer on: the last unit of the window re-arms it with the window after next
             if (lane == 0) {
@@ -1071,7 +1196,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             __syncwarp();
         } else {
             c1.img = a.frames[f] + (size_t)b * 3 * plane;
-            march_unit<2, PIX>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
+            march_unit<2, PIX, ERR>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
         }
     }
     __syncthreads();  // the marching warps' global stores are visible to the whole CTA from here on
@@ -1086,9 +1211,9 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     // exp(-alpha (sad - min sad)^2) with sad = (1 - sv) / 2 is ex2(-(k (max sv - sv))^2), k = sqrt(alpha log2(e)) / 2
     pp.kq = 0.5f * sqrtf(a.alpha * 1.4426950408889634f);
     pp.pol_stream = pol_stream;
-    if (D <= kChunk) pixel_phase<1>(pp);
-    else if (D <= 2 * kChunk) pixel_phase<2>(pp);
-    else pixel_phase<4>(pp);
+    if (D <= kChunk) pixel_phase<1, CENTER>(pp);
+    else if (D <= 2 * kChunk) pixel_phase<2, CENTER>(pp);
+    else pixel_phase<4, CENTER>(pp);
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -1168,23 +1293,37 @@ __global__ void projection_tables_kernel(const float* kf_pose, const float* kf_K
     }
 }
 
-int pick_tile_rows(int D, int F, int use_tma, bool pix) {
+int pick_tile_rows(int D, int F, int use_tma, bool pix, int err) {
     const int limit = 227 * 1024;
     for (int th = kTileRows; th >= 2; th >>= 1)
-        if (make_layout(D, th, F, use_tma, pix).total <= limit) return th;
+        if (make_layout(D, th, F, use_tma, pix, err).total <= limit) return th;
     return 0;
 }
 
-template <bool PIX>
+template <bool PIX, int ERR, bool CENTER>
 int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
     static int smem_set = 0;   // the attribute is per function and per device context; setting it again is harmless
     if (smem_set < smem) {
-        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX, ERR, CENTER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     227 * 1024));
         smem_set = 227 * 1024;
     }
-    cost_volume_kernel<PIX><<<grid, kThreads, smem, stream>>>(a, maps);
+    cost_volume_kernel<PIX, ERR, CENTER><<<grid, kThreads, smem, stream>>>(a, maps);
     MR_LAUNCH_CHECK("cost_volume_kernel");
     return MR_OK;
+}
+
+// the instantiation for (error mode, centring); matching was checked by the caller
+template <bool PIX>
+int launch_variant(int matching, int centered, dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
+    if (matching == kErrSsimL1)
+        return centered ? launch_kernel<PIX, kErrSsimL1, true>(grid, smem, stream, a, maps)
+                        : launch_kernel<PIX, kErrSsimL1, false>(grid, smem, stream, a, maps);
+    if (matching == kErrBoxL1)
+        return centered ? launch_kernel<PIX, kErrBoxL1, true>(grid, smem, stream, a, maps)
+                        : launch_kernel<PIX, kErrBoxL1, false>(grid, smem, stream, a, maps);
+    return centered ? launch_kernel<PIX, kErrSsim, true>(grid, smem, stream, a, maps)
+                    : launch_kernel<PIX, kErrSsim, false>(grid, smem, stream, a, maps);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1229,13 +1368,16 @@ extern "C" int mr_projection_tables(const float* keyframe_pose, const float* key
 int mr::launch_cost_volume(const float* keyframe, const float* const* frames, const float* proj,
                            const float* depths, float* out_cv, float* out_sfcv, int B, int F, int D, int H, int W,
                            float alpha, const float* chan_w, int b_begin, int b_count, int gather_only,
-                           cudaStream_t stream, void* sf_nhwc, int sf_nhwc_dtype, int per_pixel_depths) {
+                           cudaStream_t stream, void* sf_nhwc, int sf_nhwc_dtype, int per_pixel_depths, int matching,
+                           int centered) {
     MR_REQUIRE(keyframe && frames && proj && depths && out_cv && out_sfcv, "mr_cost_volume_fwd: null pointer");
     MR_REQUIRE(b_begin >= 0 && b_count >= 1 && b_begin + b_count <= B, "mr_cost_volume_fwd: bad batch range");
     MR_REQUIRE(B >= 1 && B <= 21845, "mr_cost_volume_fwd: batch %d out of range", B);
     MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "mr_cost_volume_fwd: 1 <= F <= %d required (got %d)", MR_MAX_FRAMES, F);
     MR_REQUIRE(D >= 2 && D <= 128, "mr_cost_volume_fwd: 2 <= D <= 128 required (got %d)", D);
     MR_REQUIRE(H >= 5 && W >= 5 && H <= 16384 && W <= 16384, "mr_cost_volume_fwd: image size %dx%d out of range", H, W);
+    MR_REQUIRE(matching == MR_CV_SSIM || matching == MR_CV_SSIM_L1 || matching == MR_CV_BOX_L1,
+               "mr_cost_volume_fwd: unknown matching %d", matching);
     CvArgs a{};
     a.key = keyframe;
     for (int f = 0; f < F; ++f) {
@@ -1272,16 +1414,17 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
         }
     }
     const bool pix = per_pixel_depths != 0;
-    a.TH = pick_tile_rows(D, F, a.use_tma, pix);
+    a.TH = pick_tile_rows(D, F, a.use_tma, pix, matching);
     MR_REQUIRE(a.TH > 0, "mr_cost_volume_fwd: no tile height fits shared memory for D=%d F=%d", D, F);
     a.alpha = alpha;
     a.inv_dm1 = (float)(1.0 / (double)(D - 1));
     const float def_w[3] = {5.f / 32.f, 16.f / 32.f, 11.f / 32.f};  // monorec_model.py:133
     const float* cw = chan_w ? chan_w : def_w;
     a.cw0 = cw[0] / 9.f; a.cw1 = cw[1] / 9.f; a.cw2 = cw[2] / 9.f;  // monorec_model.py:141 (weights / patch_size^2)
-    const SmemLayout L = make_layout(D, a.TH, F, a.use_tma, pix);
+    const SmemLayout L = make_layout(D, a.TH, F, a.use_tma, pix, matching);
     dim3 grid((W + kOutCols - 1) / kOutCols, (H + a.TH - 1) / a.TH, b_count);
-    return pix ? launch_kernel<true>(grid, L.total, stream, a, local) : launch_kernel<false>(grid, L.total, stream, a, local);
+    return pix ? launch_variant<true>(matching, centered, grid, L.total, stream, a, local)
+               : launch_variant<false>(matching, centered, grid, L.total, stream, a, local);
 }
 
 extern "C" int mr_cost_volume_fwd(const float* keyframe, const float* const* frames, const float* proj,
@@ -1319,4 +1462,29 @@ extern "C" int mr_cost_volume_fwd_depthmap(const float* keyframe, const float* c
                "mr_cost_volume_fwd_depthmap: nhwc_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", nhwc_dtype);
     return mr::launch_cost_volume(keyframe, frames, proj, pixel_depths, out_cv, out_sfcv, B, F, D, H, W, alpha, chan_w, 0, B,
                                   0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, 1);
+}
+
+extern "C" int mr_cost_volume_fwd_matching(const float* keyframe, const float* const* frames, const float* proj,
+                                           const float* depths, const float* pixel_depths, float* out_cv, float* out_sfcv,
+                                           void* out_sfcv_nhwc, int nhwc_dtype, int B, int F, int D, int H, int W, float alpha,
+                                           const float* chan_w, int matching, int centered, void* stream) {
+    if (matching == 0) {   // use_ssim falsy: the plain |w - k| difference (monorec_model.py:227-228)
+        ::mr::set_error("mr_cost_volume_fwd_matching: matching 0 (plain L1 difference) is not implemented");
+        return MR_ENOSUPPORT;
+    }
+    MR_REQUIRE(matching == MR_CV_SSIM || matching == MR_CV_SSIM_L1 || matching == MR_CV_BOX_L1,
+               "mr_cost_volume_fwd_matching: unknown matching %d (MR_CV_SSIM, MR_CV_SSIM_L1 or MR_CV_BOX_L1)", matching);
+    MR_REQUIRE(centered == 0 || centered == 1, "mr_cost_volume_fwd_matching: centered must be 0 or 1 (got %d)", centered);
+    MR_REQUIRE((depths == nullptr) != (pixel_depths == nullptr),
+               "mr_cost_volume_fwd_matching: exactly one of depths / pixel_depths must be given (got %s)",
+               depths ? "both" : "neither");
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(pixel_depths) & 3) == 0,
+               "mr_cost_volume_fwd_matching: pixel_depths must be 4-byte aligned");
+    MR_REQUIRE(D >= 2 && D <= 128, "mr_cost_volume_fwd_matching: 2 <= D <= 128 required (got D=%d)", D);
+    MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "mr_cost_volume_fwd_matching: 1 <= F <= %d required (got F=%d)", MR_MAX_FRAMES, F);
+    MR_REQUIRE(nhwc_dtype == MR_DT_F32 || nhwc_dtype == MR_DT_F16,
+               "mr_cost_volume_fwd_matching: nhwc_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", nhwc_dtype);
+    const int pix = pixel_depths != nullptr;
+    return mr::launch_cost_volume(keyframe, frames, proj, pix ? pixel_depths : depths, out_cv, out_sfcv, B, F, D, H, W, alpha,
+                                  chan_w, 0, B, 0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, pix, matching, centered);
 }

@@ -15,7 +15,8 @@ void count_launch(int n = 1);
 int launch_cost_volume(const float* keyframe, const float* const* frames, const float* proj, const float* depths,
                        float* out_cv, float* out_sfcv, int B, int F, int D, int H, int W, float alpha,
                        const float* chan_w, int b_begin, int b_count, int gather_only, cudaStream_t stream,
-                       void* sf_nhwc = nullptr, int sf_nhwc_dtype = 0, int per_pixel_depths = 0);
+                       void* sf_nhwc = nullptr, int sf_nhwc_dtype = 0, int per_pixel_depths = 0,
+                       int matching = MR_CV_SSIM, int centered = 1);
 
 inline int check_cuda(cudaError_t e, const char* what) {
     if (e == cudaSuccess) return MR_OK;

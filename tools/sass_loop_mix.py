@@ -6,8 +6,12 @@ Compiles cost_volume.cu (default: the package's) for sm_90a with the library's f
 it with line information and finds the loops of cost_volume_kernel (backward branches).  A loop is attributed to a
 call site of march_unit<MODE> or pixel_phase<T> when the inlining chains of its instructions reach that call's source
 line.  For each march mode it prints the largest such loop, the row loop (three row steps per body), and for the
-per-pixel phase its loops; counts are per row step for the march and per loop iteration otherwise.  The plane-depth
-instantiation cost_volume_kernel<false> is reported first, the per-pixel-depth one (cv_depths) after it.
+per-pixel phase its loops; counts are per row step for the march and per loop iteration otherwise.
+
+The kernel is instantiated as cost_volume_kernel<PIX, ERR, CENTER>: depth source (plane table / per-pixel cv_depths), error
+mode (1 SSIM, 2 SSIM + L1, 3 box L1: MR_CV_*) and centred or uncentred fused volume.  The two default instantiations (SSIM,
+centred) are reported first, plane depths then per-pixel depths, and the other ten after them.  A source from before the
+error mode was a template parameter has only cost_volume_kernel<PIX>; it is reported under the same two titles.
 """
 import collections
 import re
@@ -48,13 +52,18 @@ def disassemble(src):
                               capture_output=True, text=True).stdout
 
 
-INSTANTIATIONS = [  # (label, mangled template argument of cost_volume_kernel<PIX>)
-    ("plane depths (cost_volume_kernel<false>)", "cost_volume_kernelILb0E"),
-    ("per-pixel depths (cost_volume_kernel<true>)", "cost_volume_kernelILb1E"),
+ERR_NAMES = {1: "SSIM", 2: "SSIM + L1", 3: "box L1"}
+# (label, mangled template arguments of cost_volume_kernel<PIX, ERR, CENTER>, those of a source with only <PIX>)
+INSTANTIATIONS = [
+    (f"{'per-pixel' if pix else 'plane'} depths, {ERR_NAMES[err]}, {'centred' if ctr else 'uncentred'} "
+     f"(cost_volume_kernel<{'true' if pix else 'false'}, {err}, {'true' if ctr else 'false'}>)",
+     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}EE", f"cost_volume_kernelILb{pix}EE" if err == 1 and ctr else None)
+    for err, ctr, pix in [(1, 1, 0), (1, 1, 1)] + [(e, c, p) for e in (1, 2, 3) for c in (1, 0) for p in (0, 1)
+                                                    if (e, c) != (1, 1)]
 ]
 
 
-def kernel_instructions(dis, name="cost_volume_kernelILb0E"):
+def kernel_instructions(dis, name="cost_volume_kernelILb0ELi1ELb1EE"):
     """[(addr, opcode, text, source lines of the inlining chain)] and {label: addr} of the kernel whose .text section
     name contains `name` (default: the plane instantiation)."""
     ins, labels, cur, inside, pending = [], {}, [], False, []
@@ -88,15 +97,19 @@ def main():
     text = src.read_text().splitlines()
     sites = {}
     for i, l in enumerate(text, 1):
-        m = re.search(r"\b(march_unit|pixel_phase)<(\d)(?:, PIX)?>\(", l)
+        m = re.search(r"\b(march_unit|pixel_phase)<(\d)(?:, \w+)*>\(", l)
         if m and "__device__" not in l and "void" not in l:
             sites[f"{m.group(1)}<{m.group(2)}>"] = i
     dis = disassemble(src)
-    for k, (title, name) in enumerate(INSTANTIATIONS):
-        if name not in dis:      # (a source from before the depth source became a template parameter)
-            if k == 0:
+    for k, (title, name, old) in enumerate(INSTANTIATIONS):
+        if name not in dis:
+            if old is not None and old in dis:       # (a source from before the error mode became a template parameter)
+                name = old
+            elif k == 0 and "cost_volume_kernelILb" not in dis:   # (from before the depth source became one)
                 report(src, "cost_volume_kernel", *kernel_instructions(dis, "cost_volume_kernel"), sites)
-            continue
+                continue
+            else:
+                continue
         if k:
             print("\n" + "=" * 100)
         report(src, title, *kernel_instructions(dis, name), sites)

@@ -1,0 +1,89 @@
+"""Kernel time of the cost volume's error modes and of the uncentred fused volume against the default, interleaved, in one
+process.
+
+    python tools/time_cv_variants.py [--iters=N] [--rounds=R]
+
+For config 2 (B 8, F 4, D 32, 256x512) and hires (B 4, F 6, D 64, 512x1024) it times, on the default inverse-depth planes,
+every round in turn:
+  ssim        mr_cost_volume_fwd (use_ssim=True, the default)
+  ssim_l1     mr_cost_volume_fwd_matching, MR_CV_SSIM_L1 (use_ssim=2)
+  box_l1      mr_cost_volume_fwd_matching, MR_CV_BOX_L1 (any other truthy use_ssim)
+  uncentred   mr_cost_volume_fwd_matching, MR_CV_SSIM with centered = 0 (not_center_cv=True)
+CUDA events bracket each launch; a round's number is the mean over N launches, the report the median over the rounds, and
+vs_ssim its ratio to the default's median.  The card name and its power limit are printed with the numbers.
+"""
+import json
+import statistics
+import subprocess
+import sys
+from pathlib import Path
+
+import torch
+
+ROOT = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(ROOT))
+from monorec_b200 import _lib  # noqa: E402
+from monorec_b200.synthetic import make_inputs, to_device  # noqa: E402
+
+CASES = {"ssim": None, "ssim_l1": (2, 1), "box_l1": (3, 1), "uncentred": (1, 0)}   # name -> (matching, centered)
+
+
+def power_limit():
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception as e:  # (no nvidia-smi: report why)
+        return f"unknown ({e})"
+
+
+def main():
+    opts = dict(a[2:].split("=", 1) for a in sys.argv[1:] if a.startswith("--"))
+    iters, rounds = int(opts.get("iters", 20)), int(opts.get("rounds", 5))
+    lib = _lib.load()
+    dev = "cuda:0"
+    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "power_limit": power_limit()}))
+    for name, (B, F, D, H, W) in (("config2", (8, 4, 32, 256, 512)), ("hires", (4, 6, 64, 512, 1024))):
+        d = to_device(make_inputs(B, F, H, W, seed=0), dev)
+        proj = torch.empty(B, F, 3, 4, device=dev)
+        planes = torch.empty(D, device=dev)
+        cv = torch.empty(B, D, H, W, device=dev)
+        sfcv = torch.empty(F, B, D, H, W, device=dev)
+        stream = torch.cuda.current_stream().cuda_stream
+        frames = _lib.ptr_array(d["frames"])
+        _lib.check(lib.mr_projection_tables(d["keyframe_pose"].data_ptr(), d["keyframe_intrinsics"].data_ptr(),
+                                            _lib.ptr_array(d["poses"]), _lib.ptr_array(d["intrinsics"]), B, F, H, W,
+                                            proj.data_ptr(), planes.data_ptr(), D, 0.0025, 0.33, stream), "tables")
+
+        def launch(case):
+            if CASES[case] is None:
+                rc = lib.mr_cost_volume_fwd(d["keyframe"].data_ptr(), frames, proj.data_ptr(), planes.data_ptr(), cv.data_ptr(),
+                                            sfcv.data_ptr(), B, F, D, H, W, 10.0, None, stream)
+            else:
+                matching, centered = CASES[case]
+                rc = lib.mr_cost_volume_fwd_matching(d["keyframe"].data_ptr(), frames, proj.data_ptr(), planes.data_ptr(), None,
+                                                     cv.data_ptr(), sfcv.data_ptr(), None, 0, B, F, D, H, W, 10.0, None,
+                                                     matching, centered, stream)
+            _lib.check(rc, case)
+
+        means = {c: [] for c in CASES}
+        for _ in range(rounds):
+            for c in CASES:
+                for _ in range(3):
+                    launch(c)
+                ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(iters)]
+                for e0, e1 in ev:
+                    e0.record()
+                    launch(c)
+                    e1.record()
+                torch.cuda.synchronize()
+                means[c].append(sum(e0.elapsed_time(e1) for e0, e1 in ev) / iters)
+        base = statistics.median(means["ssim"])
+        for c in CASES:
+            m = means[c]
+            print(json.dumps({"config": name, "shape": [B, F, D, H, W], "case": c, "ms_median": round(statistics.median(m), 4),
+                              "ms_min": round(min(m), 4), "ms_max": round(max(m), 4),
+                              "vs_ssim": round(statistics.median(m) / base, 3)}))
+
+
+if __name__ == "__main__":
+    main()
