@@ -297,6 +297,28 @@ int mr_sparse_metrics(const float* result, const float* target, const float* mvo
                       void* workspace, long long workspace_bytes, void* stream);
 int mr_images_u8_to_f32(const unsigned char* src, float* dst, int B, int Hs, int Ws, int crop_top, int crop_left,
                         int H, int W, void* stream);
+/* mr_dense_metrics: the twelve dense-ground-truth metrics of model/metric_functions/ in one pass: the seven *_metric functions of
+ * sparse_metrics.py:6-78, sc_inv / l1_rel / l1_inv of dense_metrics.py and completeness / covered_gt of
+ * completeness_metrics.py.  There is no validity mask: every pixel of the region of interest counts, and a zero depth gives
+ * the reference's IEEE outcome (inf / NaN values, a miss in a1-a3).
+ *   result, target   [B,1,H,W] predicted / ground-truth inverse depth
+ *   roi              host int[4] {r0, r1, c0, c1} (python slice semantics) or NULL (completeness and covered_gt ignore it)
+ *   min_inv_depth    > 0: inverse depths are clamped from below to it before inverting (1 / max_distance, as the reference's
+ *                    `max_distance is not None` branch computes it); <= 0: no clamp
+ *   out_metrics      device float[12]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel, sc_inv, l1_rel, l1_inv, completeness,
+ *                    covered_gt; no host synchronisation
+ *   workspace        device buffer of mr_dense_metrics_workspace(B) bytes, 8-byte aligned
+ * mr_median_scaling: the evaluater's median scaling (utils/util.py:135-142): out[b] = result[b] * (median(target[b][m]) /
+ *   median(result[b][m])) with m = target[b] > 0, all in fp32; each median is the lower one (torch.median), found by an exact
+ *   selection; an image with no target > 0 or a NaN among the selected results gets a NaN ratio.  result, target, out:
+ *   [B,1,H,W], out must not alias result; workspace: device buffer of mr_median_scaling_workspace(B,H,W) bytes, 4-byte
+ *   aligned.  No host synchronisation. */
+long long mr_dense_metrics_workspace(int B);
+int mr_dense_metrics(const float* result, const float* target, int B, int H, int W, const int* roi, float min_inv_depth,
+                     float* out_metrics, void* workspace, long long workspace_bytes, void* stream);
+long long mr_median_scaling_workspace(int B, int H, int W);
+int mr_median_scaling(const float* result, const float* target, float* out, int B, int H, int W, void* workspace,
+                      long long workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Point-cloud side (SURVEY.md section 8f row 3): create_pointcloud.py:65-105 + utils/ply_utils.py:34-53 on the device.

@@ -1,12 +1,15 @@
-"""Drop-ins for the reference's sparse depth metrics (model/metric_functions/sparse_metrics.py:81-251) and the loader's image
+"""Drop-ins for the reference's depth metrics (model/metric.py: model/metric_functions/sparse_metrics.py,
+dense_metrics.py, completeness_metrics.py), the evaluater's median scaling (utils/util.py:135-142) and the loader's image
 normalisation (data_loader/kitti_odometry_dataset.py:121-132), computed on the device by libmonorec_b200.so.
 
-The reference's evaluater (evaluater/evaluater.py:78-112) calls the seven `*_sparse_metric(data_dict, roi, max_distance)`
-functions one after the other, each a dozen elementwise torch kernels and a few reductions.  Here all seven come out of ONE
-fused pass (`mr_sparse_metrics`); the functions below keep the reference's names and signatures and share that pass through a
-small per-data_dict cache, so `model.metric` can be pointed at this module unchanged.  No CPU fallback.
+The reference's evaluater (evaluater/evaluater.py:78-112) calls the configured metric functions one after the other, each a
+dozen elementwise torch kernels and a few reductions.  Here the 21 `*_sparse*` metrics come out of ONE fused pass
+(`mr_sparse_metrics`) and the 12 dense and completeness metrics out of another (`mr_dense_metrics`); the functions below keep
+the reference's names and signatures and share those passes through a small cache, so `model.metric` can be pointed at this
+module unchanged.  No CPU fallback.
 """
 import ctypes
+import weakref
 
 import torch
 
@@ -57,6 +60,106 @@ for _i, _n in enumerate(NAMES):
     globals()[f"{_n}_sparse_metric"] = _make(_i)                                        # sparse_metrics.py:81-156
     globals()[f"{_n}_sparse_onlyvalid_metric"] = _make(_i, pred_all_valid=False)        # :159-184
     globals()[f"{_n}_sparse_onlydynamic_metric"] = _make(_i, use_cvmask=True)           # :187-212
+
+
+DENSE_NAMES = NAMES + ("sc_inv", "l1_rel", "l1_inv", "completeness", "covered_gt")
+# the last dense pass: (weakref to result, weakref to target, key, out).  Keyed on the tensors rather than on a data_dict, so
+# that the data_dict functions and the tensor-signature functions of one call set share it, and weak, so that a freed
+# tensor whose id is reused never matches
+_dense_last = [None]
+
+
+def _check_pair(pred, gt, what):
+    if not pred.is_cuda:
+        raise _lib.MonorecLibraryError(f"{what} needs CUDA tensors (no CPU fallback)")
+    if pred.dim() != 4 or pred.shape[1] != 1 or tuple(gt.shape) != tuple(pred.shape):
+        raise ValueError(f"{what}: result and target must both be [B,1,H,W], got {tuple(pred.shape)} and {tuple(gt.shape)}")
+
+
+def dense_metrics(depth_prediction, depth_gt, roi=None, max_distance=None):
+    """-> device tensor [12] in the order of DENSE_NAMES (no host synchronisation), from one fused pass (`mr_dense_metrics`).
+
+    The pass is remembered for these two tensors at their current version and this (roi, max_distance), so the twelve
+    reference-named functions below cost one launch group per call set."""
+    pred, gt = depth_prediction, depth_gt
+    _check_pair(pred, gt, "monorec_b200.metrics.dense_metrics")
+    key = (pred._version, gt._version, None if roi is None else tuple(int(v) for v in roi),
+           None if max_distance is None else float(max_distance))
+    hit = _dense_last[0]
+    if hit is not None and hit[0]() is pred and hit[1]() is gt and hit[2] == key:
+        return hit[3]
+    # get_absolute_depth (utils/util.py:46-56) clamps at the fp32 rounding of 1 / max_distance (a ZeroDivisionError for 0)
+    min_inv = 0.0 if max_distance is None else 1 / max_distance
+    lib = _lib.load()
+    p = pred.to(torch.float32).contiguous()
+    g = gt.to(device=p.device, dtype=torch.float32).contiguous()
+    B, _, H, W = p.shape
+    out = torch.empty(len(DENSE_NAMES), device=p.device, dtype=torch.float32)
+    ws_bytes = lib.mr_dense_metrics_workspace(B)
+    ws = torch.empty(ws_bytes // 8, device=p.device, dtype=torch.float64)
+    roi_c = None if roi is None else (ctypes.c_int * 4)(*[int(v) for v in roi])
+    with torch.cuda.device(p.device):
+        _lib.check(lib.mr_dense_metrics(p.data_ptr(), g.data_ptr(), B, H, W, roi_c, float(min_inv), out.data_ptr(), ws.data_ptr(),
+                                        ws_bytes, torch.cuda.current_stream(p.device).cuda_stream), "mr_dense_metrics")
+    _dense_last[0] = (weakref.ref(pred), weakref.ref(gt), key, out)
+    return out
+
+
+def _make_dense_dict(index):
+    def metric(data_dict, roi=None, max_distance=None):
+        return dense_metrics(data_dict["result"], data_dict["target"], roi, max_distance)[index]
+    metric.__name__ = f"{DENSE_NAMES[index]}_metric"
+    return metric
+
+
+def _make_dense_tensor(index, doc):
+    def metric(depth_prediction, depth_gt, roi=None, max_distance=None):
+        return dense_metrics(depth_prediction, depth_gt, roi, max_distance)[index]
+    metric.__name__ = f"{DENSE_NAMES[index]}_metric"
+    metric.__doc__ = doc
+    return metric
+
+
+# sparse_metrics.py:6-78: data_dict signature, every pixel of the roi counts
+for _i, _n in enumerate(NAMES):
+    globals()[f"{_n}_metric"] = _make_dense_dict(_i)
+# dense_metrics.py and completeness_metrics.py: (depth_prediction, depth_gt, roi, max_distance)
+sc_inv_metric = _make_dense_tensor(7, """Scale-invariant error: per image sqrt(sum E^2 / n - (sum E)^2 / n^2) with E = log of the
+    predicted over the true depth (NaN -> 0) and n the roi's pixel count; an image whose value is NaN counts 0.  Sums in
+    float64, where the reference sums in fp32: images whose E is nearly constant can differ by more than rounding.""")
+l1_rel_metric = _make_dense_tensor(8, "Mean |d_pred - d_gt| / d_gt of the depths (the formula of abs_rel_metric).")
+l1_inv_metric = _make_dense_tensor(9, "Mean |p - g| of the inverse depths after relu: no clamp at max_distance.")
+completeness_metric = _make_dense_tensor(10, "Share of pixels with result != 0 over the whole tensor (ignores roi and "
+                                             "max_distance).")
+covered_gt_metric = _make_dense_tensor(11, """mask_mean((result != 0), target != 0) as written in the reference: mask_mean
+    drops the masked entries, so this is the share of pixels with result != 0 among the pixels where target == 0 (NaN when
+    there is none), not among the pixels with ground truth.  Ignores roi and max_distance.""")
+
+
+def median_scaling(data_dict):
+    """utils/util.py:135-142 on the device (`mr_median_scaling`): a shallow copy of `data_dict` whose "result" is the
+    prediction times, per image, median(target[target > 0]) / median(result[target > 0]), in fp32 and bit for bit as the
+    reference computes it, without a host synchronisation.  Each median is torch.median's lower median; an image with no
+    target > 0, or a NaN among its selected predictions, gets a NaN ratio.  The input dict and its tensors are not modified."""
+    pred, gt = data_dict["result"], data_dict["target"]
+    _check_pair(pred, gt, "monorec_b200.metrics.median_scaling")
+    if pred.dtype != torch.float32:
+        raise ValueError(f"median_scaling: result must be float32, got {pred.dtype}")
+    lib = _lib.load()
+    p = pred.contiguous()
+    g = gt.to(device=p.device, dtype=torch.float32).contiguous()
+    B, _, H, W = p.shape
+    out = torch.empty_like(p)
+    ws_bytes = lib.mr_median_scaling_workspace(B, H, W)
+    ws = torch.empty(ws_bytes // 4, device=p.device, dtype=torch.float32)
+    with torch.cuda.device(p.device):
+        _lib.check(lib.mr_median_scaling(p.data_ptr(), g.data_ptr(), out.data_ptr(), B, H, W, ws.data_ptr(), ws_bytes,
+                                         torch.cuda.current_stream(p.device).cuda_stream), "mr_median_scaling")
+    scaled = dict(data_dict)
+    scaled["result"] = out
+    # the sparse pass cached for the unscaled result is keyed on its id, which a later tensor may reuse once it is freed
+    scaled.pop("_mr_metrics_cache", None)
+    return scaled
 
 
 def images_u8_to_f32(images_u8, crop_box=None):
