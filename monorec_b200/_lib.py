@@ -7,11 +7,13 @@ from ctypes import c_char_p, c_float, c_int, c_longlong, c_void_p, POINTER
 from pathlib import Path
 
 import os
+import threading
 
 _PKG = Path(__file__).resolve().parent
 # MONOREC_B200_LIB: load another build of the library (kernel-variant experiments: tools/build_variant_src.py)
 LIB_PATH = Path(os.environ["MONOREC_B200_LIB"]) if os.environ.get("MONOREC_B200_LIB") else _PKG / "libmonorec_b200.so"
 _lib = None
+_LOAD_LOCK = threading.Lock()
 
 c_float_p = POINTER(c_float)
 
@@ -82,22 +84,26 @@ class MonorecLibraryError(RuntimeError):
 
 
 def load(build_if_missing=True):
-    """Returns the loaded CDLL.  Builds it in-tree with nvcc if absent and a compiler is available."""
+    """Returns the loaded CDLL.  Builds it in-tree with nvcc if absent and a compiler is available.  Thread-safe: concurrent
+    first calls (DataParallel replicas, several host threads) build and bind the library once."""
     global _lib
     if _lib is not None:
         return _lib
-    if build_if_missing and not os.environ.get("MONOREC_B200_LIB"):
-        # no-op when the source digest matches the stamp; rebuilds a stale library (sources newer than the .so)
-        from . import build as _build
-        _build.build()
-    if not LIB_PATH.exists():
-        raise MonorecLibraryError(f"{LIB_PATH} not found: run `python -m monorec_b200.build` (needs nvcc, sm_90a)")
-    lib = ctypes.CDLL(str(LIB_PATH))
-    for name, (res, args) in SIGNATURES.items():
-        fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
-        fn.restype = res
-        fn.argtypes = args
-    _lib = lib
+    with _LOAD_LOCK:
+        if _lib is not None:
+            return _lib
+        if build_if_missing and not os.environ.get("MONOREC_B200_LIB"):
+            # no-op when the source digest matches the stamp; rebuilds a stale library (sources newer than the .so)
+            from . import build as _build
+            _build.build()
+        if not LIB_PATH.exists():
+            raise MonorecLibraryError(f"{LIB_PATH} not found: run `python -m monorec_b200.build` (needs nvcc, sm_90a)")
+        lib = ctypes.CDLL(str(LIB_PATH))
+        for name, (res, args) in SIGNATURES.items():
+            fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol
+            fn.restype = res
+            fn.argtypes = args
+        _lib = lib   # published only once every signature is bound
     return lib
 
 

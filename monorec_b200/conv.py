@@ -13,6 +13,7 @@ import torch
 from . import _lib
 
 import os
+import threading
 
 MAX_SRC = 3
 ACT_NONE, ACT_LEAKY, ACT_SIGMOID, ACT_ABSTANH = 0, 1, 2, 3
@@ -24,6 +25,7 @@ LEAKY_SLOPE = 0.1  # model/layers.py:290, 318, 381
 MODE = os.environ.get("MONOREC_B200_CONV", "tf32").lower()
 DT_F32, DT_F16 = 0, 1
 FLOPS = None       # set to [0] to count the conv stacks' flops during a forward (bench.py's tensor roofline)
+_WTC_LOCK = threading.Lock()
 
 
 def set_mode(mode):
@@ -265,16 +267,19 @@ class PackedConv:
         # to 16: 5.93 -> 5.83 ms per half-mode forward at B=8 against the CUDA-core per-pixel kernel
         self.tc_ok = self.cout <= 256 and all(c % 4 == 0 for c in self.src_c)
         self.tc_ok_f16 = self.tc_ok and all(c % 8 == 0 for c in self.src_c)
-        self._wtc = {}
+        self._wtc = {}     # half -> packed tensor-core weights, on the device of `weight` like every tensor here
         self._w_src = w
 
     def wtc(self, half=False):
         if half not in self._wtc:
-            self._wtc[half] = pack_tc_weight(self._w_src, self.src_c, half=half)
+            with _WTC_LOCK:   # (concurrent forwards pack it once)
+                if half not in self._wtc:
+                    self._wtc[half] = pack_tc_weight(self._w_src, self.src_c, half=half)
         return self._wtc[half]
 
-    def __call__(self, srcs, out=None, out_hw=None, final=False, out_coff=0):
-        """out_coff: first channel of the slice of `out` this layer writes (tensor-core path)."""
+    def __call__(self, srcs, out=None, out_hw=None, final=False, out_coff=0, act_ab=None):
+        """out_coff: first channel of the slice of `out` this layer writes (tensor-core path).  act_ab: (act_a, act_b) of
+        this launch instead of the layer's own (the depth heads' inverse-depth affine), so that a call mutates nothing."""
         assert tuple(s.shape[3] for s in srcs) == self.src_c, (tuple(s.shape[3] for s in srcs), self.src_c)
         if FLOPS is not None:      # bench.py: multiply-adds of this layer (2 flops each), counted on one eager forward
             Bn, Hs, Ws, _ = srcs[0].shape
@@ -282,18 +287,20 @@ class PackedConv:
             FLOPS[0] += 2 * Bn * ho * wo * self.cout * sum(self.src_c) * self.kh * self.kw
         if MODE == "f16" and srcs[0].dtype == torch.float16:
             if self.tc_ok_f16:
-                return conv2d_tc(srcs, self, out=out, out_hw=out_hw, round_out=False, half=True, out_f32=final, out_coff=out_coff)
+                return conv2d_tc(srcs, self, out=out, out_hw=out_hw, round_out=False, half=True, out_f32=final, out_coff=out_coff,
+                                 act_ab=act_ab)
             assert self.cout == 1, "f16 mode: only the single-channel heads run on the CUDA-core kernel"
         if MODE == "tf32" and self.tc_ok:
-            return conv2d_tc(srcs, self, out=out, out_hw=out_hw, round_out=not final, out_coff=out_coff)
+            return conv2d_tc(srcs, self, out=out, out_hw=out_hw, round_out=not final, out_coff=out_coff, act_ab=act_ab)
         if out_coff:
             raise NotImplementedError("monorec_b200.conv: channel-slice outputs need the tensor-core path")
-        return conv2d(srcs, self.w32, self.bias, self.kh, self.kw, stride=self.stride, act=self.act, act_a=self.act_a,
-                      act_b=self.act_b, out=out, pad=self.pad, out_hw=out_hw, out_step=self.out_step, out_off=self.out_off)
+        act_a, act_b = (self.act_a, self.act_b) if act_ab is None else act_ab
+        return conv2d(srcs, self.w32, self.bias, self.kh, self.kw, stride=self.stride, act=self.act, act_a=act_a,
+                      act_b=act_b, out=out, pad=self.pad, out_hw=out_hw, out_step=self.out_step, out_off=self.out_off)
 
 
-def conv2d_tc(srcs, L, out=None, out_hw=None, round_out=True, half=False, out_f32=False, out_coff=0):
-    """Tensor-core launch (csrc/conv_tc.cu) of a PackedConv."""
+def conv2d_tc(srcs, L, out=None, out_hw=None, round_out=True, half=False, out_f32=False, out_coff=0, act_ab=None):
+    """Tensor-core launch (csrc/conv_tc.cu) of a PackedConv; act_ab overrides the layer's (act_a, act_b)."""
     lib = _lib.load()
     x0 = srcs[0]
     B = x0.shape[0]
@@ -303,7 +310,7 @@ def conv2d_tc(srcs, L, out=None, out_hw=None, round_out=True, half=False, out_f3
                           dtype=torch.float16 if (half and not out_f32) else torch.float32)
     wtc, n_pad, k_pad = L.wtc(half)
     d = ConvDesc()
-    _fill_desc(d, srcs, L, out, (Ho, Wo), _tc_pad(srcs, L), wtc, half, out_coff)
+    _fill_desc(d, srcs, L, out, (Ho, Wo), _tc_pad(srcs, L), wtc, half, out_coff, act_ab)
     with torch.cuda.device(x0.device):
         _lib.check(lib.mr_conv2d_nhwc_tc(ctypes.byref(d), n_pad, k_pad, int(round_out), _stream(x0)), "mr_conv2d_nhwc_tc")
     return out
@@ -343,7 +350,7 @@ def tc_plan(srcs, subs, out, out_hw=None, half=False, out_coff=0):
     return plan.as_dict()
 
 
-def _fill_desc(d, srcs, L, out, out_hw, pad, wtc, half, out_coff=0):
+def _fill_desc(d, srcs, L, out, out_hw, pad, wtc, half, out_coff=0, act_ab=None):
     x0 = srcs[0]
     B, Hs, Ws, _ = x0.shape
     sy, sx = L.stride
@@ -362,7 +369,8 @@ def _fill_desc(d, srcs, L, out, out_hw, pad, wtc, half, out_coff=0):
     d.dst = out.data_ptr()
     d.dst_H, d.dst_W, d.dst_c, d.dst_coff = out.shape[1], out.shape[2], out.shape[3], int(out_coff)
     d.oy_step, d.ox_step, d.oy_off, d.ox_off = L.out_step[0], L.out_step[1], L.out_off[0], L.out_off[1]
-    d.act, d.act_a, d.act_b = L.act, L.act_a, L.act_b
+    d.act = L.act
+    d.act_a, d.act_b = (L.act_a, L.act_b) if act_ab is None else act_ab
     d.src_dtype, d.dst_dtype = (DT_F16 if half else DT_F32), _dt(out)
 
 

@@ -34,6 +34,7 @@
 #include "mr_common.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <atomic>
 #include <cstdint>
 #include <type_traits>
 
@@ -1302,11 +1303,16 @@ int pick_tile_rows(int D, int F, int use_tma, bool pix, int err) {
 
 template <bool PIX, int ERR, bool CENTER>
 int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
-    static int smem_set = 0;   // the attribute is per function and per device context; setting it again is harmless
-    if (smem_set < smem) {
+    // The opt-in is per function and per device context, so it is remembered per device (bit d: device d; devices from 64 on
+    // set it before every launch).  Two threads that both find the bit clear both set the attribute: harmless.
+    static std::atomic<unsigned long long> opted_in{0};
+    int dev = 0;
+    MR_CUDA(cudaGetDevice(&dev));
+    const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
+    if ((opted_in.load(std::memory_order_acquire) & bit) == 0) {
         MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX, ERR, CENTER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      227 * 1024));
-        smem_set = 227 * 1024;
+        opted_in.fetch_or(bit, std::memory_order_release);
     }
     cost_volume_kernel<PIX, ERR, CENTER><<<grid, kThreads, smem, stream>>>(a, maps);
     MR_LAUNCH_CHECK("cost_volume_kernel");

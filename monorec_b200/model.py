@@ -8,6 +8,7 @@ convolution engine) through the C ABI.  The ResNet-18 trunk stays on torchvision
 reference too; SURVEY.md §8f "next" row 1) with its eval-mode BatchNorms folded, in half precision in half mode.  (Round 2
 measured the trunk on the conv engine at 1.03 ms against cuDNN's 0.71 ms in half mode, so that variant was removed.)
 """
+import threading
 import warnings
 
 import torch
@@ -20,6 +21,7 @@ from .cost_volume import CostVolumeModule
 __all__ = ["MonoRecModel", "CostVolumeModule", "MaskModule", "DepthModule", "ResnetEncoder"]
 
 _CUDNN_FUSED = hasattr(torch, "cudnn_convolution_relu") and hasattr(torch, "cudnn_convolution_add_relu")
+_PACK_LOCK = threading.Lock()   # every _Packed lookup and build (module-level: a lock in a module would break deepcopy / pickle)
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -60,26 +62,65 @@ class Refine(nn.Module):
         self.conv2d_t = nn.ConvTranspose2d(in_channels, out_channels, kernel_size=4, stride=2)
 
 
+def _source_sig(tensors):
+    return (C.MODE,) + tuple((t.data_ptr(), t._version, str(t.device)) for t in tensors)
+
+
 class _Packed:
-    """Kernel-layout copies of a module's parameters, rebuilt when a parameter changes (load_state_dict, .to(), an optimizer
-    step: anything that bumps the tensors' version counters or moves them).  In-place edits through `.data` (e.g.
-    `p.data.copy_(ema)`) are invisible to autograd's version counter: call `invalidate()` (or the owning module's
-    `invalidate_packed_weights()`) after such an edit."""
+    """Kernel-layout copies of a module's parameters, one per device, rebuilt when a parameter changes (load_state_dict, .to(),
+    an optimizer step: anything that bumps the tensors' version counters or moves them).  In-place edits through `.data`
+    (e.g. `p.data.copy_(ema)`) are invisible to autograd's version counter: call `invalidate()` (or the owning module's
+    `invalidate_packed_weights()`) after such an edit.
+
+    An entry is keyed on the device its tensors live on and holds the signature of the source parameters it was built from
+    (`_PackedSource._pack_sig`).  DataParallel replicas share this object with the module they were replicated from (their
+    `__dict__` is a shallow copy), so the replicas of every later forward find the entry of their device.  Lookups and builds
+    hold one lock: concurrent forwards build an entry once and never see a half-built one.  A new signature drops the entries
+    of the old one on every device."""
 
     def __init__(self):
-        self.sig, self.data = None, {}
+        self.entries = {}     # str(device) -> (signature, packed data)
 
     def invalidate(self):
-        self.sig = None
+        with _PACK_LOCK:
+            self.entries = {}
 
-    def get(self, module, builder):   # noqa: D401
-        params = list(module.parameters())
-        sig = (C.MODE,) + tuple((p.data_ptr(), p._version, str(p.device)) for p in params)
-        if sig != self.sig:
-            with torch.no_grad():
-                self.data = builder()
-            self.sig = sig
-        return self.data
+    def get(self, sig, device, builder):
+        key = str(device)
+        with _PACK_LOCK:
+            entry = self.entries.get(key)
+            if entry is None or entry[0] != sig:
+                with torch.no_grad():
+                    entry = (sig, builder())
+                if device.type == "cuda":   # built on this thread's stream: complete before another stream reads it
+                    torch.cuda.current_stream(device).synchronize()
+                entries = {k: v for k, v in self.entries.items() if v[0] == sig}
+                entries[key] = entry
+                self.entries = entries
+            return entry[1]
+
+
+class _PackedSource:
+    """Where a module's kernel-layout copies come from.  The signature is that of the module's own parameters -- except in a
+    DataParallel replica, which has no registered parameters (its copies on its device are plain attributes, broadcast anew
+    for every forward): it carries the signature of the original's parameters, taken when it is replicated."""
+
+    _src_sig = None
+
+    def _source_tensors(self):
+        return list(self.parameters())
+
+    def _pack_sig(self):
+        return self._src_sig if self._src_sig is not None else _source_sig(self._source_tensors())
+
+    def _replicate_for_data_parallel(self):
+        replica = super()._replicate_for_data_parallel()
+        replica._src_sig = self._pack_sig()
+        return replica
+
+    def _packs(self, builder):
+        """The entry of the device this module's weights are on, built by `builder` (from those weights) if missing."""
+        return self._packed.get(self._pack_sig(), self._pack_device(), builder)
 
 
 def _leaky(conv, src_c, stride=(1, 1)):
@@ -87,7 +128,7 @@ def _leaky(conv, src_c, stride=(1, 1)):
 
 
 # --------------------------------------------------------------------------------------------------------------------
-class ResnetEncoder(nn.Module):
+class ResnetEncoder(_PackedSource, nn.Module):
     """torchvision ResNet-18 trunk, 5 feature maps (monorec_model.py:95-129)."""
 
     def __init__(self, num_layers=18, pretrained=True):
@@ -112,6 +153,7 @@ class ResnetEncoder(nn.Module):
                 # the reference would download them here; MonoRecModel warns if no checkpoint supplies the encoder either
                 self.pretrained_requested_but_missing = True
         self.encoder = torchvision.models.resnet18(weights=weights)
+        self._packed = _Packed()
 
     # ---- inference fast path: BatchNorm (eval mode = a fixed per-channel affine) folded into the preceding convolution ----
     @staticmethod
@@ -125,24 +167,38 @@ class ResnetEncoder(nn.Module):
 
     def invalidate_packed_weights(self):
         """Forget the folded / packed copies (needed only after in-place `.data` edits of the parameters or BatchNorm buffers)."""
-        self._fold_sig = None
+        self._packed.invalidate()
+
+    def _source_tensors(self):
+        e = self.encoder
+        return [t for n, t in list(e.named_parameters()) + list(e.named_buffers()) if not n.startswith("fc.")]
+
+    def _pack_device(self):
+        return self.encoder.conv1.weight.device
+
+    def _build(self):
+        e = self.encoder
+        f = {"stem": self._fold(e.conv1, e.bn1), "blocks": []}
+        for layer in (e.layer1, e.layer2, e.layer3, e.layer4):
+            blocks = []
+            for blk in layer:
+                down = None if blk.downsample is None else self._fold(blk.downsample[0], blk.downsample[1]) + (
+                    blk.downsample[0].stride,)
+                blocks.append((self._fold(blk.conv1, blk.bn1), blk.conv1.stride, self._fold(blk.conv2, blk.bn2), down))
+            f["blocks"].append(blocks)
+        # in half mode the trunk runs in half as well (folded weights and activations): its NHWC outputs feed the conv engine
+        # without casts (0.82 -> 0.71 ms at B=8)
+        if C.MODE == "f16" and f["stem"][0].is_cuda:
+            conv = lambda wb: (wb[0].half().contiguous(memory_format=torch.channels_last), wb[1].half())   # noqa: E731
+            f = {"stem": conv(f["stem"]),
+                 "blocks": [[(conv(a), s_, conv(b), None if d is None else conv(d[:2]) + (d[2],)) for a, s_, b, d in blocks]
+                            for blocks in f["blocks"]]}
+        return f
 
     def _folded(self):
-        e = self.encoder
-        tensors = [t for n, t in list(e.named_parameters()) + list(e.named_buffers()) if not n.startswith("fc.")]
-        sig = tuple((t.data_ptr(), t._version, str(t.device)) for t in tensors)
-        if sig != getattr(self, "_fold_sig", None):
-            with torch.no_grad():
-                f = {"stem": self._fold(e.conv1, e.bn1), "blocks": []}
-                for layer in (e.layer1, e.layer2, e.layer3, e.layer4):
-                    blocks = []
-                    for blk in layer:
-                        down = None if blk.downsample is None else self._fold(blk.downsample[0], blk.downsample[1]) + (
-                            blk.downsample[0].stride,)
-                        blocks.append((self._fold(blk.conv1, blk.bn1), blk.conv1.stride, self._fold(blk.conv2, blk.bn2), down))
-                    f["blocks"].append(blocks)
-            self._fold_cache, self._fold_sig = f, sig
-        return self._fold_cache
+        """The folded trunk weights the inference path runs on (half in f16 mode on CUDA), built once per parameter version
+        and device."""
+        return self._packs(self._build)
 
     # cuDNN's fused epilogues where the build offers them (conv + bias + ReLU, conv + residual + bias + ReLU: the ~24
     # element-wise add / clamp launches of the trunk disappear); the folded trunk also runs on the CPU, on F.conv2d
@@ -169,16 +225,7 @@ class ResnetEncoder(nn.Module):
     def _forward_folded(self, input_image):
         e, f = self.encoder, self._folded()
         x = (input_image - 0.45) / 0.225
-        # in half mode the trunk runs in half as well (folded weights and activations): its NHWC outputs feed the conv engine
-        # without casts (0.82 -> 0.71 ms at B=8)
-        if C.MODE == "f16" and x.is_cuda:
-            if getattr(self, "_fold_half_sig", None) != self._fold_sig:
-                conv = lambda wb: (wb[0].half().contiguous(memory_format=torch.channels_last), wb[1].half())   # noqa: E731
-                self._fold_half = {"stem": conv(f["stem"]),
-                                   "blocks": [[(conv(a), s_, conv(b), None if d is None else conv(d[:2]) + (d[2],)) for a, s_, b, d in blocks]
-                                              for blocks in f["blocks"]]}
-                self._fold_half_sig = self._fold_sig
-            f = self._fold_half
+        if f["stem"][0].dtype == torch.float16:
             x = x.half()
         x = self._conv_relu(x, f["stem"][0], f["stem"][1], tuple(e.conv1.stride), tuple(e.conv1.padding))
         feats = [x]
@@ -196,7 +243,7 @@ class ResnetEncoder(nn.Module):
         # (monorec_model.py:372-380), the DepthModule levels 0-2 (:545), and nothing else in the reference touches
         # data_dict["image_features"].  It is computed when somebody asks for it.
         last = f["blocks"][3]
-        self.features = _TrunkFeatures(feats, lambda t: self._run_blocks(t, last))
+        self.features = _TrunkFeatures(feats, tail_fn=lambda t: self._run_blocks(t, last))
         return self.features
 
     def forward(self, input_image):
@@ -214,20 +261,24 @@ class ResnetEncoder(nn.Module):
 
 class _TrunkFeatures(list):
     """`image_features` (monorec_model.py:118-129) with its last entry evaluated on first use.  Slices and indices below 4 --
-    everything the Mask / Depth modules do -- never trigger it; index 4 / -1, iteration, comparison, concatenation, copy do."""
+    everything the Mask / Depth modules do -- never trigger it; index 4 / -1, iteration, comparison, concatenation, copy do.
 
-    def __init__(self, first_four, tail_fn):
-        super().__init__(list(first_four) + [None])
+    Without `tail_fn` it is a plain list of `items`: `type(f)(iterable)` is how torch.nn.parallel.gather rebuilds it (after
+    iterating the replicas' lists, which evaluates their level 4), so DataParallel gathers it like the reference's list."""
+
+    def __init__(self, items=(), tail_fn=None):
+        super().__init__(list(items) + [None] if tail_fn is not None else items)
         self._tail_fn = tail_fn
 
     def _fill(self):
-        if list.__getitem__(self, 4) is None:
+        if self._tail_fn is not None and list.__getitem__(self, 4) is None:
             with torch.no_grad():
                 list.__setitem__(self, 4, self._tail_fn(list.__getitem__(self, 3)))
 
     def reset_tail(self):
         """After a CUDA-graph replay rewrote level 3 in place: the cached level 4 is stale."""
-        list.__setitem__(self, 4, None)
+        if self._tail_fn is not None:
+            list.__setitem__(self, 4, None)
 
     def __getitem__(self, i):
         if isinstance(i, slice):
@@ -268,7 +319,7 @@ class _TrunkFeatures(list):
         return (list, (list(list.__iter__(self)),))
 
 
-class MaskModule(nn.Module):
+class MaskModule(_PackedSource, nn.Module):
     """Moving-object mask U-Net over the single-frame volumes (monorec_model.py:287-385)."""
 
     def __init__(self, depth_steps=32, feature_channels=(64, 64, 128, 256, 512), use_cv=True, use_features=True):
@@ -295,6 +346,9 @@ class MaskModule(nn.Module):
         """After in-place `.data` edits of the parameters (not seen by the version counters): repack on the next call."""
         self._packed.invalidate()
 
+    def _pack_device(self):
+        return self.classifier[0].weight.device
+
     def _build(self):
         e, d, fc = self._cv_enc_feat_chns, self._dec_feat_chns, self.feat_chns
         p = {}
@@ -315,7 +369,7 @@ class MaskModule(nn.Module):
         feats_nchw = data_dict["image_features"]
         if self.training:
             raise NotImplementedError("monorec_b200.MaskModule: inference only (dropout / autograd are not implemented)")
-        P = self._packed.get(self, self._build)
+        P = self._packs(self._build)
         nF = len(sfcvs)
         B, D, H, W = sfcvs[0].shape
         # all frames go through the encoder as one batch of F*B volumes (the reference loops, :357-365)
@@ -359,7 +413,7 @@ class MaskModule(nn.Module):
         return data_dict
 
 
-class DepthModule(nn.Module):
+class DepthModule(_PackedSource, nn.Module):
     """Depth U-Net over (masked cost volume (+) keyframe) with 4 output scales (monorec_model.py:476-557)."""
 
     def __init__(self, depth_steps=32, feature_channels=(64, 64, 128, 256, 512), large_model=False):
@@ -386,11 +440,14 @@ class DepthModule(nn.Module):
         self.predictors = nn.ModuleList([nn.Sequential(nn.Identity(), nn.Conv2d(ch, 1, 3))
                                          for ch in d[:3] + d[-1:]])
         self._packed = _Packed()
-        self.out_range = (0.0, 1.0)   # (a, b): heads emit a + b * |tanh|; MonoRecModel folds the inverse-depth affine in
+        self.out_range = (0.0, 1.0)   # (a, b): heads emit a + b * |tanh| unless forward() is given another affine
 
     def invalidate_packed_weights(self):
         """After in-place `.data` edits of the parameters (not seen by the version counters): repack on the next call."""
         self._packed.invalidate()
+
+    def _pack_device(self):
+        return self.predictors[0][1].weight.device
 
     def _build(self):
         e, d, fc = self._cv_enc_feat_chns, self._dec_feat_chns, self.feat_chns
@@ -402,10 +459,10 @@ class DepthModule(nn.Module):
             return (C.PackedConv(wy, m.conv_y.bias, src_c, stride=(m.stride, 1), act=C.ACT_LEAKY, act_a=C.LEAKY_SLOPE),
                     _leaky(m.conv_x, (m.conv_x.in_channels,), stride=(1, m.stride)))
         cin0 = self._in_channels
-        self._cin0_pad = (-cin0) % (8 if C.MODE == "f16" else 4)   # NHWC pixel stride must be a multiple of 16 bytes
-        p = {"enc": []}
+        cpad = (-cin0) % (8 if C.MODE == "f16" else 4)   # NHWC pixel stride must be a multiple of 16 bytes
+        p = {"enc": [], "cin0_pad": cpad}
         for i, s in enumerate(self.enc):
-            first = cr2(s[0], (cin0 + self._cin0_pad,), self._cin0_pad) if i == 0 else cr2(s[0], (e[i - 1],))
+            first = cr2(s[0], (cin0 + cpad,), cpad) if i == 0 else cr2(s[0], (e[i - 1],))
             p["enc"].append((first, cr2(s[1], (e[i],))))
         p["dec0"] = C.refine_layer(self.dec[0].conv2d_t, (e[4],))
         p["dec1"] = (C.refine_layer(self.dec[1][0].conv2d_t, (e[3], fc[2], d[0])), cr2(self.dec[1][1], (d[1],)))
@@ -420,23 +477,27 @@ class DepthModule(nn.Module):
     def _cr2(srcs, pk):
         return pk[1]([pk[0](srcs)])
 
-    def _head(self, x, head):
-        head.act_a, head.act_b = self.out_range
-        y = head([x], final=True)
+    @staticmethod
+    def _head(x, head, out_range):
+        y = head([x], final=True, act_ab=out_range)
         B, H, W, _ = y.shape
         return y.view(B, 1, H, W)
 
-    def forward(self, data_dict):
+    def forward(self, data_dict, out_range=None):
+        """out_range: (a, b) of the heads' a + b * |tanh| for this call (MonoRecModel passes the inverse-depth affine);
+        default `self.out_range`, the reference's raw |tanh|.  Passed to the launches, never stored: concurrent calls with
+        different ranges are independent."""
         if self.training:
             raise NotImplementedError("monorec_b200.DepthModule: inference only")
-        P = self._packed.get(self, self._build)
+        out_range = tuple(self.out_range if out_range is None else out_range)
+        P = self._packs(self._build)
         keyframe = data_dict["keyframe"]
         cv = data_dict["cost_volume"]
         feats_nchw = data_dict["image_features"]
         B, D, H, W = cv.shape
         # cat(cost_volume, keyframe) (:531); when MonoRecModel passes the unmasked volume plus `_cv_mask_for_depth`
         # the (1 - cv_mask) product of :713 is applied during the layout change
-        cpad = self._cin0_pad
+        cpad = P["cin0_pad"]
         # (the pad channels behind cat(cost volume, keyframe) must be zero, not garbage; the two layout kernels below write
         # channels [0, D + 3), so only the pad channels are cleared -- not the whole 84 MB buffer)
         x = torch.empty(B, H, W, D + 3 + cpad, device=cv.device, dtype=C.act_dtype())
@@ -452,23 +513,23 @@ class DepthModule(nn.Module):
         heads = P["heads"]
         preds = []
         x = P["dec0"]([feats[4]])                                                     # 256 @ 1/8
-        preds.insert(0, self._head(x, heads[0]))
+        preds.insert(0, self._head(x, heads[0], out_range))
         up, pk = P["dec1"]
         x = self._cr2([up([feats[3], img[2], x])], pk)                                # 128 @ 1/4
-        preds.insert(0, self._head(x, heads[1]))
+        preds.insert(0, self._head(x, heads[1], out_range))
         up, pk = P["dec2"]
         x = self._cr2([up([feats[2], img[1], x])], pk)                                # 64 @ 1/2
-        preds.insert(0, self._head(x, heads[2]))
+        preds.insert(0, self._head(x, heads[2], out_range))
         x = P["dec3"]([feats[1], img[0], x])                                          # 48 @ full
         pk, last = P["dec4"]
         x = last([self._cr2([feats[0], x], pk)])                                      # 24 @ full
-        preds.insert(0, self._head(x, heads[3]))
+        preds.insert(0, self._head(x, heads[3], out_range))
         data_dict["predicted_inverse_depths"] = preds
         return data_dict
 
     def predict_depth(self, x, scale):
         """API parity with the reference (:554-557); x is NHWC inside this implementation."""
-        return self._head(x, self._packed.get(self, self._build)["heads"][scale])
+        return self._head(x, self._packs(self._build)["heads"][scale], tuple(self.out_range))
 
 
 class MonoRecModel(nn.Module):
@@ -517,7 +578,10 @@ class MonoRecModel(nn.Module):
             for param in module.parameters(True):
                 param.requires_grad_(False)
         self.augmenter = None
-        self._trunk_channels_last = False
+        # torchvision trunk on cuDNN: channels-last so that its outputs are already NHWC for the conv engine (the dict still
+        # holds logical (B,C,H,W) tensors).  Done once here, not in forward: forward mutates no module state, so concurrent
+        # calls and DataParallel replicas are safe.  load_state_dict / .to() keep the layout.
+        self._feature_extractor.to(memory_format=torch.channels_last)
 
     def invalidate_packed_weights(self):
         """Forget every kernel-layout copy of the parameters (folded trunk, packed conv stacks).  Only needed after edits
@@ -590,11 +654,7 @@ class MonoRecModel(nn.Module):
                 data_dict["cost_volume"] = keyframe.new_zeros(s)
                 data_dict["single_frame_cvs"] = [data_dict["cost_volume"].clone() for _ in data_dict["poses"]]
 
-            # torchvision trunk on cuDNN: channels-last so that its outputs are already NHWC for the conv engine (the dict
-            # still holds logical (B,C,H,W) tensors); TF32 is allowed there unless the engine runs its fp32 parity mode
-            if not self._trunk_channels_last:
-                self._feature_extractor.to(memory_format=torch.channels_last)
-                self._trunk_channels_last = True
+            # torchvision trunk on cuDNN, fed channels-last; TF32 is allowed there unless the engine runs its fp32 parity mode
             # (only TF32 is decided here: the caller's cuDNN benchmark / deterministic settings are passed through)
             with torch.backends.cudnn.flags(enabled=True, benchmark=torch.backends.cudnn.benchmark,
                                             deterministic=torch.backends.cudnn.deterministic, allow_tf32=(C.MODE != "fp32")):
@@ -613,12 +673,8 @@ class MonoRecModel(nn.Module):
                 # cost_volume * (1 - cv_mask) (:713): the product is fused into the depth module's layout change and
                 # the masked volume is also materialised for callers that read data_dict["cost_volume"]
                 data_dict["_cv_mask_for_depth"] = data_dict["cv_mask"]
-                saved_range = self.depth_module.out_range
-                self.depth_module.out_range = (lo, hi - lo)               # (1-p)*lo + p*hi, :717-718
-                try:
-                    data_dict = self.depth_module(data_dict)
-                finally:       # a standalone DepthModule call keeps returning the reference's raw |tanh| heads
-                    self.depth_module.out_range = saved_range
+                # (1-p)*lo + p*hi (:717-718) in the heads' epilogue; a standalone DepthModule call returns the raw |tanh| heads
+                data_dict = self.depth_module(data_dict, out_range=(lo, hi - lo))
                 del data_dict["_cv_mask_for_depth"]
                 data_dict["cost_volume"] = C.mask_volume(data_dict["cost_volume"], data_dict["cv_mask"])
 
