@@ -131,6 +131,22 @@ int mr_cost_volume_fwd_matching(const float* keyframe, const float* const* frame
                                 int B, int F, int D, int H, int W,
                                 float alpha, const float* chan_w, int matching, int centered, void* stream);
 
+/* mr_cost_volume_fwd_matching with a choice of storage type for both volumes:
+ *   out_dtype     MR_DT_F32: out_cv / out_sfcv are fp32, the results are mr_cost_volume_fwd_matching's bit for bit;
+ *                 MR_DT_F16: both are IEEE half.  The march and the SSIM compute in fp32 as always and each single-frame value
+ *                 1 - 2 sad is rounded to half (nearest even) where it is stored, so out_sfcv is the fp32 result rounded.  The
+ *                 view weights, fusion and centring run in fp32 on the widened half single-frame values; only the store of
+ *                 out_cv rounds.  Invalid pixels and pixels with sum_f w_f == 0 are exactly 0 as in fp32.
+ *   out_cv, out_sfcv  non-null, 8-byte (fp32) / 4-byte (half) aligned
+ *   out_sfcv_nhwc, nhwc_dtype  as in mr_cost_volume_fwd_matching; with half volumes the copy holds the stored half values
+ *                 (widened for MR_DT_F32)
+ * Every other argument as in mr_cost_volume_fwd_matching.  All arguments are checked before the first CUDA call. */
+int mr_cost_volume_fwd_typed(const float* keyframe, const float* const* frames, const float* proj,
+                             const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv,
+                             void* out_sfcv_nhwc, int nhwc_dtype,
+                             int B, int F, int D, int H, int W,
+                             float alpha, const float* chan_w, int matching, int centered, int out_dtype, void* stream);
+
 /* Same path with HOST buffers (pinned or pageable): uploads the images and matrices, runs
  * mr_projection_tables + mr_cost_volume_fwd and downloads both volumes; batch elements are pipelined on
  * internal streams so copies overlap the kernel.  This is the end-to-end entry bench.py times as `e2e`.
@@ -151,6 +167,18 @@ int mr_cost_volume_host(const float* h_keyframe, const float* h_frames,
                         int B, int F, int D, int H, int W,
                         float inv_depth_lo, float inv_depth_hi, float alpha,
                         void* workspace, long long workspace_bytes);
+/* mr_cost_volume_host with half volumes (mr_cost_volume_fwd_typed's MR_DT_F16): h_out_cv [B,D,H,W] and h_out_sfcv
+ * [F,B,D,H,W] (or NULL) are IEEE half host buffers, half the bytes of the device-to-host copies.  Its workspace is smaller,
+ * hence its own size and offset functions; the same rules for the workspace and the internal streams apply. */
+long long mr_cost_volume_host_f16_workspace(int B, int F, int D, int H, int W);
+long long mr_cost_volume_host_f16_sfcv_offset(int B, int F, int D, int H, int W);
+int mr_cost_volume_host_f16(const float* h_keyframe, const float* h_frames,
+                            const float* h_keyframe_pose, const float* h_keyframe_K,
+                            const float* h_poses, const float* h_intrinsics,
+                            void* h_out_cv, void* h_out_sfcv,
+                            int B, int F, int D, int H, int W,
+                            float inv_depth_lo, float inv_depth_hi, float alpha,
+                            void* workspace, long long workspace_bytes);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Convolution engine for the MaskModule / DepthModule stacks (model/monorec/monorec_model.py:287-385, :476-557).
@@ -276,6 +304,12 @@ int mr_maxpool2_nhwc(const float* src, float* dst, int B, int H, int W, int C, v
 int mr_max_over_frames(const float* src, float* dst, int F, long long n_per_frame, void* stream);
 /* out[b,d,p] = volume[b,d,p] * (1 - mask[b,p])   (monorec_model.py:713, NCHW volume [B,D,HW], mask [B,HW]). */
 int mr_mask_volume(const float* volume, const float* mask, float* out, int B, int D, int HW, void* stream);
+/* The half volumes of mr_cost_volume_fwd_typed (MR_DT_F16): mr_nchw_to_nhwc / mr_nchw_to_nhwc_f16 with a half source,
+ * dst_dtype MR_DT_F32 or MR_DT_F16 (the product with 1 - scale in fp32 on the widened value, rounded once for a half
+ * destination), and mr_mask_volume with half volume and out (fp32 product, rounded once); mask stays fp32. */
+int mr_nchw_f16_to_nhwc(const void* src, void* dst, int dst_dtype, int B, int C, int H, int W, int dst_c, int dst_coff,
+                        const float* one_minus_scale, void* stream);
+int mr_mask_volume_f16(const void* volume, const float* mask, void* out, int B, int D, int HW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Evaluation-side helpers (SURVEY.md section 8f row 2).

@@ -35,9 +35,15 @@ SIGNATURES = {
     "mr_cost_volume_fwd_matching": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_int,
                                             c_int, c_void_p]),
+    "mr_cost_volume_fwd_typed": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_int,
+                                         c_int, c_int, c_void_p]),
     "mr_cost_volume_host_workspace": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
     "mr_cost_volume_host_sfcv_offset": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
     "mr_cost_volume_host": (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_float] * 3 + [c_void_p, c_longlong]),
+    "mr_cost_volume_host_f16_workspace": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
+    "mr_cost_volume_host_f16_sfcv_offset": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
+    "mr_cost_volume_host_f16": (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_float] * 3 + [c_void_p, c_longlong]),
     "mr_conv2d_nhwc": (c_int, [c_void_p, c_void_p]),
     "mr_sizeof_conv_desc": (c_int, []),
     "mr_pack_conv_weights_bytes": (c_longlong, [c_int, c_int, POINTER(c_int), c_int, c_int, c_int, POINTER(c_int), POINTER(c_int)]),
@@ -76,6 +82,8 @@ SIGNATURES = {
     "mr_reprojection_loss_bwd": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                          c_int, c_void_p, c_void_p]),
     "mr_mask_volume": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "mr_mask_volume_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "mr_nchw_f16_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
 }
 
 

@@ -131,10 +131,12 @@ def conv2d(srcs, weight, bias, kh, kw, stride=(1, 1), act=ACT_NONE, act_a=0.0, a
 
 
 def nchw_to_nhwc(x, out=None, out_coff=0, one_minus=None, dtype=None):
-    """fp32 (B,C,H,W) -> NHWC fp32 / half (optionally into a channel slice of `out`, optionally scaled by
-    (1 - one_minus[b,0,h,w]))."""
+    """fp32 or half (B,C,H,W) -> NHWC fp32 / half (optionally into a channel slice of `out`, optionally scaled by
+    (1 - one_minus[b,0,h,w])).  A half source (the half cost volumes) is widened in the kernel."""
     lib = _lib.load()
     dtype = (out.dtype if out is not None else dtype) or torch.float32
+    if x.dtype == torch.float16:
+        return _nchw_f16_to_nhwc(lib, x, out, out_coff, one_minus, dtype)
     if out is None and one_minus is None and x.dim() == 4 and x.dtype == torch.float32 and x.permute(0, 2, 3, 1).is_contiguous():
         v = x.permute(0, 2, 3, 1)             # already channels-last in memory (e.g. cuDNN NHWC output): a view, no kernel
         if dtype == torch.float32:
@@ -156,6 +158,26 @@ def nchw_to_nhwc(x, out=None, out_coff=0, one_minus=None, dtype=None):
         _lib.check(fn(x.data_ptr(), out.data_ptr(), B, C, H, W, out.shape[3], out_coff,
                       om_t.data_ptr() if om_t is not None else None, _stream(x)), name)
     return out        # (om_t stays referenced until the launch has been queued; the caching allocator is stream-ordered)
+
+
+def _one_minus_f32(one_minus, x):
+    """The kernels read fp32 [B,1,H,W]: any other dtype / shape would be read out of bounds."""
+    om_t = one_minus.to(device=x.device, dtype=torch.float32).contiguous()
+    assert om_t.numel() == x.shape[0] * x.shape[2] * x.shape[3], \
+        f"one_minus must hold one value per pixel (B,1,H,W), got {tuple(one_minus.shape)}"
+    return om_t
+
+
+def _nchw_f16_to_nhwc(lib, x, out, out_coff, one_minus, dtype):
+    x = x.contiguous()
+    B, C, H, W = x.shape
+    if out is None:
+        out = torch.empty(B, H, W, C, device=x.device, dtype=dtype)
+    om_t = None if one_minus is None else _one_minus_f32(one_minus, x)
+    with torch.cuda.device(x.device):
+        _lib.check(lib.mr_nchw_f16_to_nhwc(x.data_ptr(), out.data_ptr(), _dt(out), B, C, H, W, out.shape[3], out_coff,
+                                           om_t.data_ptr() if om_t is not None else None, _stream(x)), "mr_nchw_f16_to_nhwc")
+    return out
 
 
 def as_nhwc(x, dtype):
@@ -216,15 +238,15 @@ def pool_and_frame_max(x, frames):
 
 
 def mask_volume(volume, mask):
-    """cost_volume * (1 - cv_mask) on NCHW tensors (model/monorec/monorec_model.py:713)."""
+    """cost_volume * (1 - cv_mask) on NCHW tensors (model/monorec/monorec_model.py:713); a half volume gives a half result."""
     lib = _lib.load()
     volume = volume.contiguous()
     mask = mask.to(torch.float32).contiguous()
     B, D, H, W = volume.shape
     out = torch.empty_like(volume)
+    fn, name = (lib.mr_mask_volume_f16, "mr_mask_volume_f16") if volume.dtype == torch.float16 else (lib.mr_mask_volume, "mr_mask_volume")
     with torch.cuda.device(volume.device):
-        _lib.check(lib.mr_mask_volume(volume.data_ptr(), mask.data_ptr(), out.data_ptr(), B, D, H * W, _stream(volume)),
-                   "mr_mask_volume")
+        _lib.check(fn(volume.data_ptr(), mask.data_ptr(), out.data_ptr(), B, D, H * W, _stream(volume)), name)
     return out
 
 

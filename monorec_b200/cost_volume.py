@@ -29,6 +29,13 @@ def cv_matching_mode(use_ssim):
     return CV_BOX_L1
 
 
+def check_volume_dtype(dtype):
+    """The storage type of the cost volumes: torch.float32 or torch.float16; anything else is a ValueError."""
+    if dtype is not torch.float32 and dtype is not torch.float16:
+        raise ValueError(f"volume_dtype must be torch.float32 or torch.float16, got {dtype!r}")
+    return dtype
+
+
 def _as_f32c(t):
     if t.dtype != torch.float32 or not t.is_contiguous():
         t = t.to(torch.float32).contiguous()
@@ -43,11 +50,18 @@ class CostVolumeModule(nn.Module):
     uncentred fused volume, as the reference does.  use_mono / use_stereo select the frame lists exactly like the reference
     (:160-167).  use_ssim falsy, patch_size != 3 and sfcv_mult_mask=False raise NotImplementedError instead of silently
     running something else.
+
+    volume_dtype (not a reference argument) is the storage type of `cost_volume` and `single_frame_cvs`: torch.float32 (the
+    default) or torch.float16, which halves their memory and the bytes the kernel writes.  The arithmetic is fp32 either way:
+    each single-frame value is rounded to half where it is stored, and the fused volume is computed in fp32 from the stored
+    half single-frame values and rounded once.
     """
 
     def __init__(self, use_mono=True, use_stereo=False, use_ssim=True, patch_size=3,
-                 channel_weights=(5 / 32, 16 / 32, 11 / 32), alpha=10, not_center_cv=False, sfcv_mult_mask=True):
+                 channel_weights=(5 / 32, 16 / 32, 11 / 32), alpha=10, not_center_cv=False, sfcv_mult_mask=True,
+                 volume_dtype=torch.float32):
         super().__init__()
+        self.volume_dtype = check_volume_dtype(volume_dtype)
         self.use_mono = use_mono
         self.use_stereo = use_stereo
         self.use_ssim = use_ssim
@@ -108,8 +122,8 @@ class CostVolumeModule(nn.Module):
         with torch.cuda.device(dev):
             proj = torch.empty(B, F, 3, 4, device=dev, dtype=torch.float32)
             depths = torch.empty(D, device=dev, dtype=torch.float32) if pixel_depths is None else None
-            cv = torch.empty(B, D, H, W, device=dev, dtype=torch.float32)
-            sfcv = torch.empty(F, B, D, H, W, device=dev, dtype=torch.float32)
+            cv = torch.empty(B, D, H, W, device=dev, dtype=self.volume_dtype)
+            sfcv = torch.empty(F, B, D, H, W, device=dev, dtype=self.volume_dtype)
             _lib.check(lib.mr_projection_tables(kpose.data_ptr(), kK.data_ptr(), _lib.ptr_array(poses),
                                                 _lib.ptr_array(intrinsics), B, F, H, W, proj.data_ptr(),
                                                 None if depths is None else depths.data_ptr(), D, lo, hi, stream),
@@ -123,7 +137,17 @@ class CostVolumeModule(nn.Module):
             fill_nhwc = nhwc is not None and D <= 32 and D % 8 == 0 \
                 and tuple(nhwc.shape) == (F * B, H, W, D) and nhwc.is_contiguous() \
                 and nhwc.dtype in (torch.float32, torch.float16)
-            if self.matching != CV_SSIM or self.not_center_cv:
+            if self.volume_dtype == torch.float16:
+                # half volumes: one entry for every error mode, centring and depth source
+                _lib.check(lib.mr_cost_volume_fwd_typed(
+                    keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
+                    None if depths is None else depths.data_ptr(), None if pixel_depths is None else pixel_depths.data_ptr(),
+                    cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if fill_nhwc else None,
+                    1 if fill_nhwc and nhwc.dtype == torch.float16 else 0, B, F, D, H, W, float(self.alpha), cw,
+                    self.matching, 0 if self.not_center_cv else 1, 1, stream), "mr_cost_volume_fwd_typed")
+                if fill_nhwc:
+                    data_dict["_sfcv_nhwc_filled"] = True
+            elif self.matching != CV_SSIM or self.not_center_cv:
                 # the reference's non-default error modes and the uncentred volume, on either depth source
                 _lib.check(lib.mr_cost_volume_fwd_matching(
                     keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),

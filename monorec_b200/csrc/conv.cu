@@ -182,8 +182,12 @@ __global__ void __launch_bounds__(256) conv_cout1_kernel(const mr_conv_desc d) {
 __device__ __forceinline__ void st1(float* p, float v) { *p = v; }
 __device__ __forceinline__ void st1(__half* p, float v) { *p = __float2half_rn(v); }
 
-template <typename T>
-__global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, T* __restrict__ dst, int C, int HW, int dst_c,
+// source element widened to fp32 (the half cost volumes of mr_cost_volume_fwd_typed)
+__device__ __forceinline__ float ld1(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld1(const __half* p) { return __half2float(__ldg(p)); }
+
+template <typename T, typename S = float>
+__global__ void nchw_to_nhwc_kernel(const S* __restrict__ src, T* __restrict__ dst, int C, int HW, int dst_c,
                                     int dst_coff, const float* __restrict__ oms) {
     // one CTA: 32 pixels x 32 channels tile transposed through shared memory (coalesced on both sides)
     __shared__ float t[32][33];
@@ -191,7 +195,7 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, T* __restrict
     const int tx = threadIdx.x, ty = threadIdx.y;  // 32 x 8
     for (int j = ty; j < 32; j += 8) {
         const int c = c0 + j, p = p0 + tx;
-        t[j][tx] = (c < C && p < HW) ? __ldg(src + ((size_t)b * C + c) * HW + p) : 0.f;
+        t[j][tx] = (c < C && p < HW) ? ld1(src + ((size_t)b * C + c) * HW + p) : 0.f;
     }
     __syncthreads();
     for (int j = ty; j < 32; j += 8) {
@@ -207,16 +211,17 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, T* __restrict
 // Half-precision fast path of the layout change (C % 32 == 0, HW % 128 == 0, 16-byte aligned channel slice): a CTA moves
 // 32 channels x 128 pixels; 128-byte coalesced reads per channel row, conflict-free shared-memory transpose (pitch 129),
 // one 16-byte store (8 channels) per thread so that a warp writes 8 pixels x 64 contiguous bytes.
+template <typename S = float>
 __global__ void __launch_bounds__(256)
-nchw_to_nhwc_f16_tile_kernel(const float* __restrict__ src, __half* __restrict__ dst, int C, int HW, int dst_c, int dst_coff,
+nchw_to_nhwc_f16_tile_kernel(const S* __restrict__ src, __half* __restrict__ dst, int C, int HW, int dst_c, int dst_coff,
                              const float* __restrict__ oms) {
     __shared__ float t[32][129];
     const int b = blockIdx.z, p0 = blockIdx.x * 128, c0 = blockIdx.y * 32;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int j = warp; j < 32; j += 8) {
-        const float* s = src + ((size_t)b * C + c0 + j) * HW + p0 + lane;
+        const S* s = src + ((size_t)b * C + c0 + j) * HW + p0 + lane;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) t[j][lane + 32 * k] = __ldg(s + 32 * k);
+        for (int k = 0; k < 4; ++k) t[j][lane + 32 * k] = ld1(s + 32 * k);
     }
     __syncthreads();
 #pragma unroll
@@ -267,13 +272,14 @@ __global__ void max_over_frames_kernel(const float4* __restrict__ src, float4* _
     dst[i] = m;
 }
 
-__global__ void mask_volume_kernel(const float* __restrict__ vol, const float* __restrict__ mask,
-                                   float* __restrict__ out, int D, int HW, size_t total) {
+template <typename T = float>
+__global__ void mask_volume_kernel(const T* __restrict__ vol, const float* __restrict__ mask,
+                                   T* __restrict__ out, int D, int HW, size_t total) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const size_t b = i / ((size_t)D * HW);
     const int p = (int)(i % HW);
-    out[i] = (1.0f - __ldg(mask + b * HW + p)) * __ldg(vol + i);
+    st1(out + i, (1.0f - __ldg(mask + b * HW + p)) * ld1(vol + i));
 }
 
 }  // namespace
@@ -283,6 +289,15 @@ extern "C" int mr_mask_volume(const float* volume, const float* mask, float* out
     const size_t total = (size_t)B * D * HW;
     mask_volume_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(volume, mask, out, D, HW,
                                                                                           total);
+    MR_LAUNCH_CHECK("mask_volume_kernel");
+    return MR_OK;
+}
+
+extern "C" int mr_mask_volume_f16(const void* volume, const float* mask, void* out, int B, int D, int HW, void* stream) {
+    MR_REQUIRE(volume && mask && out && B >= 1 && D >= 1 && HW >= 1, "mr_mask_volume_f16: bad argument");
+    const size_t total = (size_t)B * D * HW;
+    mask_volume_kernel<__half><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        static_cast<const __half*>(volume), mask, static_cast<__half*>(out), D, HW, total);
     MR_LAUNCH_CHECK("mask_volume_kernel");
     return MR_OK;
 }
@@ -358,6 +373,33 @@ extern "C" int mr_nchw_to_nhwc_f16(const float* src, void* dst, int B, int C, in
     dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
     nchw_to_nhwc_kernel<__half><<<grid, block, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c, dst_coff,
                                                                           one_minus_scale);
+    MR_LAUNCH_CHECK("nchw_to_nhwc_kernel");
+    return MR_OK;
+}
+
+extern "C" int mr_nchw_f16_to_nhwc(const void* src_, void* dst, int dst_dtype, int B, int C, int H, int W, int dst_c,
+                                   int dst_coff, const float* one_minus_scale, void* stream) {
+    MR_REQUIRE(src_ && dst && B >= 1 && C >= 1 && H >= 1 && W >= 1, "mr_nchw_f16_to_nhwc: bad argument");
+    MR_REQUIRE(dst_dtype == MR_DT_F32 || dst_dtype == MR_DT_F16, "mr_nchw_f16_to_nhwc: dst_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)",
+               dst_dtype);
+    MR_REQUIRE(dst_coff >= 0 && dst_coff + C <= dst_c, "mr_nchw_f16_to_nhwc: channel slice out of range");
+    const __half* src = static_cast<const __half*>(src_);
+    const int HW = H * W;
+    if (dst_dtype == MR_DT_F16 && C % 32 == 0 && HW % 128 == 0 && dst_c % 8 == 0 && dst_coff % 8 == 0 &&
+        (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+        dim3 tgrid(HW / 128, C / 32, B);
+        nchw_to_nhwc_f16_tile_kernel<__half><<<tgrid, 256, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c,
+                                                                                   dst_coff, one_minus_scale);
+        MR_LAUNCH_CHECK("nchw_to_nhwc_f16_tile_kernel");
+        return MR_OK;
+    }
+    dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
+    if (dst_dtype == MR_DT_F16)
+        nchw_to_nhwc_kernel<__half, __half><<<grid, block, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c,
+                                                                                      dst_coff, one_minus_scale);
+    else
+        nchw_to_nhwc_kernel<float, __half><<<grid, block, 0, (cudaStream_t)stream>>>(src, static_cast<float*>(dst), C, HW, dst_c,
+                                                                                     dst_coff, one_minus_scale);
     MR_LAUNCH_CHECK("nchw_to_nhwc_kernel");
     return MR_OK;
 }

@@ -26,8 +26,8 @@
 //   CTA phase 2 (thread = pixel): view weight from max_d / sum_d exp(..), zeroing of invalid pixels, fusion over
 //           frames from the L2-hot single-frame volumes.
 // Template parameters: the depth source (plane table / per-pixel cv_depths), the error mode of stage 2 (SSIM, SSIM + L1 or
-// the 3x3 box of L1: the reference's use_ssim, monorec_model.py:227-243) and the centring of the fused volume
-// (not_center_cv, :267-269).
+// the 3x3 box of L1: the reference's use_ssim, monorec_model.py:227-243), the centring of the fused volume
+// (not_center_cv, :267-269) and the storage type of both volumes (fp32, or IEEE half: stores round, arithmetic stays fp32).
 // Keyframe-only terms (9 mu_y, 81 (sigma_y + C2)) are hoisted into a smem table per tile; pixels whose reprojection leaves
 // the source for any plane (valid_f = 0) are found by a projection pre-pass over the two extreme planes (the samples of
 // one pixel lie on a line, monotone in depth, so the extremes decide) and whole row ranges / frames of a tile are skipped.
@@ -68,8 +68,8 @@ struct CvArgs {
     const float* frames[MR_MAX_FRAMES];  // each [B,3,H,W]
     const float* proj;                   // [B,F,12]
     const float* depths;                 // [D]
-    float* cv;                           // [B,D,H,W]
-    float* sfcv;                         // [F,B,D,H,W]
+    void* cv;                            // [B,D,H,W] in the kernel's storage type OUT (fp32 or IEEE half)
+    void* sfcv;                          // [F,B,D,H,W], OUT
     void* sf_nhwc;                       // optional [F,B,H,W,D] copy of sfcv for the conv engine (D <= 32, D % 8 == 0) or nullptr
     int sf_nhwc_half;                    // 1: that copy is IEEE half, 0: fp32
     int B, F, D, H, W, TH, b0;
@@ -163,6 +163,23 @@ __device__ __forceinline__ void st_hint_f2(float* ptr, float2 v, uint64_t pol) {
 __device__ __forceinline__ void st_hint_f1(float* ptr, float v, uint64_t pol) {
     asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(ptr), "f"(v), "l"(pol) : "memory");
 }
+
+// Stores of the volumes in their storage type OUT (float or IEEE half).  Half rounds each fp32 value once, to nearest even
+// (__floats2half2_rn rounds both halves exactly like two __float2half_rn).
+__device__ __forceinline__ void st_vol2(float* ptr, float2 v, uint64_t pol) { st_hint_f2(ptr, v, pol); }
+__device__ __forceinline__ void st_vol1(float* ptr, float v, uint64_t pol) { st_hint_f1(ptr, v, pol); }
+__device__ __forceinline__ void st_vol2(__half* ptr, float2 v, uint64_t pol) {
+    const __half2 h = __floats2half2_rn(v.x, v.y);
+    asm volatile("st.global.L2::cache_hint.b32 [%0], %1, %2;" ::"l"(ptr), "r"(*reinterpret_cast<const uint32_t*>(&h)), "l"(pol)
+                 : "memory");
+}
+__device__ __forceinline__ void st_vol1(__half* ptr, float v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.b16 [%0], %1, %2;" ::"l"(ptr), "h"(__half_as_ushort(__float2half_rn(v))), "l"(pol)
+                 : "memory");
+}
+// the per-pixel phase's read-back of one single-frame value (L2 only: written by this CTA's march), widened to fp32
+__device__ __forceinline__ float ld_vol(const float* ptr) { return __ldcg(ptr); }
+__device__ __forceinline__ float ld_vol(const __half* ptr) { return __half2float(__ldcg(ptr)); }
 
 // ---- mbarrier / TMA wrappers ----------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -465,8 +482,8 @@ struct Stage2State<kErrBoxL1> {
 
 // Patch cost of one row step, common to every error mode: E is the channel-weighted error of the lane's two columns in the
 // row whose error was just finished; its horizontal 3-sum joins the two rows before it in hE (rolling like Stage2State).
-template <int P>
-__device__ __forceinline__ void patch_cost_row(float2 (&hE)[3], const Stage2Ctx& c, const float2 E, float* out,
+template <int P, typename OUT>
+__device__ __forceinline__ void patch_cost_row(float2 (&hE)[3], const Stage2Ctx& c, const float2 E, OUT* out,
                                                const bool store) {
     constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
     const float eL = __shfl_up_sync(0xffffffffu, E.y, 1);
@@ -477,10 +494,11 @@ __device__ __forceinline__ void patch_cost_row(float2 (&hE)[3], const Stage2Ctx&
     // per-pixel phase (which zeroes invalid pixels) once all planes are known
     const float2 sv = make_float2(fmaf(-2.0f, (hE[P1].x + hE[P2].x) + hEc.x, 1.0f),
                                   fmaf(-2.0f, (hE[P1].y + hE[P2].y) + hEc.y, 1.0f));
-    // predicated stores (no divergent branch in the row loop): the lane's pair as one 8-byte store, or its single column
-    if (store && c.pairflag) st_hint_f2(out, sv, c.pol_keep);
-    if (store && c.st0) st_hint_f1(out, sv.x, c.pol_keep);
-    if (store && c.st1) st_hint_f1(out + 1, sv.y, c.pol_keep);
+    // predicated stores (no divergent branch in the row loop): the lane's pair as one 8-byte (half: 4-byte) store, or its
+    // single column
+    if (store && c.pairflag) st_vol2(out, sv, c.pol_keep);
+    if (store && c.st0) st_vol1(out, sv.x, c.pol_keep);
+    if (store && c.st1) st_vol1(out + 1, sv.y, c.pol_keep);
     hE[P] = hEc;
 }
 
@@ -492,9 +510,9 @@ __device__ __forceinline__ void patch_cost_row(float2 (&hE)[3], const Stage2Ctx&
 // ERR: kErrSsim or kErrSsimL1 (kErrBoxL1 is box_l1_row below).  The row buffer and the keyframe tile both hold values
 // + 0.5, so the |X - Y| of kErrSsimL1 and kErrBoxL1 is |(w + .5) - (k + .5)|: it differs from the reference's |w - k| by the
 // rounding of the two additions (of order 1e-7).
-template <int P, int ERR>
+template <int P, int ERR, typename OUT>
 __device__ __forceinline__ void ssim_row(Stage2State<ERR>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
-                                         const uint32_t cr, float* out, const bool store, const uint32_t xb) {
+                                         const uint32_t cr, OUT* out, const bool store, const uint32_t xb) {
     constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
     float2 xl[3], xrr[3], yl[3], yrr[3];
     float4 k4[3];
@@ -568,9 +586,9 @@ __device__ __forceinline__ void ssim_row(Stage2State<ERR>& st, const Stage2Ctx& 
 
 // kErrBoxL1: horizontal 3-sums of |X - Y| of the new row, their vertical 3-sum over the rolling rows (the 3x3 box of the
 // row above, at the step where the SSIM modes finish that row's SSIM), patch cost of the row above that
-template <int P>
+template <int P, typename OUT>
 __device__ __forceinline__ void box_l1_row(Stage2State<kErrBoxL1>& st, const Stage2Ctx& c, const uint32_t xr,
-                                           const uint32_t yr, float* out, const bool store) {
+                                           const uint32_t yr, OUT* out, const bool store) {
     constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
     float2 xl[3], xrr[3], yl[3], yrr[3];
     xl[0] = lds64<0>(xr);                  xrr[0] = lds64<8>(xr);
@@ -596,9 +614,9 @@ __device__ __forceinline__ void box_l1_row(Stage2State<kErrBoxL1>& st, const Sta
 }
 
 // xb: the lane's address in the warp's first row buffer (xr without the buffer toggle)
-template <int P, int ERR>
+template <int P, int ERR, typename OUT>
 __device__ __forceinline__ void stage2_row(Stage2State<ERR>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
-                                           const uint32_t cr, float* out, const bool store, const uint32_t xb) {
+                                           const uint32_t cr, OUT* out, const bool store, const uint32_t xb) {
     if constexpr (ERR == kErrBoxL1) box_l1_row<P>(st, c, xr, yr, out, store);
     else ssim_row<P, ERR>(st, c, xr, yr, cr, out, store, xb);
 }
@@ -609,10 +627,10 @@ __device__ __forceinline__ void stage2_row(Stage2State<ERR>& st, const Stage2Ctx
 //   xb: shared address of this warp's two row buffers; yr / cr: keyframe row rlo-2 / table row rlo-2 (lane columns);
 //   out: single-frame volume at output row rlo - 4 (advanced every step, stored from the fifth step on); wstride = W
 //   PIX: per-pixel depths, read from image row v0 (= fv0) on; each row's depths are loaded one row step before they are used
-//   ERR: the error mode of stage 2
-template <int MODE, bool PIX, int ERR>
+//   ERR: the error mode of stage 2; OUT: the storage type of the single-frame volume
+template <int MODE, bool PIX, int ERR, typename OUT>
 __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx& c2, const uint32_t xb, const int lane,
-                                           const float fv0, const int nsteps, uint32_t yr, uint32_t cr, float* out,
+                                           const float fv0, const int nsteps, uint32_t yr, uint32_t cr, OUT* out,
                                            const int wstride, const int v0 = 0) {
     Stage2State<ERR> st;
     st.clear();
@@ -684,9 +702,11 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
 //      read back exactly once; max / sum over the planes are combined across the T lanes by shuffles.
 //      CENTER = false (not_center_cv, :267-269) stores the fused sad sum_f w_f sad_f / sum_f w_f = (1 - cv) / 2 instead,
 //      still 0 where sum_f w_f == 0.
+//      OUT = __half: the single-frame values are read back as half and widened; weights, fusion and centring stay fp32 and
+//      only the store of the fused volume rounds to half.
 struct PixelPhase {
-    float* cv;
-    float* sfcv;
+    void* cv;                            // OUT [B,D,H,W]
+    void* sfcv;                          // OUT [F,B,D,H,W]
     void* sf_nhwc;
     int sf_nhwc_half;
     const unsigned char* vmask;
@@ -695,7 +715,7 @@ struct PixelPhase {
     uint64_t pol_stream;
 };
 
-template <int T, bool CENTER>
+template <int T, bool CENTER, typename OUT>
 __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
     constexpr int kSlots = 32 / T;                       // pixels per warp iteration
     // the thread index is read again here (volatile: not merged with the kernel's own read) instead of being kept live in a
@@ -707,7 +727,7 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
     const int D = c.D, F = c.F, TH = c.TH;
     const int d_lo = chunk * kChunk;                     // this lane's planes [d_lo, d_lo + kChunk) of D
     const size_t plane = (size_t)c.H * c.W;
-    const size_t pstride = plane * sizeof(float);        // bytes between the planes of a pixel
+    const size_t pstride = plane * sizeof(OUT);          // bytes between the planes of a pixel
     const size_t fstride = (size_t)c.B * D * pstride;    // bytes between the frames
     const int vstride = TH * kTileCols;
     const int per_iter = kWarps * kSlots;
@@ -719,8 +739,8 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
         if (T == 1 && !own) continue;                    // (with T > 1 every lane stays for the shuffles)
         const size_t pix = own ? (size_t)v * c.W + u : 0;
         // addresses advance by pointer increments (one 64-bit add per access; an index expression costs a wide multiply each)
-        char* cv_out = reinterpret_cast<char*>(c.cv + ((size_t)c.b * D + d_lo) * plane + pix);
-        char* sf = reinterpret_cast<char*>(c.sfcv + ((size_t)c.b * D + d_lo) * plane + pix);       // frame f: + f * fstride
+        char* cv_out = reinterpret_cast<char*>(static_cast<OUT*>(c.cv) + ((size_t)c.b * D + d_lo) * plane + pix);
+        char* sf = reinterpret_cast<char*>(static_cast<OUT*>(c.sfcv) + ((size_t)c.b * D + d_lo) * plane + pix);  // frame f: + f * fstride
         float acc[kChunk], vv[kChunk], nv[kChunk];
 #pragma unroll
         for (int j = 0; j < kChunk; ++j) acc[j] = 0.f;
@@ -731,10 +751,10 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
             if (own && (c.vmask[f * vstride + p] != 0)) {
                 if (D == T * kChunk) {                   // 32 / 64 / 128 planes: no per-plane predicates
 #pragma unroll
-                    for (int j = 0; j < kChunk; ++j, q += pstride) nv[j] = __ldcg(reinterpret_cast<const float*>(q));
+                    for (int j = 0; j < kChunk; ++j, q += pstride) nv[j] = ld_vol(reinterpret_cast<const OUT*>(q));
                 } else {
 #pragma unroll
-                    for (int j = 0; j < kChunk; ++j, q += pstride) nv[j] = (d_lo + j < D) ? __ldcg(reinterpret_cast<const float*>(q)) : -2.0f;
+                    for (int j = 0; j < kChunk; ++j, q += pstride) nv[j] = (d_lo + j < D) ? ld_vol(reinterpret_cast<const OUT*>(q)) : -2.0f;
                 }
             } else {
 #pragma unroll
@@ -756,8 +776,13 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
             char* q = sf;
             if (own && !valid) {                         // invalid pixel of frame f: the whole plane stack is 0
 #pragma unroll 4
-                for (int j = 0; j < kChunk; ++j, q += pstride)
-                    if (d_lo + j < D) *reinterpret_cast<float*>(q) = 0.f;
+                for (int j = 0; j < kChunk; ++j, q += pstride) {
+                    if constexpr (std::is_same<OUT, float>::value) {
+                        if (d_lo + j < D) *reinterpret_cast<float*>(q) = 0.f;
+                    } else {
+                        if (d_lo + j < D) *reinterpret_cast<unsigned short*>(q) = 0;   // +0 in half
+                    }
+                }
                 if (nh != nullptr)
                     for (int o = 0; o < D * (c.sf_nhwc_half ? 2 : 4); o += 16) *reinterpret_cast<uint4*>(nh + o) = make_uint4(0, 0, 0, 0);
             }
@@ -812,20 +837,21 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
         if constexpr (CENTER) {
 #pragma unroll
             for (int j = 0; j < kChunk; ++j, q += pstride)
-                if (D == T * kChunk || d_lo + j < D) st_hint_f1(reinterpret_cast<float*>(q), acc[j] * inv, c.pol_stream);
+                if (D == T * kChunk || d_lo + j < D) st_vol1(reinterpret_cast<OUT*>(q), acc[j] * inv, c.pol_stream);
         } else {
             const float h = (wsum == 0.f) ? 0.f : 0.5f;
 #pragma unroll
             for (int j = 0; j < kChunk; ++j, q += pstride)
-                if (D == T * kChunk || d_lo + j < D) st_hint_f1(reinterpret_cast<float*>(q), fmaf(-h, acc[j] * inv, h), c.pol_stream);
+                if (D == T * kChunk || d_lo + j < D) st_vol1(reinterpret_cast<OUT*>(q), fmaf(-h, acc[j] * inv, h), c.pol_stream);
         }
     }
 }
 
 // PIX selects the depth source: false = one depth per plane (a.depths = zs[D], the default linspace planes), true = one depth
 // per plane and pixel (a.depths = cv_depths [B,D,H,W]).  ERR is the error mode of stage 2 (use_ssim), CENTER false stores the
-// uncentred fused volume (not_center_cv).
-template <bool PIX, int ERR, bool CENTER>
+// uncentred fused volume (not_center_cv).  OUT is the storage type of both volumes: float, or __half (the march and the
+// per-pixel phase compute in fp32 either way; only the stores round, and the per-pixel phase widens what it reads back).
+template <bool PIX, int ERR, bool CENTER, typename OUT>
 __global__ void __launch_bounds__(kThreads, kMinBlocks)
 cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -1158,7 +1184,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
         // the SSIM row of step t is tile row rlo-3+t, whose table row is rlo-2+t (t = 0, 1 read throw-away rows, possibly
         // in front of the table: still inside this CTA's shared memory, see make_layout)
         const uint32_t cr = cs_s + (rlo - 2) * kCRowBytes;
-        float* out = a.sfcv + (((size_t)f * a.B + b) * D + d) * plane + ((ptrdiff_t)(v0 + rlo - 4) * W + ucol);
+        OUT* out = static_cast<OUT*>(a.sfcv) + (((size_t)f * a.B + b) * D + d) * plane + ((ptrdiff_t)(v0 + rlo - 4) * W + ucol);
         const unsigned g = gid[unit];
         if (g != 0xFFFFu) {
             const GroupInfo gi = ginfo[g];
@@ -1212,9 +1238,9 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     // exp(-alpha (sad - min sad)^2) with sad = (1 - sv) / 2 is ex2(-(k (max sv - sv))^2), k = sqrt(alpha log2(e)) / 2
     pp.kq = 0.5f * sqrtf(a.alpha * 1.4426950408889634f);
     pp.pol_stream = pol_stream;
-    if (D <= kChunk) pixel_phase<1, CENTER>(pp);
-    else if (D <= 2 * kChunk) pixel_phase<2, CENTER>(pp);
-    else pixel_phase<4, CENTER>(pp);
+    if (D <= kChunk) pixel_phase<1, CENTER, OUT>(pp);
+    else if (D <= 2 * kChunk) pixel_phase<2, CENTER, OUT>(pp);
+    else pixel_phase<4, CENTER, OUT>(pp);
 }
 
 // ----------------------------------------------------------------------------------------------------------------
@@ -1301,7 +1327,7 @@ int pick_tile_rows(int D, int F, int use_tma, bool pix, int err) {
     return 0;
 }
 
-template <bool PIX, int ERR, bool CENTER>
+template <bool PIX, int ERR, bool CENTER, typename OUT>
 int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
     // The opt-in is per function and per device context, so it is remembered per device (bit d: device d; devices from 64 on
     // set it before every launch).  Two threads that both find the bit clear both set the attribute: harmless.
@@ -1310,26 +1336,26 @@ int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, con
     MR_CUDA(cudaGetDevice(&dev));
     const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
     if ((opted_in.load(std::memory_order_acquire) & bit) == 0) {
-        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX, ERR, CENTER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX, ERR, CENTER, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      227 * 1024));
         opted_in.fetch_or(bit, std::memory_order_release);
     }
-    cost_volume_kernel<PIX, ERR, CENTER><<<grid, kThreads, smem, stream>>>(a, maps);
+    cost_volume_kernel<PIX, ERR, CENTER, OUT><<<grid, kThreads, smem, stream>>>(a, maps);
     MR_LAUNCH_CHECK("cost_volume_kernel");
     return MR_OK;
 }
 
 // the instantiation for (error mode, centring); matching was checked by the caller
-template <bool PIX>
+template <bool PIX, typename OUT>
 int launch_variant(int matching, int centered, dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
     if (matching == kErrSsimL1)
-        return centered ? launch_kernel<PIX, kErrSsimL1, true>(grid, smem, stream, a, maps)
-                        : launch_kernel<PIX, kErrSsimL1, false>(grid, smem, stream, a, maps);
+        return centered ? launch_kernel<PIX, kErrSsimL1, true, OUT>(grid, smem, stream, a, maps)
+                        : launch_kernel<PIX, kErrSsimL1, false, OUT>(grid, smem, stream, a, maps);
     if (matching == kErrBoxL1)
-        return centered ? launch_kernel<PIX, kErrBoxL1, true>(grid, smem, stream, a, maps)
-                        : launch_kernel<PIX, kErrBoxL1, false>(grid, smem, stream, a, maps);
-    return centered ? launch_kernel<PIX, kErrSsim, true>(grid, smem, stream, a, maps)
-                    : launch_kernel<PIX, kErrSsim, false>(grid, smem, stream, a, maps);
+        return centered ? launch_kernel<PIX, kErrBoxL1, true, OUT>(grid, smem, stream, a, maps)
+                        : launch_kernel<PIX, kErrBoxL1, false, OUT>(grid, smem, stream, a, maps);
+    return centered ? launch_kernel<PIX, kErrSsim, true, OUT>(grid, smem, stream, a, maps)
+                    : launch_kernel<PIX, kErrSsim, false, OUT>(grid, smem, stream, a, maps);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1372,11 +1398,12 @@ extern "C" int mr_projection_tables(const float* keyframe_pose, const float* key
 }
 
 int mr::launch_cost_volume(const float* keyframe, const float* const* frames, const float* proj,
-                           const float* depths, float* out_cv, float* out_sfcv, int B, int F, int D, int H, int W,
+                           const float* depths, void* out_cv, void* out_sfcv, int B, int F, int D, int H, int W,
                            float alpha, const float* chan_w, int b_begin, int b_count, int gather_only,
                            cudaStream_t stream, void* sf_nhwc, int sf_nhwc_dtype, int per_pixel_depths, int matching,
-                           int centered) {
+                           int centered, int out_dtype) {
     MR_REQUIRE(keyframe && frames && proj && depths && out_cv && out_sfcv, "mr_cost_volume_fwd: null pointer");
+    MR_REQUIRE(out_dtype == MR_DT_F32 || out_dtype == MR_DT_F16, "mr_cost_volume_fwd: unknown out_dtype %d", out_dtype);
     MR_REQUIRE(b_begin >= 0 && b_count >= 1 && b_begin + b_count <= B, "mr_cost_volume_fwd: bad batch range");
     MR_REQUIRE(B >= 1 && B <= 21845, "mr_cost_volume_fwd: batch %d out of range", B);
     MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "mr_cost_volume_fwd: 1 <= F <= %d required (got %d)", MR_MAX_FRAMES, F);
@@ -1429,8 +1456,11 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
     a.cw0 = cw[0] / 9.f; a.cw1 = cw[1] / 9.f; a.cw2 = cw[2] / 9.f;  // monorec_model.py:141 (weights / patch_size^2)
     const SmemLayout L = make_layout(D, a.TH, F, a.use_tma, pix, matching);
     dim3 grid((W + kOutCols - 1) / kOutCols, (H + a.TH - 1) / a.TH, b_count);
-    return pix ? launch_variant<true>(matching, centered, grid, L.total, stream, a, local)
-               : launch_variant<false>(matching, centered, grid, L.total, stream, a, local);
+    if (out_dtype == MR_DT_F16)
+        return pix ? launch_variant<true, __half>(matching, centered, grid, L.total, stream, a, local)
+                   : launch_variant<false, __half>(matching, centered, grid, L.total, stream, a, local);
+    return pix ? launch_variant<true, float>(matching, centered, grid, L.total, stream, a, local)
+               : launch_variant<false, float>(matching, centered, grid, L.total, stream, a, local);
 }
 
 extern "C" int mr_cost_volume_fwd(const float* keyframe, const float* const* frames, const float* proj,
@@ -1470,27 +1500,56 @@ extern "C" int mr_cost_volume_fwd_depthmap(const float* keyframe, const float* c
                                   0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, 1);
 }
 
+namespace {
+// the checks the general entries share; fn names the entry in the messages
+int check_general_args(const char* fn, const float* depths, const float* pixel_depths, int nhwc_dtype, int F, int D,
+                       int matching, int centered) {
+    if (matching == 0) {   // use_ssim falsy: the plain |w - k| difference (monorec_model.py:227-228)
+        ::mr::set_error("%s: matching 0 (plain L1 difference) is not implemented", fn);
+        return MR_ENOSUPPORT;
+    }
+    MR_REQUIRE(matching == MR_CV_SSIM || matching == MR_CV_SSIM_L1 || matching == MR_CV_BOX_L1,
+               "%s: unknown matching %d (MR_CV_SSIM, MR_CV_SSIM_L1 or MR_CV_BOX_L1)", fn, matching);
+    MR_REQUIRE(centered == 0 || centered == 1, "%s: centered must be 0 or 1 (got %d)", fn, centered);
+    MR_REQUIRE((depths == nullptr) != (pixel_depths == nullptr),
+               "%s: exactly one of depths / pixel_depths must be given (got %s)", fn, depths ? "both" : "neither");
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(pixel_depths) & 3) == 0, "%s: pixel_depths must be 4-byte aligned", fn);
+    MR_REQUIRE(D >= 2 && D <= 128, "%s: 2 <= D <= 128 required (got D=%d)", fn, D);
+    MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "%s: 1 <= F <= %d required (got F=%d)", fn, MR_MAX_FRAMES, F);
+    MR_REQUIRE(nhwc_dtype == MR_DT_F32 || nhwc_dtype == MR_DT_F16,
+               "%s: nhwc_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", fn, nhwc_dtype);
+    return MR_OK;
+}
+}  // namespace
+
 extern "C" int mr_cost_volume_fwd_matching(const float* keyframe, const float* const* frames, const float* proj,
                                            const float* depths, const float* pixel_depths, float* out_cv, float* out_sfcv,
                                            void* out_sfcv_nhwc, int nhwc_dtype, int B, int F, int D, int H, int W, float alpha,
                                            const float* chan_w, int matching, int centered, void* stream) {
-    if (matching == 0) {   // use_ssim falsy: the plain |w - k| difference (monorec_model.py:227-228)
-        ::mr::set_error("mr_cost_volume_fwd_matching: matching 0 (plain L1 difference) is not implemented");
-        return MR_ENOSUPPORT;
-    }
-    MR_REQUIRE(matching == MR_CV_SSIM || matching == MR_CV_SSIM_L1 || matching == MR_CV_BOX_L1,
-               "mr_cost_volume_fwd_matching: unknown matching %d (MR_CV_SSIM, MR_CV_SSIM_L1 or MR_CV_BOX_L1)", matching);
-    MR_REQUIRE(centered == 0 || centered == 1, "mr_cost_volume_fwd_matching: centered must be 0 or 1 (got %d)", centered);
-    MR_REQUIRE((depths == nullptr) != (pixel_depths == nullptr),
-               "mr_cost_volume_fwd_matching: exactly one of depths / pixel_depths must be given (got %s)",
-               depths ? "both" : "neither");
-    MR_REQUIRE((reinterpret_cast<uintptr_t>(pixel_depths) & 3) == 0,
-               "mr_cost_volume_fwd_matching: pixel_depths must be 4-byte aligned");
-    MR_REQUIRE(D >= 2 && D <= 128, "mr_cost_volume_fwd_matching: 2 <= D <= 128 required (got D=%d)", D);
-    MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "mr_cost_volume_fwd_matching: 1 <= F <= %d required (got F=%d)", MR_MAX_FRAMES, F);
-    MR_REQUIRE(nhwc_dtype == MR_DT_F32 || nhwc_dtype == MR_DT_F16,
-               "mr_cost_volume_fwd_matching: nhwc_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", nhwc_dtype);
+    const int rc = check_general_args("mr_cost_volume_fwd_matching", depths, pixel_depths, nhwc_dtype, F, D, matching, centered);
+    if (rc != MR_OK) return rc;
     const int pix = pixel_depths != nullptr;
     return mr::launch_cost_volume(keyframe, frames, proj, pix ? pixel_depths : depths, out_cv, out_sfcv, B, F, D, H, W, alpha,
                                   chan_w, 0, B, 0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, pix, matching, centered);
+}
+
+extern "C" int mr_cost_volume_fwd_typed(const float* keyframe, const float* const* frames, const float* proj,
+                                        const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv,
+                                        void* out_sfcv_nhwc, int nhwc_dtype, int B, int F, int D, int H, int W, float alpha,
+                                        const float* chan_w, int matching, int centered, int out_dtype, void* stream) {
+    const char* fn = "mr_cost_volume_fwd_typed";
+    MR_REQUIRE(out_dtype == MR_DT_F32 || out_dtype == MR_DT_F16, "%s: out_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", fn,
+               out_dtype);
+    const int rc = check_general_args(fn, depths, pixel_depths, nhwc_dtype, F, D, matching, centered);
+    if (rc != MR_OK) return rc;
+    // the march stores two columns at once: 8 bytes (fp32) / 4 bytes (half)
+    const uintptr_t align = out_dtype == MR_DT_F16 ? 3 : 7;
+    MR_REQUIRE(out_cv != nullptr && (reinterpret_cast<uintptr_t>(out_cv) & align) == 0,
+               "%s: out_cv must be a non-null, %d-byte aligned buffer", fn, (int)align + 1);
+    MR_REQUIRE(out_sfcv != nullptr && (reinterpret_cast<uintptr_t>(out_sfcv) & align) == 0,
+               "%s: out_sfcv must be a non-null, %d-byte aligned buffer", fn, (int)align + 1);
+    const int pix = pixel_depths != nullptr;
+    return mr::launch_cost_volume(keyframe, frames, proj, pix ? pixel_depths : depths, out_cv, out_sfcv, B, F, D, H, W, alpha,
+                                  chan_w, 0, B, 0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, pix, matching, centered,
+                                  out_dtype);
 }

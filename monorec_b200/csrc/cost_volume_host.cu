@@ -1,4 +1,5 @@
-// Host-buffer entry of the cost-volume path (include/monorec_b200.h: mr_cost_volume_host).
+// Host-buffer entries of the cost-volume path (include/monorec_b200.h: mr_cost_volume_host, and mr_cost_volume_host_f16 with
+// half volumes).
 // Batch elements are pipelined over a small ring of internal streams: the H2D copy of element b+1 and the D2H copy
 // of element b-1 overlap the kernel of element b.  The caller owns the device workspace; the streams and the event are
 // created once per host thread and device and reused by later calls.
@@ -11,7 +12,8 @@ struct HostPlan {
     size_t img, mats, proj, depths, cv, sfcv, total;  // byte offsets into the workspace
 };
 
-HostPlan plan(int B, int F, int D, int H, int W) {
+// vb: bytes per volume element (4: fp32, 2: half)
+HostPlan plan(int B, int F, int D, int H, int W, int vb = 4) {
     auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
     HostPlan p;
     size_t off = 0;
@@ -19,8 +21,8 @@ HostPlan plan(int B, int F, int D, int H, int W) {
     p.mats = off;   off = al(off + (size_t)(2 + 2 * F) * B * 16 * 4);
     p.proj = off;   off = al(off + (size_t)B * F * 12 * 4);
     p.depths = off; off = al(off + (size_t)D * 4);
-    p.cv = off;     off = al(off + (size_t)B * D * H * W * 4);
-    p.sfcv = off;   off = al(off + (size_t)F * B * D * H * W * 4);
+    p.cv = off;     off = al(off + (size_t)B * D * H * W * vb);
+    p.sfcv = off;   off = al(off + (size_t)F * B * D * H * W * vb);
     p.total = off;
     return p;
 }
@@ -63,23 +65,36 @@ extern "C" long long mr_cost_volume_host_sfcv_offset(int B, int F, int D, int H,
     return (long long)plan(B, F, D, H, W).sfcv;
 }
 
-extern "C" int mr_cost_volume_host(const float* h_keyframe, const float* h_frames, const float* h_keyframe_pose,
-                                   const float* h_keyframe_K, const float* h_poses, const float* h_intrinsics,
-                                   float* h_out_cv, float* h_out_sfcv, int B, int F, int D, int H, int W,
-                                   float inv_depth_lo, float inv_depth_hi, float alpha, void* workspace,
-                                   long long workspace_bytes) {
+extern "C" long long mr_cost_volume_host_f16_workspace(int B, int F, int D, int H, int W) {
+    if (B < 1 || F < 1 || D < 2 || H < 5 || W < 5) return 0;
+    return (long long)plan(B, F, D, H, W, 2).total;
+}
+
+extern "C" long long mr_cost_volume_host_f16_sfcv_offset(int B, int F, int D, int H, int W) {
+    if (B < 1 || F < 1 || D < 2 || H < 5 || W < 5) return -1;
+    return (long long)plan(B, F, D, H, W, 2).sfcv;
+}
+
+namespace {
+
+// both host entries; out_dtype MR_DT_F32 / MR_DT_F16 is the type of the volumes on the device and in the host buffers
+int cost_volume_host(const char* fn, const float* h_keyframe, const float* h_frames, const float* h_keyframe_pose,
+                     const float* h_keyframe_K, const float* h_poses, const float* h_intrinsics, void* h_out_cv,
+                     void* h_out_sfcv, int B, int F, int D, int H, int W, float inv_depth_lo, float inv_depth_hi, float alpha,
+                     void* workspace, long long workspace_bytes, int out_dtype) {
     MR_REQUIRE(h_keyframe && h_frames && h_keyframe_pose && h_keyframe_K && h_poses && h_intrinsics && h_out_cv && workspace,
-               "mr_cost_volume_host: null pointer");
+               "%s: null pointer", fn);
     MR_REQUIRE(B >= 1 && F >= 1 && F <= MR_MAX_FRAMES && D >= 2 && D <= 128 && H >= 5 && W >= 5,
-               "mr_cost_volume_host: bad shape B=%d F=%d D=%d H=%d W=%d", B, F, D, H, W);
-    const HostPlan p = plan(B, F, D, H, W);
+               "%s: bad shape B=%d F=%d D=%d H=%d W=%d", fn, B, F, D, H, W);
+    const int vb = out_dtype == MR_DT_F16 ? 2 : 4;
+    const HostPlan p = plan(B, F, D, H, W, vb);
     if ((long long)p.total > workspace_bytes) {
-        mr::set_error("mr_cost_volume_host: workspace too small (%lld < %zu bytes)", workspace_bytes, p.total);
+        mr::set_error("%s: workspace too small (%lld < %zu bytes)", fn, workspace_bytes, p.total);
         return MR_ENOMEM;
     }
     char* ws = static_cast<char*>(workspace);
     const size_t img1 = (size_t)3 * H * W;  // floats per image
-    const size_t vol1 = (size_t)D * H * W;  // floats per volume
+    const size_t vol1 = (size_t)D * H * W;  // elements per volume
     float* d_key = reinterpret_cast<float*>(ws + p.img);     // [B,3,H,W]
     float* d_frames = d_key + (size_t)B * img1;              // [F,B,3,H,W]
     float* d_kpose = reinterpret_cast<float*>(ws + p.mats);  // [B,16]
@@ -88,8 +103,10 @@ extern "C" int mr_cost_volume_host(const float* h_keyframe, const float* h_frame
     float* d_intr = d_poses + (size_t)F * B * 16;            // [F,B,16]
     float* d_proj = reinterpret_cast<float*>(ws + p.proj);
     float* d_depths = reinterpret_cast<float*>(ws + p.depths);
-    float* d_cv = reinterpret_cast<float*>(ws + p.cv);
-    float* d_sfcv = reinterpret_cast<float*>(ws + p.sfcv);
+    char* d_cv = ws + p.cv;
+    char* d_sfcv = ws + p.sfcv;
+    char* o_cv = static_cast<char*>(h_out_cv);
+    char* o_sfcv = static_cast<char*>(h_out_sfcv);
 
     StreamRing& ring = g_ring;
     int rc = ring.init();
@@ -121,12 +138,14 @@ extern "C" int mr_cost_volume_host(const float* h_keyframe, const float* h_frame
                 MR_CUDA(cudaMemcpyAsync(d_frames + o, h_frames + o, img1 * 4, cudaMemcpyHostToDevice, s));
             }
             MR_CUDA(cudaStreamWaitEvent(s, ring.ready, 0));
-            rc = mr::launch_cost_volume(d_key, fp, d_proj, d_depths, d_cv, d_sfcv, B, F, D, H, W, alpha, nullptr, b, 1, 0, s);
+            rc = mr::launch_cost_volume(d_key, fp, d_proj, d_depths, d_cv, d_sfcv, B, F, D, H, W, alpha, nullptr, b, 1, 0, s,
+                                        nullptr, 0, 0, MR_CV_SSIM, 1, out_dtype);
             if (rc != MR_OK) return rc;
-            MR_CUDA(cudaMemcpyAsync(h_out_cv + b * vol1, d_cv + b * vol1, vol1 * 4, cudaMemcpyDeviceToHost, s));
-            for (int f = 0; f < F && h_out_sfcv != nullptr; ++f) {
-                size_t o = ((size_t)f * B + b) * vol1;
-                MR_CUDA(cudaMemcpyAsync(h_out_sfcv + o, d_sfcv + o, vol1 * 4, cudaMemcpyDeviceToHost, s));
+            const size_t vbytes = vol1 * vb;
+            MR_CUDA(cudaMemcpyAsync(o_cv + b * vbytes, d_cv + b * vbytes, vbytes, cudaMemcpyDeviceToHost, s));
+            for (int f = 0; f < F && o_sfcv != nullptr; ++f) {
+                size_t o = ((size_t)f * B + b) * vbytes;
+                MR_CUDA(cudaMemcpyAsync(o_sfcv + o, d_sfcv + o, vbytes, cudaMemcpyDeviceToHost, s));
             }
         }
         return MR_OK;
@@ -134,7 +153,30 @@ extern "C" int mr_cost_volume_host(const float* h_keyframe, const float* h_frame
     rc = enqueue();
     for (int i = 0; i < ring.n; ++i) {
         const cudaError_t e = cudaStreamSynchronize(ring.st[i]);
-        if (rc == MR_OK && e != cudaSuccess) rc = mr::check_cuda(e, "mr_cost_volume_host: cudaStreamSynchronize");
+        if (rc == MR_OK && e != cudaSuccess) rc = mr::check_cuda(e, out_dtype == MR_DT_F16 ? "mr_cost_volume_host_f16: cudaStreamSynchronize"
+                                                                                  : "mr_cost_volume_host: cudaStreamSynchronize");
     }
     return rc;
+}
+
+}  // namespace
+
+extern "C" int mr_cost_volume_host(const float* h_keyframe, const float* h_frames, const float* h_keyframe_pose,
+                                   const float* h_keyframe_K, const float* h_poses, const float* h_intrinsics,
+                                   float* h_out_cv, float* h_out_sfcv, int B, int F, int D, int H, int W,
+                                   float inv_depth_lo, float inv_depth_hi, float alpha, void* workspace,
+                                   long long workspace_bytes) {
+    return cost_volume_host("mr_cost_volume_host", h_keyframe, h_frames, h_keyframe_pose, h_keyframe_K, h_poses, h_intrinsics,
+                            h_out_cv, h_out_sfcv, B, F, D, H, W, inv_depth_lo, inv_depth_hi, alpha, workspace, workspace_bytes,
+                            MR_DT_F32);
+}
+
+extern "C" int mr_cost_volume_host_f16(const float* h_keyframe, const float* h_frames, const float* h_keyframe_pose,
+                                       const float* h_keyframe_K, const float* h_poses, const float* h_intrinsics,
+                                       void* h_out_cv, void* h_out_sfcv, int B, int F, int D, int H, int W,
+                                       float inv_depth_lo, float inv_depth_hi, float alpha, void* workspace,
+                                       long long workspace_bytes) {
+    return cost_volume_host("mr_cost_volume_host_f16", h_keyframe, h_frames, h_keyframe_pose, h_keyframe_K, h_poses,
+                            h_intrinsics, h_out_cv, h_out_sfcv, B, F, D, H, W, inv_depth_lo, inv_depth_hi, alpha, workspace,
+                            workspace_bytes, MR_DT_F16);
 }

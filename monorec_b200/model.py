@@ -319,6 +319,11 @@ class _TrunkFeatures(list):
         return (list, (list(list.__iter__(self)),))
 
 
+def _f32_or_f16(v):
+    """A cost volume as the layout kernels read it: half volumes (volume_dtype=torch.float16) are widened by the kernel."""
+    return v if v.dtype == torch.float16 else v.to(torch.float32)
+
+
 class MaskModule(_PackedSource, nn.Module):
     """Moving-object mask U-Net over the single-frame volumes (monorec_model.py:287-385)."""
 
@@ -378,7 +383,7 @@ class MaskModule(_PackedSource, nn.Module):
             # (standalone call, or a configuration the fused kernel does not write the engine layout for)
             x = torch.empty(nF * B, H, W, D, device=sfcvs[0].device, dtype=C.act_dtype())
             for f, v in enumerate(sfcvs):
-                C.nchw_to_nhwc(v.to(torch.float32), out=x[f * B:(f + 1) * B])
+                C.nchw_to_nhwc(_f32_or_f16(v), out=x[f * B:(f + 1) * B])
         if not self.use_cv:
             x.zero_()
         cv_feats = []
@@ -503,7 +508,7 @@ class DepthModule(_PackedSource, nn.Module):
         x = torch.empty(B, H, W, D + 3 + cpad, device=cv.device, dtype=C.act_dtype())
         if cpad:
             x[..., D + 3:].zero_()
-        C.nchw_to_nhwc(cv.to(torch.float32), out=x, out_coff=0, one_minus=data_dict.get("_cv_mask_for_depth"))
+        C.nchw_to_nhwc(_f32_or_f16(cv), out=x, out_coff=0, one_minus=data_dict.get("_cv_mask_for_depth"))
         C.nchw_to_nhwc(keyframe.to(torch.float32), out=x, out_coff=D)
         img = [C.as_nhwc(f, C.act_dtype()) for f in feats_nchw[:3]]
         feats = []
@@ -539,7 +544,7 @@ class MonoRecModel(nn.Module):
                  pretrain_dropout_mode=0, augmentation=None, use_mono=True, use_stereo=False, use_ssim=True,
                  sfcv_mult_mask=True, simple_mask=False, mask_use_cv=True, mask_use_feats=True, cv_patch_size=3,
                  depth_large_model=False, no_cv=False, freeze_resnet=True, freeze_module=(), checkpoint_location=None,
-                 mask_cp_loc=None, depth_cp_loc=None):
+                 mask_cp_loc=None, depth_cp_loc=None, volume_dtype=torch.float32):
         super().__init__()
         self.inv_depth_min_max = inv_depth_min_max
         self.cv_depth_steps = cv_depth_steps
@@ -564,7 +569,9 @@ class MonoRecModel(nn.Module):
             for p in self._feature_extractor.parameters(True):
                 p.requires_grad_(False)
         self.cv_module = CostVolumeModule(use_mono=use_mono, use_stereo=use_stereo, use_ssim=use_ssim,
-                                          sfcv_mult_mask=self.sfcv_mult_mask, patch_size=cv_patch_size)
+                                          sfcv_mult_mask=self.sfcv_mult_mask, patch_size=cv_patch_size,
+                                          volume_dtype=volume_dtype)
+        self.volume_dtype = volume_dtype
         if not (self.pretrain_mode == 1 or self.pretrain_mode == 3):
             self.att_module = MaskModule(self.cv_depth_steps, self._feature_extractor.num_ch_enc, use_cv=mask_use_cv,
                                          use_features=mask_use_feats)
@@ -651,7 +658,7 @@ class MonoRecModel(nn.Module):
             else:
                 s = list(keyframe.shape)
                 s[1] = self.cv_depth_steps
-                data_dict["cost_volume"] = keyframe.new_zeros(s)
+                data_dict["cost_volume"] = keyframe.new_zeros(s, dtype=self.volume_dtype)
                 data_dict["single_frame_cvs"] = [data_dict["cost_volume"].clone() for _ in data_dict["poses"]]
 
             # torchvision trunk on cuDNN, fed channels-last; TF32 is allowed there unless the engine runs its fp32 parity mode

@@ -8,10 +8,12 @@ call site of march_unit<MODE> or pixel_phase<T> when the inlining chains of its 
 line.  For each march mode it prints the largest such loop, the row loop (three row steps per body), and for the
 per-pixel phase its loops; counts are per row step for the march and per loop iteration otherwise.
 
-The kernel is instantiated as cost_volume_kernel<PIX, ERR, CENTER>: depth source (plane table / per-pixel cv_depths), error
-mode (1 SSIM, 2 SSIM + L1, 3 box L1: MR_CV_*) and centred or uncentred fused volume.  The two default instantiations (SSIM,
-centred) are reported first, plane depths then per-pixel depths, and the other ten after them.  A source from before the
-error mode was a template parameter has only cost_volume_kernel<PIX>; it is reported under the same two titles.
+The kernel is instantiated as cost_volume_kernel<PIX, ERR, CENTER, OUT>: depth source (plane table / per-pixel cv_depths),
+error mode (1 SSIM, 2 SSIM + L1, 3 box L1: MR_CV_*), centred or uncentred fused volume, and the volumes' storage type (float
+or __half).  The twelve fp32 instantiations come first (the two default ones, SSIM centred, plane depths then per-pixel
+depths, lead), the twelve half ones after them in the same order.  A source from before the volume type was a template
+parameter is reported under the fp32 titles; one from before the error mode was has only cost_volume_kernel<PIX>, reported
+under the first two titles.
 """
 import collections
 import re
@@ -53,17 +55,22 @@ def disassemble(src):
 
 
 ERR_NAMES = {1: "SSIM", 2: "SSIM + L1", 3: "box L1"}
-# (label, mangled template arguments of cost_volume_kernel<PIX, ERR, CENTER>, those of a source with only <PIX>)
+OUT_TYPES = (("f", "float", "fp32"), ("6__half", "__half", "half"))
+# (label, mangled template arguments of cost_volume_kernel<PIX, ERR, CENTER, OUT>, those of a source from before the volume
+# type was a template parameter (fp32 only), those of a source with only <PIX>)
 INSTANTIATIONS = [
-    (f"{'per-pixel' if pix else 'plane'} depths, {ERR_NAMES[err]}, {'centred' if ctr else 'uncentred'} "
-     f"(cost_volume_kernel<{'true' if pix else 'false'}, {err}, {'true' if ctr else 'false'}>)",
-     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}EE", f"cost_volume_kernelILb{pix}EE" if err == 1 and ctr else None)
+    (f"{'per-pixel' if pix else 'plane'} depths, {ERR_NAMES[err]}, {'centred' if ctr else 'uncentred'}, {oname} volumes "
+     f"(cost_volume_kernel<{'true' if pix else 'false'}, {err}, {'true' if ctr else 'false'}, {otype}>)",
+     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}E{omangled}EE",
+     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}EE" if omangled == "f" else None,
+     f"cost_volume_kernelILb{pix}EE" if err == 1 and ctr and omangled == "f" else None)
+    for omangled, otype, oname in OUT_TYPES
     for err, ctr, pix in [(1, 1, 0), (1, 1, 1)] + [(e, c, p) for e in (1, 2, 3) for c in (1, 0) for p in (0, 1)
                                                     if (e, c) != (1, 1)]
 ]
 
 
-def kernel_instructions(dis, name="cost_volume_kernelILb0ELi1ELb1EE"):
+def kernel_instructions(dis, name="cost_volume_kernelILb0ELi1ELb1EfEE"):
     """[(addr, opcode, text, source lines of the inlining chain)] and {label: addr} of the kernel whose .text section
     name contains `name` (default: the plane instantiation)."""
     ins, labels, cur, inside, pending = [], {}, [], False, []
@@ -101,9 +108,11 @@ def main():
         if m and "__device__" not in l and "void" not in l:
             sites[f"{m.group(1)}<{m.group(2)}>"] = i
     dis = disassemble(src)
-    for k, (title, name, old) in enumerate(INSTANTIATIONS):
+    for k, (title, name, old3, old) in enumerate(INSTANTIATIONS):
         if name not in dis:
-            if old is not None and old in dis:       # (a source from before the error mode became a template parameter)
+            if old3 is not None and old3 in dis:     # (a source from before the volume type became a template parameter)
+                name = old3
+            elif old is not None and old in dis:     # (a source from before the error mode became a template parameter)
                 name = old
             elif k == 0 and "cost_volume_kernelILb" not in dis:   # (from before the depth source became one)
                 report(src, "cost_volume_kernel", *kernel_instructions(dis, "cost_volume_kernel"), sites)
