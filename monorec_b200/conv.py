@@ -238,7 +238,14 @@ def pool_and_frame_max(x, frames):
 
 
 def mask_volume(volume, mask):
-    """cost_volume * (1 - cv_mask) on NCHW tensors (model/monorec/monorec_model.py:713); a half volume gives a half result."""
+    """cost_volume * (1 - cv_mask) on NCHW tensors (model/monorec/monorec_model.py:713); a half volume gives a half result.
+    Under torch.compile: the `monorec_b200::mask_volume` op, whose implementation is mask_volume_impl."""
+    if torch.compiler.is_compiling():
+        return torch.ops.monorec_b200.mask_volume(volume, mask)
+    return mask_volume_impl(volume, mask)
+
+
+def mask_volume_impl(volume: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
     lib = _lib.load()
     volume = volume.contiguous()
     mask = mask.to(torch.float32).contiguous()
@@ -470,3 +477,6 @@ def upconv_layer(conv, src_c):
             _lib.check(lib.mr_subpixel_upconv2(w.data_ptr(), cout, cin, py, px, sub.data_ptr(), None, None), "mr_subpixel_upconv2")
             subs.append(PackedConv(sub.to(conv.weight.device), conv.bias, src_c, pad=(0, 0), out_step=(2, 2), out_off=(py, px)))
     return PackedSubpixel(subs)
+
+
+from . import ops  # noqa: E402,F401  (registers monorec_b200::mask_volume, which mask_volume calls under torch.compile)

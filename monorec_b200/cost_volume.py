@@ -4,9 +4,10 @@ Same constructor arguments, same data_dict keys in and out; the arithmetic runs 
 libmonorec_b200.so (csrc/cost_volume.cu) through the C ABI.  No torch fallback.
 """
 import time
+from typing import List, Optional, Tuple
 
 import torch
-from torch import nn
+from torch import Tensor, nn
 
 from . import _lib
 
@@ -40,6 +41,72 @@ def _as_f32c(t):
     if t.dtype != torch.float32 or not t.is_contiguous():
         t = t.to(torch.float32).contiguous()
     return t
+
+
+def fills_nhwc(nhwc, F, B, D, H, W):
+    """Whether the kernel writes the MaskModule's NHWC input [F*B,H,W,D] (fp32 or half) beside the volumes."""
+    return nhwc is not None and D <= 32 and D % 8 == 0 and tuple(nhwc.shape) == (F * B, H, W, D) \
+        and nhwc.is_contiguous() and nhwc.dtype in (torch.float32, torch.float16)
+
+
+def launch(keyframe: Tensor, frames: List[Tensor], intrinsics: List[Tensor], poses: List[Tensor], keyframe_pose: Tensor,
+           keyframe_intrinsics: Tensor, cv_depths: Optional[Tensor], sfcv_nhwc: Optional[Tensor], lo: float, hi: float,
+           steps: int, alpha: float, channel_weights: List[float], matching: int, center: bool,
+           half: bool) -> Tuple[Tensor, Tensor]:
+    """Projection tables and the fused cost-volume kernel on contiguous fp32 CUDA inputs -> (cost_volume [B,D,H,W],
+    single-frame volumes [F,B,D,H,W]), half when `half`.  D is cv_depths.shape[1] with per-pixel hypotheses, else `steps`
+    planes uniform in inverse depth over [lo, hi].  `sfcv_nhwc`, when given, must satisfy `fills_nhwc` and is filled with
+    the single-frame volumes in the MaskModule's layout.  CostVolumeModule.forward calls this directly; under torch.compile
+    it is the implementation of the `monorec_b200::cost_volume` op (monorec_b200/ops.py)."""
+    lib = _lib.load()
+    B, _, H, W = keyframe.shape
+    F = len(frames)
+    D = steps if cv_depths is None else cv_depths.shape[1]
+    vdt = torch.float16 if half else torch.float32
+    nhwc = sfcv_nhwc
+    nhwc_half = 1 if nhwc is not None and nhwc.dtype == torch.float16 else 0
+    centre = 1 if center else 0
+    dev = keyframe.device
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    with torch.cuda.device(dev):
+        proj = torch.empty(B, F, 3, 4, device=dev, dtype=torch.float32)
+        depths = torch.empty(D, device=dev, dtype=torch.float32) if cv_depths is None else None
+        cv = torch.empty(B, D, H, W, device=dev, dtype=vdt)
+        sfcv = torch.empty(F, B, D, H, W, device=dev, dtype=vdt)
+        _lib.check(lib.mr_projection_tables(keyframe_pose.data_ptr(), keyframe_intrinsics.data_ptr(), _lib.ptr_array(poses),
+                                            _lib.ptr_array(intrinsics), B, F, H, W, proj.data_ptr(),
+                                            None if depths is None else depths.data_ptr(), D, lo, hi, stream),
+                   "mr_projection_tables")
+        cw = (_lib.c_float * 3)(*channel_weights)
+        if half:
+            # half volumes: one entry for every error mode, centring and depth source
+            _lib.check(lib.mr_cost_volume_fwd_typed(
+                keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
+                None if depths is None else depths.data_ptr(), None if cv_depths is None else cv_depths.data_ptr(),
+                cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if nhwc is not None else None, nhwc_half,
+                B, F, D, H, W, alpha, cw, matching, centre, 1, stream), "mr_cost_volume_fwd_typed")
+        elif matching != CV_SSIM or not center:
+            # the reference's non-default error modes and the uncentred volume, on either depth source
+            _lib.check(lib.mr_cost_volume_fwd_matching(
+                keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
+                None if depths is None else depths.data_ptr(), None if cv_depths is None else cv_depths.data_ptr(),
+                cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if nhwc is not None else None, nhwc_half,
+                B, F, D, H, W, alpha, cw, matching, centre, stream), "mr_cost_volume_fwd_matching")
+        elif cv_depths is not None:
+            # (one entry: it chooses TMA windows or the gather itself, like mr_cost_volume_fwd)
+            _lib.check(lib.mr_cost_volume_fwd_depthmap(
+                keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), cv_depths.data_ptr(), cv.data_ptr(),
+                sfcv.data_ptr(), nhwc.data_ptr() if nhwc is not None else None, nhwc_half, B, F, D, H, W, alpha, cw,
+                stream), "mr_cost_volume_fwd_depthmap")
+        elif nhwc is not None:
+            _lib.check(lib.mr_cost_volume_fwd_nhwc(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
+                                                   depths.data_ptr(), cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr(),
+                                                   nhwc_half, B, F, D, H, W, alpha, cw, stream), "mr_cost_volume_fwd_nhwc")
+        else:
+            _lib.check(lib.mr_cost_volume_fwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), depths.data_ptr(),
+                                              cv.data_ptr(), sfcv.data_ptr(), B, F, D, H, W, alpha, cw, stream),
+                       "mr_cost_volume_fwd")
+    return cv, sfcv
 
 
 class CostVolumeModule(nn.Module):
@@ -94,14 +161,16 @@ class CostVolumeModule(nn.Module):
         inverse-depth planes, and its D is the one of the view weight.  It is read as contiguous fp32: other dtypes and
         expanded or strided views (such as a broadcast of per-plane depths) are materialised first.
         """
-        start_time = time.time()
+        compiling = torch.compiler.is_compiling()
+        start_time = None if compiling else time.time()
         keyframe = _as_f32c(data_dict["keyframe"])
         if not keyframe.is_cuda:
             raise _lib.MonorecLibraryError("monorec_b200.CostVolumeModule needs CUDA tensors (no CPU fallback)")
         pixel_depths = None
         if "cv_depths" in data_dict:
             pixel_depths = self._check_cv_depths(data_dict["cv_depths"], keyframe)
-        lib = _lib.load()
+        if not compiling:
+            _lib.load()
         frames, intrinsics, poses = self._gather(data_dict)
         frames = [_as_f32c(f) for f in frames]
         intrinsics = [_as_f32c(k) for k in intrinsics]
@@ -117,69 +186,22 @@ class CostVolumeModule(nn.Module):
         else:
             # .item()-free: the ranges are python floats on the model, mirrored into the dict as 1-element tensors
             lo, hi, D = self._plane_range(data_dict)
-        dev = keyframe.device
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            proj = torch.empty(B, F, 3, 4, device=dev, dtype=torch.float32)
-            depths = torch.empty(D, device=dev, dtype=torch.float32) if pixel_depths is None else None
-            cv = torch.empty(B, D, H, W, device=dev, dtype=self.volume_dtype)
-            sfcv = torch.empty(F, B, D, H, W, device=dev, dtype=self.volume_dtype)
-            _lib.check(lib.mr_projection_tables(kpose.data_ptr(), kK.data_ptr(), _lib.ptr_array(poses),
-                                                _lib.ptr_array(intrinsics), B, F, H, W, proj.data_ptr(),
-                                                None if depths is None else depths.data_ptr(), D, lo, hi, stream),
-                       "mr_projection_tables")
-            cw = None
-            if self.channel_weights is not None:
-                cw = (_lib.c_float * 3)(*self.channel_weights)
-            else:
-                cw = (_lib.c_float * 3)(1 / 3, 1 / 3, 1 / 3)  # monorec_model.py:174-177
-            nhwc = data_dict.get("_sfcv_nhwc")   # MonoRecModel: the MaskModule's input buffer [F*B,H,W,D], filled by the kernel
-            fill_nhwc = nhwc is not None and D <= 32 and D % 8 == 0 \
-                and tuple(nhwc.shape) == (F * B, H, W, D) and nhwc.is_contiguous() \
-                and nhwc.dtype in (torch.float32, torch.float16)
-            if self.volume_dtype == torch.float16:
-                # half volumes: one entry for every error mode, centring and depth source
-                _lib.check(lib.mr_cost_volume_fwd_typed(
-                    keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
-                    None if depths is None else depths.data_ptr(), None if pixel_depths is None else pixel_depths.data_ptr(),
-                    cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if fill_nhwc else None,
-                    1 if fill_nhwc and nhwc.dtype == torch.float16 else 0, B, F, D, H, W, float(self.alpha), cw,
-                    self.matching, 0 if self.not_center_cv else 1, 1, stream), "mr_cost_volume_fwd_typed")
-                if fill_nhwc:
-                    data_dict["_sfcv_nhwc_filled"] = True
-            elif self.matching != CV_SSIM or self.not_center_cv:
-                # the reference's non-default error modes and the uncentred volume, on either depth source
-                _lib.check(lib.mr_cost_volume_fwd_matching(
-                    keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
-                    None if depths is None else depths.data_ptr(), None if pixel_depths is None else pixel_depths.data_ptr(),
-                    cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if fill_nhwc else None,
-                    1 if fill_nhwc and nhwc.dtype == torch.float16 else 0, B, F, D, H, W, float(self.alpha), cw,
-                    self.matching, 0 if self.not_center_cv else 1, stream), "mr_cost_volume_fwd_matching")
-                if fill_nhwc:
-                    data_dict["_sfcv_nhwc_filled"] = True
-            elif pixel_depths is not None:
-                # (one entry: it chooses TMA windows or the gather itself, like mr_cost_volume_fwd)
-                _lib.check(lib.mr_cost_volume_fwd_depthmap(
-                    keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), pixel_depths.data_ptr(), cv.data_ptr(),
-                    sfcv.data_ptr(), nhwc.data_ptr() if fill_nhwc else None,
-                    1 if fill_nhwc and nhwc.dtype == torch.float16 else 0, B, F, D, H, W, float(self.alpha), cw, stream),
-                    "mr_cost_volume_fwd_depthmap")
-                if fill_nhwc:
-                    data_dict["_sfcv_nhwc_filled"] = True
-            elif fill_nhwc:
-                _lib.check(lib.mr_cost_volume_fwd_nhwc(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
-                                                       depths.data_ptr(), cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr(),
-                                                       1 if nhwc.dtype == torch.float16 else 0, B, F, D, H, W,
-                                                       float(self.alpha), cw, stream), "mr_cost_volume_fwd_nhwc")
-                data_dict["_sfcv_nhwc_filled"] = True
-            else:
-                _lib.check(lib.mr_cost_volume_fwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), depths.data_ptr(),
-                                                  cv.data_ptr(), sfcv.data_ptr(), B, F, D, H, W, float(self.alpha), cw, stream),
-                           "mr_cost_volume_fwd")
+        # monorec_model.py:174-177 without channel weights
+        cw = list(self.channel_weights) if self.channel_weights is not None else [1 / 3, 1 / 3, 1 / 3]
+        nhwc = data_dict.get("_sfcv_nhwc")   # MonoRecModel: the MaskModule's input buffer [F*B,H,W,D], filled by the kernel
+        fill_nhwc = fills_nhwc(nhwc, F, B, D, H, W)
+        run = torch.ops.monorec_b200.cost_volume if compiling else launch
+        cv, sfcv = run(keyframe, frames, intrinsics, poses, kpose, kK, pixel_depths, nhwc if fill_nhwc else None,
+                       float(lo), float(hi), int(D), float(self.alpha), cw, int(self.matching), not self.not_center_cv,
+                       self.volume_dtype == torch.float16)
+        if fill_nhwc:
+            data_dict["_sfcv_nhwc_filled"] = True
         data_dict["cost_volume"] = cv
         data_dict["single_frame_cvs"] = [sfcv[f] for f in range(F)]
-        # host-side issue time (the reference's number includes its device work only because it synchronises implicitly)
-        data_dict["cv_module_time"] = torch.full((1,), time.time() - start_time, device=dev, dtype=torch.float32)
+        # host-side issue time (the reference's number includes its device work only because it synchronises implicitly);
+        # 0 in a torch.compile / torch.export graph, where no host clock is read
+        elapsed = 0.0 if compiling else time.time() - start_time
+        data_dict["cv_module_time"] = torch.full((1,), elapsed, device=keyframe.device, dtype=torch.float32)
         return data_dict
 
     @staticmethod
@@ -215,3 +237,6 @@ class CostVolumeModule(nn.Module):
         mask = torch.zeros(c, 1, height, width, device=device)
         mask[:, :, border_radius:height - border_radius, border_radius:width - border_radius] = 1
         return mask
+
+
+from . import ops  # noqa: E402,F401  (registers monorec_b200::cost_volume, which forward calls under torch.compile)

@@ -8,7 +8,10 @@ own losses pass (model/loss_functions/monorec_loss.py:185-188, :264-265, :355, :
 differentiable w.r.t. `depth_prediction` through a torch.autograd.Function whose backward is one kernel; nothing but the
 [B,H,W] index of the winning frame is kept between the passes (the reference keeps ~25 full-size temporaries per frame).
 """
+from typing import List
+
 import torch
+from torch import Tensor
 
 from . import _lib
 
@@ -29,19 +32,53 @@ def _collect(data_dict, use_mono, use_stereo):
     return frames, poses, intrinsics
 
 
+def projection(keyframe: Tensor, keyframe_pose: Tensor, keyframe_intrinsics: Tensor, poses: List[Tensor],
+               intrinsics: List[Tensor]) -> Tensor:
+    """[B,F,12] keyframe-to-frame projection tables (mr_projection_tables) from contiguous fp32 CUDA tensors."""
+    lib = _lib.load()
+    B, _, H, W = keyframe.shape
+    dev = keyframe.device
+    proj = torch.empty(B, len(poses), 12, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        _lib.check(lib.mr_projection_tables(keyframe_pose.data_ptr(), keyframe_intrinsics.data_ptr(), _lib.ptr_array(poses),
+                                            _lib.ptr_array(intrinsics), B, len(poses), H, W, proj.data_ptr(), None, 0, 0.0,
+                                            0.0, torch.cuda.current_stream(dev).cuda_stream), "mr_projection_tables")
+    return proj
+
+
+def errors_fwd(keyframe, frames, proj, invd, automasking, border):
+    """mr_reprojection_loss_fwd on fp32 contiguous inputs (invd: [B,1,H,W] inverse depth) -> (errors, winner) [B,H,W]."""
+    lib = _lib.load()
+    B, _, H, W = keyframe.shape
+    errors = torch.empty(B, H, W, device=keyframe.device, dtype=torch.float32)
+    winner = torch.empty(B, H, W, device=keyframe.device, dtype=torch.int32)
+    with torch.cuda.device(keyframe.device):
+        _lib.check(lib.mr_reprojection_loss_fwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), invd.data_ptr(),
+                                                B, len(frames), H, W, 1 if automasking else 0, int(border), errors.data_ptr(),
+                                                winner.data_ptr(), torch.cuda.current_stream(keyframe.device).cuda_stream),
+                   "mr_reprojection_loss_fwd")
+    return errors, winner
+
+
+def errors_bwd(keyframe, frames, proj, invd, grad_errors, winner):
+    """mr_reprojection_loss_bwd -> the gradient [B,1,H,W] fp32 w.r.t. the inverse depth."""
+    lib = _lib.load()
+    B, _, H, W = keyframe.shape
+    g = grad_errors.to(torch.float32).contiguous()
+    out = torch.empty(B, 1, H, W, device=keyframe.device, dtype=torch.float32)
+    with torch.cuda.device(keyframe.device):
+        _lib.check(lib.mr_reprojection_loss_bwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), invd.data_ptr(),
+                                                g.data_ptr(), winner.data_ptr(), B, len(frames), H, W, out.data_ptr(),
+                                                torch.cuda.current_stream(keyframe.device).cuda_stream),
+                   "mr_reprojection_loss_bwd")
+    return out
+
+
 class _ReprojectionErrors(torch.autograd.Function):
     @staticmethod
     def forward(ctx, depth_prediction, keyframe, proj, automasking, border, *frames):
-        lib = _lib.load()
-        B, _, H, W = keyframe.shape
         invd = depth_prediction.detach().to(torch.float32).contiguous()
-        errors = torch.empty(B, H, W, device=keyframe.device, dtype=torch.float32)
-        winner = torch.empty(B, H, W, device=keyframe.device, dtype=torch.int32)
-        with torch.cuda.device(keyframe.device):
-            _lib.check(lib.mr_reprojection_loss_fwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), invd.data_ptr(),
-                                                    B, len(frames), H, W, 1 if automasking else 0, int(border), errors.data_ptr(),
-                                                    winner.data_ptr(), torch.cuda.current_stream(keyframe.device).cuda_stream),
-                       "mr_reprojection_loss_fwd")
+        errors, winner = errors_fwd(keyframe, frames, proj, invd, automasking, border)
         ctx.save_for_backward(invd, keyframe, proj, winner, *frames)
         ctx.mark_non_differentiable(winner)
         ctx.in_dtype = depth_prediction.dtype
@@ -50,15 +87,7 @@ class _ReprojectionErrors(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_errors, _grad_winner):
         invd, keyframe, proj, winner, *frames = ctx.saved_tensors
-        lib = _lib.load()
-        B, _, H, W = keyframe.shape
-        g = grad_errors.to(torch.float32).contiguous()
-        out = torch.empty(B, 1, H, W, device=keyframe.device, dtype=torch.float32)
-        with torch.cuda.device(keyframe.device):
-            _lib.check(lib.mr_reprojection_loss_bwd(keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(), invd.data_ptr(),
-                                                    g.data_ptr(), winner.data_ptr(), B, len(frames), H, W, out.data_ptr(),
-                                                    torch.cuda.current_stream(keyframe.device).cuda_stream),
-                       "mr_reprojection_loss_bwd")
+        out = errors_bwd(keyframe, frames, proj, invd, grad_errors, winner)
         return (out.to(ctx.in_dtype), None, None, None, None) + (None,) * len(frames)
 
 
@@ -70,7 +99,6 @@ def reprojection_errors(depth_prediction, data_dict, automasking=False, use_mono
     frames, poses, intrinsics = _collect(data_dict, use_mono, use_stereo)
     if not frames:
         raise ValueError("reprojection_loss: no source frames (use_mono / use_stereo)")
-    lib = _lib.load()
     B, C, H, W = keyframe.shape
     if C != 3 or tuple(depth_prediction.shape) != (B, 1, H, W):
         raise ValueError(f"reprojection_loss: keyframe {tuple(keyframe.shape)} / depth_prediction {tuple(depth_prediction.shape)}")
@@ -82,11 +110,12 @@ def reprojection_errors(depth_prediction, data_dict, automasking=False, use_mono
     frames = [f32(t) for t in frames]
     kf_pose, kf_K = f32(data_dict["keyframe_pose"]), f32(data_dict["keyframe_intrinsics"])
     poses, intrinsics = [f32(t) for t in poses], [f32(t) for t in intrinsics]
-    proj = torch.empty(B, len(frames), 12, device=dev, dtype=torch.float32)
-    with torch.cuda.device(dev):
-        _lib.check(lib.mr_projection_tables(kf_pose.data_ptr(), kf_K.data_ptr(), _lib.ptr_array(poses), _lib.ptr_array(intrinsics),
-                                            B, len(frames), H, W, proj.data_ptr(), None, 0, 0.0, 0.0,
-                                            torch.cuda.current_stream(dev).cuda_stream), "mr_projection_tables")
+    if torch.compiler.is_compiling():
+        # one op for the tables and the forward pass; its autograd formula runs the backward op (monorec_b200/ops.py)
+        errors, winner, _ = torch.ops.monorec_b200.reprojection_loss_fwd(depth_prediction, keyframe, frames, kf_pose, kf_K,
+                                                                         poses, intrinsics, bool(automasking), int(border))
+        return errors, winner
+    proj = projection(keyframe, kf_pose, kf_K, poses, intrinsics)
     return _ReprojectionErrors.apply(depth_prediction, keyframe, proj, bool(automasking), int(border), *frames)
 
 
@@ -110,3 +139,6 @@ def reprojection_loss(depth_prediction, data_dict, automasking=False, error_func
     if reduce:                                                                  # :110-111
         return wts[0] * mask_mean(errors, torch.isinf(errors))
     return wts[0] * errors                                                      # :112-113
+
+
+from . import ops  # noqa: E402,F401  (registers the loss ops, which reprojection_errors calls under torch.compile)

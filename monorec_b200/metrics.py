@@ -10,8 +10,10 @@ module unchanged.  No CPU fallback.
 """
 import ctypes
 import weakref
+from typing import List, Optional
 
 import torch
+from torch import Tensor
 
 from . import _lib
 
@@ -23,28 +25,40 @@ def sparse_metrics(data_dict, roi=None, max_distance=None, pred_all_valid=True, 
     pred, gt = data_dict["result"], data_dict["target"]
     if not pred.is_cuda:
         raise _lib.MonorecLibraryError("monorec_b200.metrics needs CUDA tensors (no CPU fallback)")
+    mv = data_dict["mvobj_mask"] if use_cvmask else None
+    roi_l = None if roi is None else [int(v) for v in roi]
+    max_d = float(max_distance) if max_distance else 0.0
+    if torch.compiler.is_compiling():
+        return torch.ops.monorec_b200.sparse_metrics(pred, gt, mv, roi_l, max_d, bool(pred_all_valid))
     key = (id(pred), pred._version, id(gt), gt._version, None if roi is None else tuple(int(v) for v in roi),
            None if max_distance is None else float(max_distance), bool(pred_all_valid), bool(use_cvmask))
     cache = data_dict.get("_mr_metrics_cache")
     if cache is not None and cache[0] == key:
         return cache[1]
+    out = sparse_metrics_impl(pred, gt, mv, roi_l, max_d, bool(pred_all_valid))
+    data_dict["_mr_metrics_cache"] = (key, out)
+    return out
+
+
+def sparse_metrics_impl(pred: Tensor, gt: Tensor, mvobj_mask: Optional[Tensor], roi: Optional[List[int]],
+                        max_distance: float, pred_all_valid: bool) -> Tensor:
+    """The fused sparse pass (mr_sparse_metrics) -> [7]; max_distance 0 = none.  sparse_metrics calls this directly; under
+    torch.compile it is the implementation of the `monorec_b200::sparse_metrics` op."""
     lib = _lib.load()
     pred = pred.to(torch.float32).contiguous()
     gt = gt.to(device=pred.device, dtype=torch.float32).contiguous()
     B, _, H, W = pred.shape
     mv = None
-    if use_cvmask:
-        mv = data_dict["mvobj_mask"].to(device=pred.device, dtype=torch.float32).contiguous()
+    if mvobj_mask is not None:
+        mv = mvobj_mask.to(device=pred.device, dtype=torch.float32).contiguous()
     out = torch.empty(7, device=pred.device, dtype=torch.float32)
     ws_bytes = lib.mr_sparse_metrics_workspace(B)
     ws = torch.empty(ws_bytes // 8, device=pred.device, dtype=torch.float64)
-    roi_c = None if roi is None else (ctypes.c_int * 4)(*[int(v) for v in roi])
+    roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
     with torch.cuda.device(pred.device):
         _lib.check(lib.mr_sparse_metrics(pred.data_ptr(), gt.data_ptr(), None if mv is None else mv.data_ptr(), B, H, W, roi_c,
-                                         float(max_distance) if max_distance else 0.0, 1 if pred_all_valid else 0,
-                                         out.data_ptr(), ws.data_ptr(), ws_bytes,
+                                         max_distance, 1 if pred_all_valid else 0, out.data_ptr(), ws.data_ptr(), ws_bytes,
                                          torch.cuda.current_stream(pred.device).cuda_stream), "mr_sparse_metrics")
-    data_dict["_mr_metrics_cache"] = (key, out)
     return out
 
 
@@ -83,13 +97,24 @@ def dense_metrics(depth_prediction, depth_gt, roi=None, max_distance=None):
     reference-named functions below cost one launch group per call set."""
     pred, gt = depth_prediction, depth_gt
     _check_pair(pred, gt, "monorec_b200.metrics.dense_metrics")
+    roi_l = None if roi is None else [int(v) for v in roi]
+    # get_absolute_depth (utils/util.py:46-56) clamps at the fp32 rounding of 1 / max_distance (a ZeroDivisionError for 0)
+    min_inv = 0.0 if max_distance is None else 1 / max_distance
+    if torch.compiler.is_compiling():
+        return torch.ops.monorec_b200.dense_metrics(pred, gt, roi_l, float(min_inv))
     key = (pred._version, gt._version, None if roi is None else tuple(int(v) for v in roi),
            None if max_distance is None else float(max_distance))
     hit = _dense_last[0]
     if hit is not None and hit[0]() is pred and hit[1]() is gt and hit[2] == key:
         return hit[3]
-    # get_absolute_depth (utils/util.py:46-56) clamps at the fp32 rounding of 1 / max_distance (a ZeroDivisionError for 0)
-    min_inv = 0.0 if max_distance is None else 1 / max_distance
+    out = dense_metrics_impl(pred, gt, roi_l, float(min_inv))
+    _dense_last[0] = (weakref.ref(pred), weakref.ref(gt), key, out)
+    return out
+
+
+def dense_metrics_impl(pred: Tensor, gt: Tensor, roi: Optional[List[int]], min_inv: float) -> Tensor:
+    """The fused dense pass (mr_dense_metrics) -> [12].  dense_metrics calls this directly; under torch.compile it is the
+    implementation of the `monorec_b200::dense_metrics` op."""
     lib = _lib.load()
     p = pred.to(torch.float32).contiguous()
     g = gt.to(device=p.device, dtype=torch.float32).contiguous()
@@ -97,11 +122,10 @@ def dense_metrics(depth_prediction, depth_gt, roi=None, max_distance=None):
     out = torch.empty(len(DENSE_NAMES), device=p.device, dtype=torch.float32)
     ws_bytes = lib.mr_dense_metrics_workspace(B)
     ws = torch.empty(ws_bytes // 8, device=p.device, dtype=torch.float64)
-    roi_c = None if roi is None else (ctypes.c_int * 4)(*[int(v) for v in roi])
+    roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
     with torch.cuda.device(p.device):
-        _lib.check(lib.mr_dense_metrics(p.data_ptr(), g.data_ptr(), B, H, W, roi_c, float(min_inv), out.data_ptr(), ws.data_ptr(),
+        _lib.check(lib.mr_dense_metrics(p.data_ptr(), g.data_ptr(), B, H, W, roi_c, min_inv, out.data_ptr(), ws.data_ptr(),
                                         ws_bytes, torch.cuda.current_stream(p.device).cuda_stream), "mr_dense_metrics")
-    _dense_last[0] = (weakref.ref(pred), weakref.ref(gt), key, out)
     return out
 
 
@@ -145,6 +169,17 @@ def median_scaling(data_dict):
     _check_pair(pred, gt, "monorec_b200.metrics.median_scaling")
     if pred.dtype != torch.float32:
         raise ValueError(f"median_scaling: result must be float32, got {pred.dtype}")
+    run = torch.ops.monorec_b200.median_scaling if torch.compiler.is_compiling() else median_scaling_impl
+    scaled = dict(data_dict)
+    scaled["result"] = run(pred, gt)
+    # the sparse pass cached for the unscaled result is keyed on its id, which a later tensor may reuse once it is freed
+    scaled.pop("_mr_metrics_cache", None)
+    return scaled
+
+
+def median_scaling_impl(pred: Tensor, gt: Tensor) -> Tensor:
+    """mr_median_scaling: the scaled prediction.  median_scaling calls this directly; under torch.compile it is the
+    implementation of the `monorec_b200::median_scaling` op."""
     lib = _lib.load()
     p = pred.contiguous()
     g = gt.to(device=p.device, dtype=torch.float32).contiguous()
@@ -155,11 +190,7 @@ def median_scaling(data_dict):
     with torch.cuda.device(p.device):
         _lib.check(lib.mr_median_scaling(p.data_ptr(), g.data_ptr(), out.data_ptr(), B, H, W, ws.data_ptr(), ws_bytes,
                                          torch.cuda.current_stream(p.device).cuda_stream), "mr_median_scaling")
-    scaled = dict(data_dict)
-    scaled["result"] = out
-    # the sparse pass cached for the unscaled result is keyed on its id, which a later tensor may reuse once it is freed
-    scaled.pop("_mr_metrics_cache", None)
-    return scaled
+    return out
 
 
 def images_u8_to_f32(images_u8, crop_box=None):
@@ -177,3 +208,6 @@ def images_u8_to_f32(images_u8, crop_box=None):
         _lib.check(lib.mr_images_u8_to_f32(x.data_ptr(), out.data_ptr(), B, Hs, Ws, top, left, H, W,
                                            torch.cuda.current_stream(x.device).cuda_stream), "mr_images_u8_to_f32")
     return out
+
+
+from . import ops  # noqa: E402,F401  (registers the metric ops, which the functions above call under torch.compile)

@@ -16,6 +16,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import conv as C
+from . import ops
 from .cost_volume import CostVolumeModule
 
 __all__ = ["MonoRecModel", "CostVolumeModule", "MaskModule", "DepthModule", "ResnetEncoder"]
@@ -100,6 +101,30 @@ class _Packed:
             return entry[1]
 
 
+class _PackedShared(_Packed):
+    """The cache of a module that packs weights it is handed (ops.py: the weights of any model of one configuration).  One
+    entry per (device, signature), the last `keep` kept.  An entry holds its source tensors, so their memory cannot be
+    freed and reused by other tensors that would then match the signature's data pointers and versions."""
+
+    def __init__(self, keep=4):
+        super().__init__()
+        self.keep = keep
+
+    def get(self, sig, device, builder, sources=()):
+        key = (str(device), sig)
+        with _PACK_LOCK:
+            entry = self.entries.pop(key, None)
+            if entry is None:
+                with torch.no_grad():
+                    entry = (builder(), list(sources))
+                if device.type == "cuda":
+                    torch.cuda.current_stream(device).synchronize()
+            self.entries[key] = entry                  # most recent last
+            while len(self.entries) > self.keep:
+                self.entries.pop(next(iter(self.entries)))
+            return entry[0]
+
+
 class _PackedSource:
     """Where a module's kernel-layout copies come from.  The signature is that of the module's own parameters -- except in a
     DataParallel replica, which has no registered parameters (its copies on its device are plain attributes, broadcast anew
@@ -120,7 +145,14 @@ class _PackedSource:
 
     def _packs(self, builder):
         """The entry of the device this module's weights are on, built by `builder` (from those weights) if missing."""
+        if isinstance(self._packed, _PackedShared):
+            src = self._source_tensors()
+            return self._packed.get(_source_sig(src), self._pack_device(), builder, src)
         return self._packed.get(self._pack_sig(), self._pack_device(), builder)
+
+    def _source_names(self):
+        """Names (relative to this module) of `_source_tensors()`, in that order."""
+        return [n for n, _ in self.named_parameters()]
 
 
 def _leaky(conv, src_c, stride=(1, 1)):
@@ -172,6 +204,10 @@ class ResnetEncoder(_PackedSource, nn.Module):
     def _source_tensors(self):
         e = self.encoder
         return [t for n, t in list(e.named_parameters()) + list(e.named_buffers()) if not n.startswith("fc.")]
+
+    def _source_names(self):
+        e = self.encoder
+        return ["encoder." + n for n, _ in list(e.named_parameters()) + list(e.named_buffers()) if not n.startswith("fc.")]
 
     def _pack_device(self):
         return self.encoder.conv1.weight.device
@@ -257,6 +293,15 @@ class ResnetEncoder(_PackedSource, nn.Module):
         self.features.append(e.layer3(self.features[-1]))
         self.features.append(e.layer4(self.features[-1]))
         return self.features
+
+
+def trunk_features(encoder, image, allow_tf32):
+    """The trunk's levels of `image` with cuDNN's TF32 switch set as given (only TF32 is decided here: the caller's cuDNN
+    benchmark / deterministic settings are passed through).  MonoRecModel.forward calls this directly; under torch.compile
+    it is the implementation of the `monorec_b200::resnet_trunk` op, which returns all five levels."""
+    with torch.backends.cudnn.flags(enabled=True, benchmark=torch.backends.cudnn.benchmark,
+                                    deterministic=torch.backends.cudnn.deterministic, allow_tf32=allow_tf32):
+        return encoder(image)
 
 
 class _TrunkFeatures(list):
@@ -374,18 +419,30 @@ class MaskModule(_PackedSource, nn.Module):
         feats_nchw = data_dict["image_features"]
         if self.training:
             raise NotImplementedError("monorec_b200.MaskModule: inference only (dropout / autograd are not implemented)")
+        x = data_dict.pop("_sfcv_nhwc", None) if data_dict.pop("_sfcv_nhwc_filled", False) else None
+        if torch.compiler.is_compiling():
+            m = torch.ops.monorec_b200.mask_module(list(sfcvs), list(feats_nchw[:4]), x, list(self.parameters()),
+                                                   self.depth_steps, list(self.feat_chns), self.use_cv, self.use_features)
+        else:
+            m = self._run(sfcvs, feats_nchw, x)
+        data_dict["cv_mask"] = m
+        return data_dict
+
+    def _run(self, sfcvs, feats_nchw, x):
+        """The U-Net on the single-frame volumes and trunk levels 0-3 -> cv_mask [B,1,H,W].  x: the volumes already in the
+        engine's NHWC layout (written by the cost-volume kernel) or None.  The implementation of the
+        `monorec_b200::mask_module` op as well."""
         P = self._packs(self._build)
         nF = len(sfcvs)
         B, D, H, W = sfcvs[0].shape
         # all frames go through the encoder as one batch of F*B volumes (the reference loops, :357-365)
-        x = data_dict.pop("_sfcv_nhwc", None) if data_dict.pop("_sfcv_nhwc_filled", False) else None
         if x is None or x.dtype != C.act_dtype() or tuple(x.shape) != (nF * B, H, W, D):
             # (standalone call, or a configuration the fused kernel does not write the engine layout for)
             x = torch.empty(nF * B, H, W, D, device=sfcvs[0].device, dtype=C.act_dtype())
             for f, v in enumerate(sfcvs):
                 C.nchw_to_nhwc(_f32_or_f16(v), out=x[f * B:(f + 1) * B])
         if not self.use_cv:
-            x.zero_()
+            x = torch.zeros_like(x)      # (x may be the caller's buffer: not written)
         cv_feats = []
         fused_pool = nF > 1 and H % 16 == 0 and W % 16 == 0   # (one pass writes the pooled tensor and the frame maximum)
         for lvl in range(5):
@@ -414,8 +471,7 @@ class MaskModule(_PackedSource, nn.Module):
                 cat = [cv_feats[3 - i], img[2 - i], x]
             x = c2([c1(cat)])
         m = P["cls"]([x], final=True)                                                # [B,H,W,1]
-        data_dict["cv_mask"] = m.view(B, 1, H, W)                                    # C == 1: NHWC == NCHW
-        return data_dict
+        return m.view(B, 1, H, W)                                                    # C == 1: NHWC == NCHW
 
 
 class DepthModule(_PackedSource, nn.Module):
@@ -495,10 +551,23 @@ class DepthModule(_PackedSource, nn.Module):
         if self.training:
             raise NotImplementedError("monorec_b200.DepthModule: inference only")
         out_range = tuple(self.out_range if out_range is None else out_range)
-        P = self._packs(self._build)
         keyframe = data_dict["keyframe"]
         cv = data_dict["cost_volume"]
         feats_nchw = data_dict["image_features"]
+        cv_mask = data_dict.get("_cv_mask_for_depth")
+        if torch.compiler.is_compiling():
+            preds = torch.ops.monorec_b200.depth_module(keyframe, cv, list(feats_nchw[:3]), cv_mask, float(out_range[0]),
+                                                        float(out_range[1]), list(self.parameters()), self.depth_steps,
+                                                        list(self.feat_chns))
+        else:
+            preds = self._run(keyframe, cv, feats_nchw, cv_mask, out_range)
+        data_dict["predicted_inverse_depths"] = preds
+        return data_dict
+
+    def _run(self, keyframe, cv, feats_nchw, cv_mask, out_range):
+        """The U-Net on cat(cost volume * (1 - cv_mask), keyframe) and trunk levels 0-2 -> the four inverse-depth maps,
+        finest first.  The implementation of the `monorec_b200::depth_module` op as well."""
+        P = self._packs(self._build)
         B, D, H, W = cv.shape
         # cat(cost_volume, keyframe) (:531); when MonoRecModel passes the unmasked volume plus `_cv_mask_for_depth`
         # the (1 - cv_mask) product of :713 is applied during the layout change
@@ -508,7 +577,7 @@ class DepthModule(_PackedSource, nn.Module):
         x = torch.empty(B, H, W, D + 3 + cpad, device=cv.device, dtype=C.act_dtype())
         if cpad:
             x[..., D + 3:].zero_()
-        C.nchw_to_nhwc(_f32_or_f16(cv), out=x, out_coff=0, one_minus=data_dict.get("_cv_mask_for_depth"))
+        C.nchw_to_nhwc(_f32_or_f16(cv), out=x, out_coff=0, one_minus=cv_mask)
         C.nchw_to_nhwc(keyframe.to(torch.float32), out=x, out_coff=D)
         img = [C.as_nhwc(f, C.act_dtype()) for f in feats_nchw[:3]]
         feats = []
@@ -529,8 +598,7 @@ class DepthModule(_PackedSource, nn.Module):
         pk, last = P["dec4"]
         x = last([self._cr2([feats[0], x], pk)])                                      # 24 @ full
         preds.insert(0, self._head(x, heads[3], out_range))
-        data_dict["predicted_inverse_depths"] = preds
-        return data_dict
+        return preds
 
     def predict_depth(self, x, scale):
         """API parity with the reference (:554-557); x is NHWC inside this implementation."""
@@ -662,11 +730,16 @@ class MonoRecModel(nn.Module):
                 data_dict["single_frame_cvs"] = [data_dict["cost_volume"].clone() for _ in data_dict["poses"]]
 
             # torchvision trunk on cuDNN, fed channels-last; TF32 is allowed there unless the engine runs its fp32 parity mode
-            # (only TF32 is decided here: the caller's cuDNN benchmark / deterministic settings are passed through)
-            with torch.backends.cudnn.flags(enabled=True, benchmark=torch.backends.cudnn.benchmark,
-                                            deterministic=torch.backends.cudnn.deterministic, allow_tf32=(C.MODE != "fp32")):
-                data_dict["image_features"] = self._feature_extractor(
-                    (keyframe + .5).contiguous(memory_format=torch.channels_last))
+            image = (keyframe + .5).contiguous(memory_format=torch.channels_last)
+            if torch.compiler.is_compiling():
+                # the cuDNN flags and the folded-weight cache are host state: set and looked up inside the op
+                enc = self._feature_extractor
+                if enc.training or enc.encoder.training:
+                    raise NotImplementedError("monorec_b200: a compiled forward runs the trunk in eval mode only")
+                data_dict["image_features"] = torch.ops.monorec_b200.resnet_trunk(image, enc._source_tensors(),
+                                                                                  C.MODE != "fp32")
+            else:
+                data_dict["image_features"] = trunk_features(self._feature_extractor, image, C.MODE != "fp32")
 
             if self.pretrain_mode == 0 or self.pretrain_mode == 2:
                 data_dict = self.att_module(data_dict)
