@@ -376,6 +376,18 @@ int mr_pointcloud_add(const float* inv_depth, const float* keyframe, const float
                       float min_d, float max_d, const int* roi, const float* dropout_rand, float dropout,
                       float* vertices, long long capacity, long long n_before, long long* n_after,
                       void* workspace, long long workspace_bytes, void* stream);
+/* mr_pointcloud_add_windows: mr_pointcloud_add for B consecutive key frames of a sequence, each voted with its own window
+ *   of keep masks (create_pointcloud.py:80-104 at batch size 1, B calls in one): a pixel of key frame b survives iff more
+ *   than n_masks - min_hits of the keep masks in ring slots window_start[b], window_start[b] + 1, ... (mod ring_len),
+ *   n_masks of them, are 1.  The vertices are appended key frame by key frame, in the order of B mr_pointcloud_add calls.
+ *   keep_ring: device [ring_len,1,H,W]; window_start: host int[B], each in [0, ring_len); 1 <= n_masks <= ring_len;
+ *   1 <= min_hits <= n_masks; 1 <= B <= 256; the other arguments as for mr_pointcloud_add (workspace:
+ *   mr_pointcloud_workspace(B,H,W) bytes). */
+int mr_pointcloud_add_windows(const float* inv_depth, const float* keyframe, const float* K, const float* pose,
+                              const float* keep_ring, int ring_len, const int* window_start, int n_masks, int min_hits,
+                              int B, int H, int W, float min_d, float max_d, const int* roi, const float* dropout_rand,
+                              float dropout, float* vertices, long long capacity, long long n_before, long long* n_after,
+                              void* workspace, long long workspace_bytes, void* stream);
 
 /* ---- photometric reprojection loss, forward and backward (SURVEY.md 8f row 4) -------------------------------------------
  * Replaces reprojection_loss (reference: model/loss_functions/common_losses.py:16-114) with error_function=compute_errors

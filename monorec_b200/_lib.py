@@ -77,6 +77,9 @@ SIGNATURES = {
     "mr_pointcloud_add": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int,
                                   c_float, c_float, POINTER(c_int), c_void_p, c_float, c_void_p, c_longlong, c_longlong, c_void_p,
                                   c_void_p, c_longlong, c_void_p]),
+    "mr_pointcloud_add_windows": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, POINTER(c_int), c_int, c_int,
+                                          c_int, c_int, c_int, c_float, c_float, POINTER(c_int), c_void_p, c_float, c_void_p,
+                                          c_longlong, c_longlong, c_void_p, c_void_p, c_longlong, c_void_p]),
     "mr_reprojection_loss_fwd": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
                                          c_void_p, c_void_p, c_void_p]),
     "mr_reprojection_loss_bwd": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,

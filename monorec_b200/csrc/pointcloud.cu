@@ -4,6 +4,8 @@
 // depth *= mask) and utils/ply_utils.py:34-53 PLYSaver.add_depthmap (1/x, distance / roi / dropout filter, Backprojection
 // (model/layers.py:43-58) with inv(K), pose transform, boolean-mask compaction, .cpu().tolist() per frame).  Here the
 // vertices stay on the device in one growing buffer, in the reference's order (batch element, then pixel, row-major).
+// mr_pointcloud_add_windows runs the same vote for a batch of consecutive key frames of a sequence, each with its own window
+// of keep masks in a device ring (create_pointcloud.py's sliding window, which crosses batch boundaries).
 #include "mr_common.cuh"
 #include <cstdint>
 
@@ -28,17 +30,47 @@ __global__ void keep_mask_kernel(const float* __restrict__ cv_mask, float* __res
     keep[((size_t)b * H + y) * W + x] = hit ? 0.f : 1.f;
 }
 
+constexpr int kMaxWindows = 256;   // key frames per mr_pointcloud_add_windows call (their window starts are kernel arguments)
+
 struct PtrPackPC {
     const float* p[16];
 };
 
+// mr_pointcloud_add: n_masks keep masks [B,1,H,W] (sliding window), the same window for every batch element; may be empty
+struct ListVote {
+    PtrPackPC keeps;
+    int n_masks;
+    __device__ __forceinline__ float sum(int b, int i, size_t hw) const {
+        float s = 0.f;
+        for (int k = 0; k < n_masks; ++k) s += __ldg(keeps.p[k] + b * hw + i);
+        return s;
+    }
+};
+
+// mr_pointcloud_add_windows: batch element b votes with ring slots start[b], start[b] + 1, ... (mod ring_len), n_masks of them
+struct RingVote {
+    const float* ring;        // [ring_len,1,H,W]
+    int ring_len, n_masks;
+    int start[kMaxWindows];
+    __device__ __forceinline__ float sum(int b, int i, size_t hw) const {
+        float s = 0.f;
+        int slot = start[b];
+        for (int k = 0; k < n_masks; ++k) {
+            s += __ldg(ring + slot * hw + i);
+            if (++slot == ring_len) slot = 0;
+        }
+        return s;
+    }
+};
+
+template <class Vote>
 struct PcArgs {
     const float* inv_depth;   // [B,1,H,W] data_dict["result"]
     const float* image;       // [B,3,H,W] keyframe in [-0.5, 0.5]
     const float* K;           // [B,4,4] keyframe intrinsics
     const float* pose;        // [B,4,4] keyframe pose (camera -> world)
-    PtrPackPC keeps;          // n_masks keep masks [B,1,H,W] (sliding window), may be empty
-    int n_masks, min_hits;
+    Vote vote;
+    int min_hits;
     const float* rnd;         // [B,1,H,W] uniform numbers for the dropout, or nullptr
     float dropout, min_d, max_d;
     int B, H, W, r0, r1, c0, c1, use_roi;
@@ -49,13 +81,13 @@ struct PcArgs {
     long long* total;         // device: number of vertices in the buffer after this call
 };
 
-__device__ __forceinline__ bool keep_vertex(const PcArgs& a, int b, int i, float& depth) {
+template <class Vote>
+__device__ __forceinline__ bool keep_vertex(const PcArgs<Vote>& a, int b, int i, float& depth) {
     const size_t o = (size_t)b * a.H * a.W + i;
     float inv = __ldg(a.inv_depth + o);
-    if (a.n_masks > 0) {     // mask = sum(mask_buffer) > buffer_length - min_hits; depth *= mask  (create_pointcloud.py:93-95)
-        float s = 0.f;
-        for (int k = 0; k < a.n_masks; ++k) s += __ldg(a.keeps.p[k] + o);
-        inv *= (s > (float)(a.n_masks - a.min_hits)) ? 1.f : 0.f;
+    if (a.vote.n_masks > 0) {   // mask = sum(mask_buffer) > buffer_length - min_hits; depth *= mask  (create_pointcloud.py:93-95)
+        const float s = a.vote.sum(b, i, (size_t)a.H * a.W);
+        inv *= (s > (float)(a.vote.n_masks - a.min_hits)) ? 1.f : 0.f;
     }
     depth = __fdiv_rn(1.0f, inv);                           // ply_utils.py:36 (1 / 0 = inf fails the range test below)
     bool ok = (a.min_d <= depth) && (depth <= a.max_d);     // :38
@@ -67,7 +99,8 @@ __device__ __forceinline__ bool keep_vertex(const PcArgs& a, int b, int i, float
     return ok;
 }
 
-__global__ void pc_count_kernel(const PcArgs a) {
+template <class Vote>
+__global__ void pc_count_kernel(const __grid_constant__ PcArgs<Vote> a) {
     const int b = blockIdx.y, i = blockIdx.x * kBlk + threadIdx.x;
     float depth;
     const bool ok = (i < a.H * a.W) && keep_vertex(a, b, i, depth);
@@ -116,7 +149,8 @@ __device__ bool invert4d(const float* src, double* out) {
     return true;
 }
 
-__global__ void pc_write_kernel(const PcArgs a) {
+template <class Vote>
+__global__ void pc_write_kernel(const __grid_constant__ PcArgs<Vote> a) {
     __shared__ float kinv[9], pose[12];
     __shared__ int wsum[kBlk / 32];
     const int b = blockIdx.y, i = blockIdx.x * kBlk + threadIdx.x;
@@ -172,6 +206,34 @@ extern "C" long long mr_pointcloud_workspace(int B, int H, int W) {
     return (long long)B * ((H * W + kBlk - 1) / kBlk) * (long long)sizeof(int);
 }
 
+namespace {
+
+// the arguments both entries share, then count -> scan -> write
+template <class Vote>
+int add_vertices(PcArgs<Vote>& a, const float* inv_depth, const float* keyframe, const float* K, const float* pose,
+                 int min_hits, int B, int H, int W, float min_d, float max_d, const int* roi, const float* dropout_rand,
+                 float dropout, float* vertices, long long capacity, long long n_before, long long* n_after, void* workspace,
+                 cudaStream_t st) {
+    a.inv_depth = inv_depth; a.image = keyframe; a.K = K; a.pose = pose;
+    a.min_hits = min_hits;
+    a.rnd = dropout_rand; a.dropout = dropout; a.min_d = min_d; a.max_d = max_d;
+    a.B = B; a.H = H; a.W = W;
+    a.use_roi = roi != nullptr;
+    if (roi) { a.r0 = roi[0]; a.r1 = roi[1]; a.c0 = roi[2]; a.c1 = roi[3]; }
+    a.counts = static_cast<int*>(workspace);
+    a.out = vertices; a.capacity = capacity; a.base = n_before; a.total = n_after;
+    const int nb = (H * W + kBlk - 1) / kBlk;
+    pc_count_kernel<<<dim3(nb, B), kBlk, 0, st>>>(a);
+    MR_LAUNCH_CHECK("pc_count_kernel");
+    pc_scan_kernel<<<1, 1024, 0, st>>>(a.counts, nb * B, n_before, capacity, n_after);
+    MR_LAUNCH_CHECK("pc_scan_kernel");
+    pc_write_kernel<<<dim3(nb, B), kBlk, 0, st>>>(a);
+    MR_LAUNCH_CHECK("pc_write_kernel");
+    return MR_OK;
+}
+
+}  // namespace
+
 extern "C" int mr_pointcloud_add(const float* inv_depth, const float* keyframe, const float* K, const float* pose,
                                  const float* const* keep_masks, int n_masks, int min_hits, int B, int H, int W, float min_d,
                                  float max_d, const int* roi, const float* dropout_rand, float dropout, float* vertices,
@@ -185,26 +247,51 @@ extern "C" int mr_pointcloud_add(const float* inv_depth, const float* keyframe, 
         mr::set_error("mr_pointcloud_add: workspace too small (%lld < %lld bytes)", workspace_bytes, mr_pointcloud_workspace(B, H, W));
         return MR_ENOMEM;
     }
-    PcArgs a{};
-    a.inv_depth = inv_depth; a.image = keyframe; a.K = K; a.pose = pose;
+    PcArgs<ListVote> a{};
     for (int k = 0; k < n_masks; ++k) {
         MR_REQUIRE(keep_masks[k] != nullptr, "mr_pointcloud_add: null mask %d", k);
-        a.keeps.p[k] = keep_masks[k];
+        a.vote.keeps.p[k] = keep_masks[k];
     }
-    a.n_masks = n_masks; a.min_hits = min_hits;
-    a.rnd = dropout_rand; a.dropout = dropout; a.min_d = min_d; a.max_d = max_d;
-    a.B = B; a.H = H; a.W = W;
-    a.use_roi = roi != nullptr;
-    if (roi) { a.r0 = roi[0]; a.r1 = roi[1]; a.c0 = roi[2]; a.c1 = roi[3]; }
-    a.counts = static_cast<int*>(workspace);
-    a.out = vertices; a.capacity = capacity; a.base = n_before; a.total = n_after;
-    const int nb = (H * W + kBlk - 1) / kBlk;
-    cudaStream_t st = (cudaStream_t)stream;
-    pc_count_kernel<<<dim3(nb, B), kBlk, 0, st>>>(a);
-    MR_LAUNCH_CHECK("pc_count_kernel");
-    pc_scan_kernel<<<1, 1024, 0, st>>>(a.counts, nb * B, n_before, capacity, n_after);
-    MR_LAUNCH_CHECK("pc_scan_kernel");
-    pc_write_kernel<<<dim3(nb, B), kBlk, 0, st>>>(a);
-    MR_LAUNCH_CHECK("pc_write_kernel");
-    return MR_OK;
+    a.vote.n_masks = n_masks;
+    return add_vertices(a, inv_depth, keyframe, K, pose, min_hits, B, H, W, min_d, max_d, roi, dropout_rand, dropout, vertices,
+                        capacity, n_before, n_after, workspace, (cudaStream_t)stream);
+}
+
+extern "C" int mr_pointcloud_add_windows(const float* inv_depth, const float* keyframe, const float* K, const float* pose,
+                                         const float* keep_ring, int ring_len, const int* window_start, int n_masks,
+                                         int min_hits, int B, int H, int W, float min_d, float max_d, const int* roi,
+                                         const float* dropout_rand, float dropout, float* vertices, long long capacity,
+                                         long long n_before, long long* n_after, void* workspace, long long workspace_bytes,
+                                         void* stream) {
+    MR_REQUIRE(inv_depth, "mr_pointcloud_add_windows: null pointer inv_depth");
+    MR_REQUIRE(keyframe, "mr_pointcloud_add_windows: null pointer keyframe");
+    MR_REQUIRE(K, "mr_pointcloud_add_windows: null pointer K");
+    MR_REQUIRE(pose, "mr_pointcloud_add_windows: null pointer pose");
+    MR_REQUIRE(keep_ring, "mr_pointcloud_add_windows: null pointer keep_ring");
+    MR_REQUIRE(window_start, "mr_pointcloud_add_windows: null pointer window_start");
+    MR_REQUIRE(vertices, "mr_pointcloud_add_windows: null pointer vertices");
+    MR_REQUIRE(n_after, "mr_pointcloud_add_windows: null pointer n_after");
+    MR_REQUIRE(workspace, "mr_pointcloud_add_windows: null pointer workspace");
+    MR_REQUIRE(B >= 1 && B <= kMaxWindows, "mr_pointcloud_add_windows: B = %d outside [1, %d]", B, kMaxWindows);
+    MR_REQUIRE(H >= 1 && W >= 1, "mr_pointcloud_add_windows: bad image size H = %d, W = %d", H, W);
+    MR_REQUIRE(ring_len >= 1 && ring_len <= 65535, "mr_pointcloud_add_windows: ring_len = %d outside [1, 65535]", ring_len);
+    MR_REQUIRE(n_masks >= 1 && n_masks <= ring_len, "mr_pointcloud_add_windows: n_masks = %d outside [1, ring_len = %d]",
+               n_masks, ring_len);
+    MR_REQUIRE(min_hits >= 1 && min_hits <= n_masks, "mr_pointcloud_add_windows: min_hits = %d outside [1, n_masks = %d]",
+               min_hits, n_masks);
+    for (int b = 0; b < B; ++b)
+        MR_REQUIRE(window_start[b] >= 0 && window_start[b] < ring_len,
+                   "mr_pointcloud_add_windows: window_start[%d] = %d outside the ring [0, %d)", b, window_start[b], ring_len);
+    MR_REQUIRE(capacity >= 0 && n_before >= 0 && n_before <= capacity,
+               "mr_pointcloud_add_windows: bad buffer position n_before = %lld, capacity = %lld", n_before, capacity);
+    if (workspace_bytes < mr_pointcloud_workspace(B, H, W)) {
+        mr::set_error("mr_pointcloud_add_windows: workspace too small (%lld < %lld bytes)", workspace_bytes,
+                      mr_pointcloud_workspace(B, H, W));
+        return MR_ENOMEM;
+    }
+    PcArgs<RingVote> a{};
+    a.vote.ring = keep_ring; a.vote.ring_len = ring_len; a.vote.n_masks = n_masks;
+    for (int b = 0; b < B; ++b) a.vote.start[b] = window_start[b];
+    return add_vertices(a, inv_depth, keyframe, K, pose, min_hits, B, H, W, min_d, max_d, roi, dropout_rand, dropout, vertices,
+                        capacity, n_before, n_after, workspace, (cudaStream_t)stream);
 }

@@ -800,6 +800,10 @@ class GraphedMonoRec:
                     dst.copy_(src, non_blocking=True)
             else:
                 v.copy_(data[k], non_blocking=True)
+        return self.replay()
+
+    def replay(self):
+        """Runs the captured forward on whatever `static_in` holds now (for callers that write the inputs in place)."""
         self.graph.replay()
         feats = self.static_out.get("image_features")
         if isinstance(feats, _TrunkFeatures):

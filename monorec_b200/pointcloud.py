@@ -60,6 +60,18 @@ class PLYSaver(torch.nn.Module):
         masks = [m.to(torch.float32).contiguous() for m in keep_masks]
         if self.dropout > 0 and rand is None:
             rand = torch.rand_like(d)                                     # ply_utils.py:44-45
+        n_before, ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.mr_pointcloud_add(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(),
+                                             _lib.ptr_array(masks) if masks else None, len(masks), int(min_hits), B, H, W,
+                                             float(self.min_d), float(self.max_d), roi,
+                                             None if rand is None else rand.contiguous().data_ptr(), float(self.dropout),
+                                             self._buf.data_ptr(), self._buf.shape[0], n_before, self._count.data_ptr(),
+                                             ws.data_ptr(), ws_bytes, torch.cuda.current_stream(dev).cuda_stream),
+                       "mr_pointcloud_add")
+
+    def _reserve(self, lib, B, H, W, dev):
+        """Room for B more depth maps: (n_before, workspace, its bytes, roi as a C array)."""
         if self._buf is None:
             self._buf = torch.empty(max(4 * B * H * W, 1 << 20), 6, device=dev)
             self._count = torch.zeros(1, dtype=torch.int64, device=dev)
@@ -72,14 +84,40 @@ class PLYSaver(torch.nn.Module):
             grown = torch.empty(2 * (n_before + B * H * W), 6, device=dev)
             grown[:n_before] = self._buf[:n_before]
             self._buf = grown
+        return n_before, ws, ws_bytes, roi
+
+    def add_depthmap_windows(self, depth, image, intrinsics, extrinsics, keep_ring, window_start, n_masks, min_hits=1,
+                             rand=None):
+        """`add_depthmap` of B consecutive key frames, each voted with its own window: key frame b keeps the pixels where
+        more than n_masks - min_hits of the keep masks in ring slots window_start[b], window_start[b] + 1, ...
+        (mod len(keep_ring)) are 1.  The vertices are those of B add_depthmap calls, in the same order.
+        keep_ring: device [R,1,H,W]; window_start: B host ints."""
+        if not depth.is_cuda:
+            raise _lib.MonorecLibraryError("monorec_b200.pointcloud needs CUDA tensors (no CPU fallback)")
+        lib = _lib.load()
+        dev = depth.device
+        d = depth.to(torch.float32).contiguous()
+        img = image.to(torch.float32).contiguous()
+        K = intrinsics.to(torch.float32).contiguous()
+        P = extrinsics.to(torch.float32).contiguous()
+        ring = keep_ring.to(torch.float32).contiguous()
+        B, _, H, W = d.shape
+        if len(window_start) != B or tuple(ring.shape[1:]) != (1, H, W):
+            raise ValueError(f"add_depthmap_windows: {len(window_start)} window starts and a keep ring of "
+                             f"{tuple(ring.shape)} for depth maps {tuple(d.shape)}")
+        if self.dropout > 0 and rand is None:
+            rand = torch.rand_like(d)                                     # ply_utils.py:44-45
+        starts = (ctypes.c_int * B)(*[int(v) for v in window_start])
+        n_before, ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.mr_pointcloud_add(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(),
-                                             _lib.ptr_array(masks) if masks else None, len(masks), int(min_hits), B, H, W,
-                                             float(self.min_d), float(self.max_d), roi,
-                                             None if rand is None else rand.contiguous().data_ptr(), float(self.dropout),
-                                             self._buf.data_ptr(), self._buf.shape[0], n_before, self._count.data_ptr(),
-                                             ws.data_ptr(), ws_bytes, torch.cuda.current_stream(dev).cuda_stream),
-                       "mr_pointcloud_add")
+            _lib.check(lib.mr_pointcloud_add_windows(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(), ring.data_ptr(),
+                                                     ring.shape[0], starts, int(n_masks), int(min_hits), B, H, W,
+                                                     float(self.min_d), float(self.max_d), roi,
+                                                     None if rand is None else rand.contiguous().data_ptr(),
+                                                     float(self.dropout), self._buf.data_ptr(), self._buf.shape[0], n_before,
+                                                     self._count.data_ptr(), ws.data_ptr(), ws_bytes,
+                                                     torch.cuda.current_stream(dev).cuda_stream),
+                       "mr_pointcloud_add_windows")
 
     def save(self, file):
         """Binary little-endian PLY, the reference's header (ply_utils.py:20-32)."""
@@ -112,3 +150,88 @@ class MaskVoter:
         del self.frames[0]
         return {"depth": key[4], "keyframe": key[3], "intrinsics": key[2], "pose": key[1], "keep_masks": masks,
                 "min_hits": self.min_hits}
+
+
+class SequencePointCloud:
+    """create_pointcloud.py:65-105 over a `MonoRecSequence`: push frames, and every key frame the sequence runs is voted with
+    the keep masks of the `buffer_length` key frames around it and added to `saver`, as the reference's loop does at batch
+    size 1.  The windows cross batch boundaries: this keeps its own ring of keep masks, and the last buffer_length // 2
+    key frames of a batch wait for the next one.  One `mr_pointcloud_add_windows` call per batch.
+
+    `push(image, pose, intrinsics, rand=None)` and `flush()` forward to the sequence and return what it returns.  `rand`
+    [1,H,W] (or [1,1,H,W]): the dropout numbers of this frame's depth map, used if it is added (`add_depthmap`'s `rand`);
+    uniform random numbers when None and `saver.dropout` > 0."""
+
+    def __init__(self, seq, saver, buffer_length=5, min_hits=1, mask_fill=32, thresh=0.1):
+        if buffer_length < 1 or not 1 <= min_hits <= buffer_length:
+            raise ValueError(f"buffer_length ({buffer_length}) >= 1 and 1 <= min_hits ({min_hits}) <= buffer_length needed")
+        if seq.batch_size > 256:
+            raise ValueError(f"sequence_pointcloud: batch_size {seq.batch_size} > 256 (mr_pointcloud_add_windows' limit)")
+        self.seq, self.saver = seq, saver
+        self.buffer_length, self.min_hits, self.mask_fill, self.thresh = buffer_length, min_hits, mask_fill, thresh
+        self.key_index = buffer_length // 2
+        # a batch's windows span its own key frames plus buffer_length - 1 earlier ones
+        self.ring_len = seq.batch_size + buffer_length - 1
+        self._keep = None          # [ring_len,1,H,W]: keep mask of the key frame run n-th in slot n % ring_len
+        self._n_run = 0            # key frames run so far
+        self._waiting = None       # (positions, depth, keyframe, intrinsics, pose) of run key frames whose window is open
+        self._rand = {}            # sequence index -> dropout numbers of the key frame
+
+    def push(self, image, pose, intrinsics, rand=None):
+        if rand is not None:
+            self._rand[self.seq.n_pushed] = rand.to(self.seq.device, torch.float32).reshape(1, 1, *rand.shape[-2:])
+        emitted = self.seq.push(image, pose, intrinsics)
+        self._add(emitted)
+        return emitted
+
+    def flush(self):
+        emitted = self.seq.flush()
+        self._add(emitted)
+        return emitted
+
+    def _add(self, emitted):
+        if not emitted:
+            return
+        n, R = len(emitted), self.ring_len
+        keep = keep_mask(torch.cat([o["cv_mask"] for _, o in emitted]), self.mask_fill, self.thresh)
+        if self._keep is None:
+            self._keep = torch.empty((R,) + tuple(keep.shape[1:]), device=keep.device)
+        first = self._n_run % R                                   # at most two contiguous runs of slots
+        k = min(n, R - first)
+        self._keep[first:first + k] = keep[:k]
+        self._keep[:n - k] = keep[k:]
+        # the key frames with a complete window: positions key_index .. last - (buffer_length - 1 - key_index)
+        pos = list(range(self._n_run, self._n_run + n))
+        fields = [torch.cat([o[key] for _, o in emitted]) for key in ("result", "keyframe", "keyframe_intrinsics",
+                                                                      "keyframe_pose")]
+        index = [i for i, _ in emitted]
+        if self._waiting is not None:
+            pos = self._waiting[0] + pos
+            index = self._waiting[1] + index
+            fields = [torch.cat([w, f]) for w, f in zip(self._waiting[2], fields)]
+        self._n_run += n
+        last_ready = self._n_run - 1 - (self.buffer_length - 1 - self.key_index)
+        lo = sum(1 for p in pos if p < self.key_index)             # never added: their window starts before the sequence
+        hi = sum(1 for p in pos if p <= last_ready)
+        if hi > lo:
+            if self.saver.dropout > 0:
+                shape = (1, 1) + tuple(fields[0].shape[-2:])
+                rand = torch.cat([self._rand[i] if i in self._rand else torch.rand(shape, device=keep.device)
+                                  for i in index[lo:hi]])
+            else:
+                rand = None
+            self.saver.add_depthmap_windows(*[f[lo:hi] for f in fields], self._keep,
+                                            [(p - self.key_index) % R for p in pos[lo:hi]], self.buffer_length,
+                                            self.min_hits, rand=rand)
+        # the rest waits for the next batch (`fields` are torch.cat copies: the next replay does not overwrite them)
+        hi = max(hi, lo)
+        self._waiting = (pos[hi:], index[hi:], [f[hi:] for f in fields]) if hi < len(pos) else None
+        upto = index[hi - 1] if hi > 0 else None
+        if upto is not None:
+            self._rand = {i: r for i, r in self._rand.items() if i > upto}
+
+
+def sequence_pointcloud(seq, saver, buffer_length=5, min_hits=1, mask_fill=32):
+    """The point-cloud export of create_pointcloud.py over `seq` (a MonoRecSequence) into `saver` (a PLYSaver); see
+    `SequencePointCloud`."""
+    return SequencePointCloud(seq, saver, buffer_length=buffer_length, min_hits=min_hits, mask_fill=mask_fill)

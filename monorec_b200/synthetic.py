@@ -84,6 +84,20 @@ def make_inputs(batch, frames, height, width, seed=0, noise=0.05, device="cpu"):
     return data
 
 
+def make_sequence(n_frames, height, width, seed=0, step=0.8, noise=0.05):
+    """A synthetic KITTI-shaped video: camera n sits n * step m down the z axis (with a <= 0.5 degree random rotation) and
+    sees the shared texture shifted by n pixels.  Returns images [N,3,H,W] in [-0.5, 0.5], cam -> world poses [N,4,4] and
+    intrinsics [N,4,4], on the CPU."""
+    gen = torch.Generator().manual_seed(seed)
+    base = _texture(gen, 1, height, width)[0]
+    images = torch.stack([_quantise(torch.roll(base, shifts=(n // 2, n), dims=(1, 2))
+                                    + noise * (torch.rand(3, height, width, generator=gen) - 0.5)) for n in range(n_frames)])
+    poses = torch.eye(4).repeat(n_frames, 1, 1)
+    poses[:, :3, :3] = _small_rotation(gen, n_frames)
+    poses[:, 2, 3] = step * torch.arange(n_frames, dtype=torch.float32)
+    return images.contiguous(), poses, kitti_intrinsics(height, width, n_frames)
+
+
 def to_device(data, device, non_blocking=False):
     out = {}
     for k, v in data.items():
