@@ -353,6 +353,22 @@ int mr_dense_metrics(const float* result, const float* target, int B, int H, int
 long long mr_median_scaling_workspace(int B, int H, int W);
 int mr_median_scaling(const float* result, const float* target, float* out, int B, int H, int W, void* workspace,
                       long long workspace_bytes, void* stream);
+/* mr_sparse_metrics_grouped / mr_dense_metrics_grouped: the same passes over G = ceil(B / group) consecutive groups of `group`
+ * images (the last group may be shorter), one row per group: out_metrics is device float[G][7] / [G][12], and row g is what
+ * mr_sparse_metrics / mr_dense_metrics return for images [g * group, min(B, (g + 1) * group)) -- the evaluater's batches of
+ * a run of key frames in one launch pair.  mr_sparse_metrics / mr_dense_metrics are the case group = B.  Same workspace.
+ * mr_eval_accumulate: the evaluater's bookkeeping (evaluater/evaluater.py:45-49, 94-103) on the device, in its float64
+ * operation order.  values: device float[G][M], the M metrics of G batches in batch order; group_sizes: host int[G], the
+ * images per batch; state: device double[3M + 1] = total[M], valid[M], running_avg[M], num_samples, zero at the start of an
+ * evaluation.  Per batch: a row holding a NaN adds zeros to total and running_avg and 0 to valid (else the widened values
+ * and 1); the first batch (num_samples == 0) is added to running_avg, a later one of b images sets it to
+ * avg * (n / (n + b)) + m * (b / (n + b)); then num_samples += b.  1 <= M <= 1024.  No host synchronisation. */
+int mr_sparse_metrics_grouped(const float* result, const float* target, const float* mvobj_mask, int B, int group, int H, int W,
+                              const int* roi, float max_distance, int pred_all_valid, float* out_metrics,
+                              void* workspace, long long workspace_bytes, void* stream);
+int mr_dense_metrics_grouped(const float* result, const float* target, int B, int group, int H, int W, const int* roi,
+                             float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes, void* stream);
+int mr_eval_accumulate(const float* values, int G, int M, const int* group_sizes, double* state, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Point-cloud side (SURVEY.md section 8f row 3): create_pointcloud.py:65-105 + utils/ply_utils.py:34-53 on the device.

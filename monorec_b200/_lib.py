@@ -72,6 +72,11 @@ SIGNATURES = {
                                  c_void_p]),
     "mr_median_scaling_workspace": (c_longlong, [c_int, c_int, c_int]),
     "mr_median_scaling": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p]),
+    "mr_sparse_metrics_grouped": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_float,
+                                          c_int, c_void_p, c_void_p, c_longlong, c_void_p]),
+    "mr_dense_metrics_grouped": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_float, c_void_p,
+                                         c_void_p, c_longlong, c_void_p]),
+    "mr_eval_accumulate": (c_int, [c_void_p, c_int, c_int, POINTER(c_int), c_void_p, c_void_p]),
     "mr_pointcloud_keep_mask": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mr_pointcloud_workspace": (c_longlong, [c_int, c_int, c_int]),
     "mr_pointcloud_add": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_void_p), c_int, c_int, c_int, c_int, c_int,

@@ -1,10 +1,12 @@
-// Evaluation-side helpers of SURVEY.md section 8f row 2 (include/monorec_b200.h: mr_sparse_metrics, mr_dense_metrics,
-// mr_median_scaling, mr_images_u8_to_f32).
+// Evaluation-side helpers of SURVEY.md section 8f row 2 (include/monorec_b200.h: mr_sparse_metrics, mr_dense_metrics and their
+// _grouped forms, mr_eval_accumulate, mr_median_scaling, mr_images_u8_to_f32).
 //
 //  * the seven sparse depth metrics of model/metric_functions/sparse_metrics.py:81-251 (a1, a2, a3, rmse, rmse_log, abs_rel,
 //    sq_rel; helpers utils/util.py:36-65, :101-118) in ONE pass over `result` / `target` instead of 7 x ~12 elementwise torch
 //    kernels per batch (evaluater/evaluater.py:78-112 calls the seven functions one after the other);
 //  * the twelve dense and completeness metrics (sparse_metrics.py:6-78, dense_metrics.py, completeness_metrics.py) in one pass;
+//  * both passes over several evaluater batches at once (consecutive groups of images, one row of metrics per group), and the
+//    evaluater's float64 totals and running average (evaluater.py:45-49, 94-103) updated on the device;
 //  * the evaluater's median scaling (utils/util.py:135-142) with an exact radix select and no host synchronisation;
 //  * the loader's image normalisation (data_loader/kitti_odometry_dataset.py:126-132: uint8 HWC -> float CHW / 255 - .5) on the
 //    device, so that uint8 images (a quarter of the bytes) cross PCIe.
@@ -77,25 +79,29 @@ __global__ void sparse_metric_sums_kernel(const MetricArgs a) {
     }
 }
 
-// out[7] = a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel exactly as the reference combines them: the a* / *_rel metrics are
-// means over every unmasked pixel of the batch (mask_mean with dim=None), rmse / rmse_log are batch means of per-image roots
-__global__ void sparse_metric_finalize_kernel(const double* sums, int B, float* out) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+// out[g][7] = a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel of images [g * group, min(B, (g + 1) * group)) exactly as the
+// reference combines a batch: the a* / *_rel metrics are means over every unmasked pixel of the batch (mask_mean with
+// dim=None), rmse / rmse_log are batch means of per-image roots.  One thread per group; group = B is the ungrouped pass
+__global__ void sparse_metric_finalize_kernel(const double* sums, int B, int group, int G, float* out) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= G) return;
+    const int b0 = g * group, b1 = min(B, b0 + group), nb = b1 - b0;
     double tot[kSums] = {0, 0, 0, 0, 0, 0, 0, 0};
     double rm = 0.0, rl = 0.0;
-    for (int b = 0; b < B; ++b) {
+    for (int b = b0; b < b1; ++b) {
         const double* s = sums + (size_t)b * kSums;
         for (int k = 0; k < kSums; ++k) tot[k] += s[k];
         rm += sqrt(s[4] / s[0]);        // 0 / 0 = NaN for an image without ground truth, like the reference
         rl += sqrt(s[5] / s[0]);
     }
-    out[0] = (float)(tot[1] / tot[0]);
-    out[1] = (float)(tot[2] / tot[0]);
-    out[2] = (float)(tot[3] / tot[0]);
-    out[3] = (float)(rm / B);
-    out[4] = (float)(rl / B);
-    out[5] = (float)(tot[6] / tot[0]);
-    out[6] = (float)(tot[7] / tot[0]);
+    float* o = out + (size_t)g * 7;
+    o[0] = (float)(tot[1] / tot[0]);
+    o[1] = (float)(tot[2] / tot[0]);
+    o[2] = (float)(tot[3] / tot[0]);
+    o[3] = (float)(rm / nb);
+    o[4] = (float)(rl / nb);
+    o[5] = (float)(tot[6] / tot[0]);
+    o[6] = (float)(tot[7] / tot[0]);
 }
 
 // ---- dense metrics (model/metric_functions/sparse_metrics.py:6-78, dense_metrics.py, completeness_metrics.py) -------------
@@ -171,14 +177,18 @@ __global__ void dense_metric_sums_kernel(const DenseArgs a) {
     }
 }
 
-// out[12] = a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel, sc_inv, l1_rel, l1_inv, completeness, covered_gt
-__global__ void dense_metric_finalize_kernel(const double* sums, int B, int H, int W, long long n_roi, float* out) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+// out[g][12] = a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel, sc_inv, l1_rel, l1_inv, completeness, covered_gt of images
+// [g * group, min(B, (g + 1) * group)), one thread per group; group = B is the ungrouped pass
+__global__ void dense_metric_finalize_kernel(const double* sums, int B, int group, int G, int H, int W, long long n_roi,
+                                             float* out) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= G) return;
+    const int b0 = g * group, b1 = min(B, b0 + group), nb = b1 - b0;
     double tot[kDenseSums];
     for (int k = 0; k < kDenseSums; ++k) tot[k] = 0.0;
     double rm = 0.0, rl = 0.0, si = 0.0;
-    const double n = (double)n_roi, N = n * B;
-    for (int b = 0; b < B; ++b) {
+    const double n = (double)n_roi, N = n * nb;
+    for (int b = b0; b < b1; ++b) {
         const double* s = sums + (size_t)b * kDenseSums;
         for (int k = 0; k < kDenseSums; ++k) tot[k] += s[k];
         rm += sqrt(s[3] / n);                             // rmse / rmse_log: batch mean of per-image roots
@@ -186,18 +196,59 @@ __global__ void dense_metric_finalize_kernel(const double* sums, int B, int H, i
         const double v = sqrt(s[8] / n - s[7] * s[7] / (n * n));
         si += isnan(v) ? 0.0 : v;                         // batch_metric[isnan(batch_metric)] = 0
     }
-    out[0] = (float)(tot[0] / N);
-    out[1] = (float)(tot[1] / N);
-    out[2] = (float)(tot[2] / N);
-    out[3] = (float)(rm / B);
-    out[4] = (float)(rl / B);
-    out[5] = (float)(tot[5] / N);
-    out[6] = (float)(tot[6] / N);
-    out[7] = (float)(si / B);
-    out[8] = out[5];                                      // l1_rel_metric is abs_rel_metric's formula
-    out[9] = (float)(tot[9] / N);
-    out[10] = (float)(tot[10] / ((double)B * H * W));
-    out[11] = (float)(tot[11] / tot[12]);                 // mask_mean over the pixels where target == 0
+    float* o = out + (size_t)g * 12;
+    o[0] = (float)(tot[0] / N);
+    o[1] = (float)(tot[1] / N);
+    o[2] = (float)(tot[2] / N);
+    o[3] = (float)(rm / nb);
+    o[4] = (float)(rl / nb);
+    o[5] = (float)(tot[5] / N);
+    o[6] = (float)(tot[6] / N);
+    o[7] = (float)(si / nb);
+    o[8] = o[5];                                          // l1_rel_metric is abs_rel_metric's formula
+    o[9] = (float)(tot[9] / N);
+    o[10] = (float)(tot[10] / ((double)nb * H * W));
+    o[11] = (float)(tot[11] / tot[12]);                   // mask_mean over the pixels where target == 0
+}
+
+// ---- the evaluater's bookkeeping (evaluater/evaluater.py:45-49, 94-103) ---------------------------------------------------
+// state: total[M], valid[M], running_avg[M], num_samples.  Thread j owns column j and applies the groups in order, in the
+// float64 operations numpy does (no contraction into an FMA): a row with a NaN adds zeros and valid 0, the first group
+// ever is added to the running average, a later one of b images gives avg * (n / (n + b)) + m * (b / (n + b)).
+constexpr int kAccGroups = 32;   // groups per launch; longer lists are applied by consecutive launches on the stream
+
+struct AccArgs {
+    const float* values;   // [G][M]
+    double* state;         // [3M + 1]
+    int G, M, g0;          // groups g0 .. g0 + G - 1 of values
+    int sizes[kAccGroups];
+};
+
+__global__ void eval_accumulate_kernel(const AccArgs a) {
+    const int j = threadIdx.x, M = a.M;
+    double* total = a.state;
+    double* valid = a.state + M;
+    double* avg = a.state + 2 * M;
+    double n = a.state[3 * M];
+    double t = 0.0, v = 0.0, r = 0.0;
+    if (j < M) { t = total[j]; v = valid[j]; r = avg[j]; }
+    for (int g = 0; g < a.G; ++g) {
+        const float* row = a.values + (size_t)(a.g0 + g) * M;
+        bool nan_row = false;
+        for (int k = 0; k < M; ++k) nan_row = nan_row || isnan(row[k]);
+        const double b = (double)a.sizes[g];
+        if (j < M) {
+            const double m = nan_row ? 0.0 : (double)row[j];
+            t = __dadd_rn(t, m);
+            v = __dadd_rn(v, nan_row ? 0.0 : 1.0);
+            if (n == 0.0) r = __dadd_rn(r, m);
+            else r = __dadd_rn(__dmul_rn(r, __ddiv_rn(n, n + b)), __dmul_rn(m, __ddiv_rn(b, n + b)));
+        }
+        n += b;
+    }
+    __syncthreads();                                      // every thread has read num_samples
+    if (j < M) { total[j] = t; valid[j] = v; avg[j] = r; }
+    if (j == 0) a.state[3 * M] = n;
 }
 
 // ---- median scaling (utils/util.py:135-142) ------------------------------------------------------------------------------
@@ -328,20 +379,22 @@ extern "C" long long mr_sparse_metrics_workspace(int B) { return B < 1 ? 0 : (lo
 
 extern "C" long long mr_dense_metrics_workspace(int B) { return B < 1 ? 0 : (long long)B * kDenseSums * (long long)sizeof(double); }
 
-extern "C" int mr_dense_metrics(const float* result, const float* target, int B, int H, int W, const int* roi, float min_inv_depth,
-                                float* out_metrics, void* workspace, long long workspace_bytes, void* stream) {
-    MR_REQUIRE(result && target && out_metrics && workspace, "mr_dense_metrics: null pointer (result, target, out_metrics, workspace)");
+static int dense_metrics_run(const char* fn, const float* result, const float* target, int B, int group, int H, int W,
+                             const int* roi, float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes,
+                             void* stream) {
+    MR_REQUIRE(result && target && out_metrics && workspace, "%s: null pointer (result, target, out_metrics, workspace)", fn);
     MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1 && (long long)H * W <= 0x7fffffffLL,
-               "mr_dense_metrics: bad shape B=%d H=%d W=%d", B, H, W);
+               "%s: bad shape B=%d H=%d W=%d", fn, B, H, W);
+    MR_REQUIRE(group >= 1, "%s: group=%d must be >= 1", fn, group);
     if (workspace_bytes < mr_dense_metrics_workspace(B)) {
-        mr::set_error("mr_dense_metrics: workspace too small (%lld < %lld bytes)", workspace_bytes, mr_dense_metrics_workspace(B));
+        mr::set_error("%s: workspace too small (%lld < %lld bytes)", fn, workspace_bytes, mr_dense_metrics_workspace(B));
         return MR_ENOMEM;
     }
-    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "mr_dense_metrics: workspace must be 8-byte aligned");
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "%s: workspace must be 8-byte aligned", fn);
     DenseArgs a{};
     a.pred = result; a.gt = target; a.B = B; a.H = H; a.W = W;
     clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
-    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "mr_dense_metrics: empty region of interest (roi)");
+    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "%s: empty region of interest (roi)", fn);
     a.min_inv = min_inv_depth;
     a.sums = static_cast<double*>(workspace);
     cudaStream_t st = (cudaStream_t)stream;
@@ -351,9 +404,24 @@ extern "C" int mr_dense_metrics(const float* result, const float* target, int B,
     if (rc != MR_OK) return rc;
     dense_metric_sums_kernel<<<dim3(blocks, B), 256, 0, st>>>(a);
     MR_LAUNCH_CHECK("dense_metric_sums_kernel");
-    dense_metric_finalize_kernel<<<1, 32, 0, st>>>(a.sums, B, H, W, (long long)(a.r1 - a.r0) * (a.c1 - a.c0), out_metrics);
+    const int G = (B + group - 1) / group;
+    dense_metric_finalize_kernel<<<(G + 31) / 32, 32, 0, st>>>(a.sums, B, group, G, H, W,
+                                                               (long long)(a.r1 - a.r0) * (a.c1 - a.c0), out_metrics);
     MR_LAUNCH_CHECK("dense_metric_finalize_kernel");
     return MR_OK;
+}
+
+extern "C" int mr_dense_metrics(const float* result, const float* target, int B, int H, int W, const int* roi, float min_inv_depth,
+                                float* out_metrics, void* workspace, long long workspace_bytes, void* stream) {
+    return dense_metrics_run("mr_dense_metrics", result, target, B, B, H, W, roi, min_inv_depth, out_metrics, workspace,
+                             workspace_bytes, stream);
+}
+
+extern "C" int mr_dense_metrics_grouped(const float* result, const float* target, int B, int group, int H, int W, const int* roi,
+                                        float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes,
+                                        void* stream) {
+    return dense_metrics_run("mr_dense_metrics_grouped", result, target, B, group, H, W, roi, min_inv_depth, out_metrics,
+                             workspace, workspace_bytes, stream);
 }
 
 extern "C" long long mr_median_scaling_workspace(int B, int H, int W) {
@@ -393,20 +461,21 @@ extern "C" int mr_median_scaling(const float* result, const float* target, float
     return MR_OK;
 }
 
-extern "C" int mr_sparse_metrics(const float* result, const float* target, const float* mvobj_mask, int B, int H, int W,
-                                 const int* roi, float max_distance, int pred_all_valid, float* out_metrics, void* workspace,
-                                 long long workspace_bytes, void* stream) {
-    MR_REQUIRE(result && target && out_metrics && workspace, "mr_sparse_metrics: null pointer");
-    MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1, "mr_sparse_metrics: bad shape B=%d H=%d W=%d", B, H, W);
+static int sparse_metrics_run(const char* fn, const float* result, const float* target, const float* mvobj_mask, int B,
+                              int group, int H, int W, const int* roi, float max_distance, int pred_all_valid, float* out_metrics,
+                              void* workspace, long long workspace_bytes, void* stream) {
+    MR_REQUIRE(result && target && out_metrics && workspace, "%s: null pointer", fn);
+    MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1, "%s: bad shape B=%d H=%d W=%d", fn, B, H, W);
+    MR_REQUIRE(group >= 1, "%s: group=%d must be >= 1", fn, group);
     if (workspace_bytes < mr_sparse_metrics_workspace(B)) {
-        mr::set_error("mr_sparse_metrics: workspace too small (%lld < %lld bytes)", workspace_bytes, mr_sparse_metrics_workspace(B));
+        mr::set_error("%s: workspace too small (%lld < %lld bytes)", fn, workspace_bytes, mr_sparse_metrics_workspace(B));
         return MR_ENOMEM;
     }
-    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "mr_sparse_metrics: workspace must be 8-byte aligned");
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "%s: workspace must be 8-byte aligned", fn);
     MetricArgs a{};
     a.pred = result; a.gt = target; a.mvobj = mvobj_mask; a.B = B; a.H = H; a.W = W;
     clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
-    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "mr_sparse_metrics: empty region of interest");
+    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "%s: empty region of interest", fn);
     a.inv_max = max_distance > 0.f ? 1.0f / max_distance : 0.f;
     a.pred_all_valid = pred_all_valid;
     a.sums = static_cast<double*>(workspace);
@@ -417,8 +486,41 @@ extern "C" int mr_sparse_metrics(const float* result, const float* target, const
     if (rc != MR_OK) return rc;
     sparse_metric_sums_kernel<<<dim3(blocks, B), 256, 0, st>>>(a);
     MR_LAUNCH_CHECK("sparse_metric_sums_kernel");
-    sparse_metric_finalize_kernel<<<1, 32, 0, st>>>(a.sums, B, out_metrics);
+    const int G = (B + group - 1) / group;
+    sparse_metric_finalize_kernel<<<(G + 31) / 32, 32, 0, st>>>(a.sums, B, group, G, out_metrics);
     MR_LAUNCH_CHECK("sparse_metric_finalize_kernel");
+    return MR_OK;
+}
+
+extern "C" int mr_sparse_metrics(const float* result, const float* target, const float* mvobj_mask, int B, int H, int W,
+                                 const int* roi, float max_distance, int pred_all_valid, float* out_metrics, void* workspace,
+                                 long long workspace_bytes, void* stream) {
+    return sparse_metrics_run("mr_sparse_metrics", result, target, mvobj_mask, B, B, H, W, roi, max_distance, pred_all_valid,
+                              out_metrics, workspace, workspace_bytes, stream);
+}
+
+extern "C" int mr_sparse_metrics_grouped(const float* result, const float* target, const float* mvobj_mask, int B, int group,
+                                         int H, int W, const int* roi, float max_distance, int pred_all_valid,
+                                         float* out_metrics, void* workspace, long long workspace_bytes, void* stream) {
+    return sparse_metrics_run("mr_sparse_metrics_grouped", result, target, mvobj_mask, B, group, H, W, roi, max_distance,
+                              pred_all_valid, out_metrics, workspace, workspace_bytes, stream);
+}
+
+extern "C" int mr_eval_accumulate(const float* values, int G, int M, const int* group_sizes, double* state, void* stream) {
+    MR_REQUIRE(values && group_sizes && state, "mr_eval_accumulate: null pointer (values, group_sizes, state)");
+    MR_REQUIRE(G >= 1 && M >= 1 && M <= 1024, "mr_eval_accumulate: bad shape G=%d M=%d (1 <= M <= 1024)", G, M);
+    for (int g = 0; g < G; ++g)
+        MR_REQUIRE(group_sizes[g] >= 1, "mr_eval_accumulate: group_sizes[%d] = %d must be >= 1", g, group_sizes[g]);
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(state) & 7) == 0, "mr_eval_accumulate: state must be 8-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    for (int g0 = 0; g0 < G; g0 += kAccGroups) {
+        AccArgs a{};
+        a.values = values; a.state = state; a.M = M; a.g0 = g0;
+        a.G = G - g0 < kAccGroups ? G - g0 : kAccGroups;
+        for (int g = 0; g < a.G; ++g) a.sizes[g] = group_sizes[g0 + g];
+        eval_accumulate_kernel<<<1, (M + 31) / 32 * 32, 0, st>>>(a);
+        MR_LAUNCH_CHECK("eval_accumulate_kernel");
+    }
     return MR_OK;
 }
 

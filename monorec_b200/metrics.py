@@ -193,6 +193,62 @@ def median_scaling_impl(pred: Tensor, gt: Tensor) -> Tensor:
     return out
 
 
+def sparse_metrics_grouped_impl(pred: Tensor, gt: Tensor, mvobj_mask: Optional[Tensor], roi: Optional[List[int]],
+                                max_distance: float, pred_all_valid: bool, group: int) -> Tensor:
+    """mr_sparse_metrics_grouped -> [G,7]: row g is sparse_metrics_impl of images [g * group, (g + 1) * group) (the last
+    group may be shorter), from one pass over the whole batch."""
+    lib = _lib.load()
+    pred = pred.to(torch.float32).contiguous()
+    gt = gt.to(device=pred.device, dtype=torch.float32).contiguous()
+    B, _, H, W = pred.shape
+    mv = None if mvobj_mask is None else mvobj_mask.to(device=pred.device, dtype=torch.float32).contiguous()
+    out = torch.empty(-(-B // group), 7, device=pred.device, dtype=torch.float32)
+    ws_bytes = lib.mr_sparse_metrics_workspace(B)
+    ws = torch.empty(ws_bytes // 8, device=pred.device, dtype=torch.float64)
+    roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
+    with torch.cuda.device(pred.device):
+        _lib.check(lib.mr_sparse_metrics_grouped(pred.data_ptr(), gt.data_ptr(), None if mv is None else mv.data_ptr(), B,
+                                                 int(group), H, W, roi_c, max_distance, 1 if pred_all_valid else 0,
+                                                 out.data_ptr(), ws.data_ptr(), ws_bytes,
+                                                 torch.cuda.current_stream(pred.device).cuda_stream),
+                   "mr_sparse_metrics_grouped")
+    return out
+
+
+def dense_metrics_grouped_impl(pred: Tensor, gt: Tensor, roi: Optional[List[int]], min_inv: float, group: int) -> Tensor:
+    """mr_dense_metrics_grouped -> [G,12]: row g is dense_metrics_impl of images [g * group, (g + 1) * group)."""
+    lib = _lib.load()
+    p = pred.to(torch.float32).contiguous()
+    g = gt.to(device=p.device, dtype=torch.float32).contiguous()
+    B, _, H, W = p.shape
+    out = torch.empty(-(-B // group), len(DENSE_NAMES), device=p.device, dtype=torch.float32)
+    ws_bytes = lib.mr_dense_metrics_workspace(B)
+    ws = torch.empty(ws_bytes // 8, device=p.device, dtype=torch.float64)
+    roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
+    with torch.cuda.device(p.device):
+        _lib.check(lib.mr_dense_metrics_grouped(p.data_ptr(), g.data_ptr(), B, int(group), H, W, roi_c, min_inv, out.data_ptr(),
+                                                ws.data_ptr(), ws_bytes, torch.cuda.current_stream(p.device).cuda_stream),
+                   "mr_dense_metrics_grouped")
+    return out
+
+
+def eval_accumulate_impl(values: Tensor, group_sizes: List[int], state: Tensor) -> Tensor:
+    """mr_eval_accumulate: folds the metric rows `values` [G,M] (fp32, device) of G evaluater batches of `group_sizes`
+    images into `state` (float64 [3M+1] on the device: total, valid, running average, number of samples), in place, as
+    evaluater.py:45-49, 94-103 does batch after batch.  Returns `state`."""
+    lib = _lib.load()
+    v = values.to(torch.float32).contiguous()
+    G, M = v.shape
+    if len(group_sizes) != G or state.dtype != torch.float64 or state.numel() != 3 * M + 1 or not state.is_contiguous():
+        raise ValueError(f"eval_accumulate: {len(group_sizes)} group sizes and a {state.dtype} state of {state.numel()} "
+                         f"values for metric rows {tuple(v.shape)} (float64 [3M+1] contiguous expected)")
+    sizes = (ctypes.c_int * G)(*[int(n) for n in group_sizes])
+    with torch.cuda.device(v.device):
+        _lib.check(lib.mr_eval_accumulate(v.data_ptr(), G, M, sizes, state.data_ptr(),
+                                          torch.cuda.current_stream(v.device).cuda_stream), "mr_eval_accumulate")
+    return state
+
+
 def images_u8_to_f32(images_u8, crop_box=None):
     """uint8 HWC images [B,Hs,Ws,3] on the device -> float CHW [B,3,H,W] = u / 255 - 0.5, optionally cropped to the PIL-style
     box (left, upper, right, lower) -- kitti_odometry_dataset.py:121-132 without the resize."""
