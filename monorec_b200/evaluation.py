@@ -61,9 +61,18 @@ class SequenceEvaluater:
     `log()` makes the one device-to-host read and returns the evaluater's dict: `loss` and `loss_loss` 0.0, `metrics` (total
     over valid batches: NaN for a metric no batch was valid for), `metrics_correct` (the running average over samples) and
     `valid_batches`.  Batches still open are not in it: call `flush()` first.
+
+    Several processes (one per GPU, or several on one GPU) evaluate one run together with `group` (a torch.distributed
+    process group) and `shard`, this rank's slices of the sequences (`dist.shard_sequences(..., eval_batch=batch_size)`):
+    `seq` and every sequence given to `next_sequence` run `shard`'s slices in order (MonoRecSequence(first_frame=
+    slice.frames[0], key_end=slice.run[1]), fed frames slice.frames[0] ... slice.frames[1] - 1), and only the key frames
+    of each slice's `emit` range are evaluated.  Each evaluater batch's metric row stays on the device, tagged with the
+    batch's index in the whole run, instead of being folded at once.  `log()` is then a collective: every rank of `group`
+    calls it, the rows of all ranks are gathered, and the one-process fold runs over them in global batch order on every
+    rank, so every rank returns the one-process log (the same device state, bit for bit).
     """
 
-    def __init__(self, seq, metrics, batch_size, roi=None, max_distance=None, median_scaling=False):
+    def __init__(self, seq, metrics, batch_size, roi=None, max_distance=None, median_scaling=False, group=None, shard=None):
         if isinstance(metrics, (str, bytes)) or not hasattr(metrics, "__iter__"):
             raise ValueError(f"metrics must be a list of metric names or functions, got {metrics!r}")
         self.names = [metric_name(m) for m in metrics]
@@ -84,6 +93,17 @@ class SequenceEvaluater:
         self._state = None         # device float64 [3M+1]: total, valid, running average, num_samples
         self._open = None          # (result, target, mvobj_mask) of the key frames of the open evaluater batch
         self._rings = None         # device [R,1,H,W] targets (and moving-object masks) of the sequence's frames
+        if (group is None) != (shard is None):
+            raise ValueError("SequenceEvaluater: group and shard go together (shard: dist.shard_sequences(...)'s slices)")
+        self.group, self._slices, self._slice = group, None if shard is None else list(shard), 0
+        if self._slices:
+            if self._slices[0].position % self.batch_size:
+                raise ValueError(f"SequenceEvaluater: the shard starts at key frame {self._slices[0].position}, inside an "
+                                 f"evaluater batch of {self.batch_size} (shard_sequences(..., eval_batch={self.batch_size}))")
+            self._check_slice(seq)
+        # sharded: the metric rows of this rank's closed evaluater batches, their sizes and their global batch indices
+        self._rows, self._row_sizes, self._row_index = [], [], []
+        self._batch_index = self._slices[0].position // self.batch_size if self._slices else 0
 
     # ---- the sequence side ---------------------------------------------------------------------------------------------
     def push(self, image, pose, intrinsics, target, mvobj_mask=None):
@@ -120,10 +140,26 @@ class SequenceEvaluater:
         batch carry over.  Returns what the current sequence's flush returns."""
         emitted = self.seq.flush() if self.seq is not None else []
         self._consume(emitted)
+        if self._slices is not None and self.seq is not None:
+            self._slice += 1
         self.seq = seq
+        self._check_slice(seq)
         return emitted
 
+    def _check_slice(self, seq):
+        if seq is None or self._slices is None:
+            return
+        if self._slice >= len(self._slices):
+            raise ValueError(f"SequenceEvaluater: a sequence after the shard's {len(self._slices)} slices")
+        emit = self._slices[self._slice].emit
+        if seq.key_begin > emit[0] or (seq.key_end is not None and seq.key_end < emit[1]):
+            raise ValueError(f"SequenceEvaluater: the sequence runs key frames {seq.key_begin} ... {seq.key_end}, which "
+                             f"do not cover the shard's key frames {emit[0]} ... {emit[1] - 1}")
+
     def _consume(self, emitted):
+        if self._slices is not None:
+            e0, e1 = self._slices[self._slice].emit if self._slice < len(self._slices) else (0, 0)
+            emitted = [(i, o) for i, o in emitted if e0 <= i < e1]
         if not emitted:
             return
         result = torch.cat([o["result"] for _, o in emitted])
@@ -188,11 +224,39 @@ class SequenceEvaluater:
             for key, col in self._specs:
                 cur = M.median_scaling_impl(cur, target)
                 cols.append(run(key, cur)[:, col])
-        M.eval_accumulate_impl(torch.stack(cols, 1), sizes, self._state)
+        if self._slices is None:
+            M.eval_accumulate_impl(torch.stack(cols, 1), sizes, self._state)
+            return
+        self._rows.append(torch.stack(cols, 1).to(torch.float32))
+        self._row_sizes += sizes
+        self._row_index += range(self._batch_index, self._batch_index + len(sizes))
+        self._batch_index += len(sizes)
+
+    def _gathered_state(self):
+        """The one-process device state from every rank's rows: gathered (a collective), put in global batch order and
+        folded by the same accumulator.  Rows travel as float64, which holds their float32 values (NaN and inf included)
+        and the integer tags exactly."""
+        from .dist import all_gather_rows
+        m = len(self.names)
+        dev = self.seq.device if self.seq is not None else (self._rows[0].device if self._rows else
+                                                            torch.device("cuda", torch.cuda.current_device()))
+        rows = torch.cat(self._rows) if self._rows else torch.zeros(0, m, device=dev)
+        tags = torch.tensor([self._row_index, self._row_sizes], dtype=torch.float64).reshape(2, len(self._row_index)).t()
+        rows = all_gather_rows(torch.cat([tags.to(rows.device), rows.to(torch.float64)], 1), self.group)
+        if rows.shape[0] == 0:
+            return None
+        rows = rows[torch.argsort(rows[:, 0])]
+        tags = rows[:, :2].cpu().to(torch.int64)
+        if not torch.equal(tags[:, 0], torch.arange(rows.shape[0])):
+            raise RuntimeError(f"SequenceEvaluater.log: the ranks hold evaluater batches {tags[:, 0].tolist()}, not each of "
+                               f"0 ... {rows.shape[0] - 1} once: the ranks' shards do not tile the run")
+        state = torch.zeros(3 * m + 1, dtype=torch.float64, device=rows.device)
+        return M.eval_accumulate_impl(rows[:, 2:].to(torch.float32), tags[:, 1].tolist(), state)
 
     def log(self):
         m = len(self.names)
-        s = np.zeros(3 * m + 1) if self._state is None else self._state.cpu().numpy()
+        state = self._state if self._slices is None else self._gathered_state()
+        s = np.zeros(3 * m + 1) if state is None else state.cpu().numpy()
         total, valid, avg = s[:m], s[m:2 * m], s[2 * m:3 * m]
         with np.errstate(divide="ignore", invalid="ignore"):
             metrics = (total / valid).tolist()

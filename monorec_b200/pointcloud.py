@@ -119,9 +119,28 @@ class PLYSaver(torch.nn.Module):
                                                      torch.cuda.current_stream(dev).cuda_stream),
                        "mr_pointcloud_add_windows")
 
-    def save(self, file):
-        """Binary little-endian PLY, the reference's header (ply_utils.py:20-32)."""
-        v = self.vertices.detach().to("cpu", torch.float32).contiguous()
+    def gather(self, group=None, dst=0):
+        """Every rank's vertices, in rank order, on rank `dst` of `group` (a torch.distributed process group; a collective:
+        every rank calls it); None on the other ranks.  With ranks holding consecutive key frames (dist.shard_sequences),
+        that is the one-process vertex order."""
+        from .dist import gather_rows
+        v = self.vertices.detach()
+        if not v.is_cuda:                                # nothing added on this rank yet: an empty buffer on its device
+            v = torch.empty(0, 6, device=torch.device("cuda", torch.cuda.current_device()) if self._buf is None
+                            else self._buf.device)
+        return gather_rows(v, dst=dst, group=group)
+
+    def save(self, file, group=None):
+        """Binary little-endian PLY, the reference's header (ply_utils.py:20-32).  With `group`, a collective: rank 0 of the
+        group writes every rank's vertices (`gather`) to its `file`; the other ranks write nothing (their `file` may be
+        None)."""
+        if group is not None:
+            v = self.gather(group)
+            if v is None:
+                return
+        else:
+            v = self.vertices
+        v = v.detach().to("cpu", torch.float32).contiguous()
         header = ("ply\nformat binary_little_endian 1.0\n"
                   f"element vertex {v.shape[0]}\n"
                   "property float x\nproperty float y\nproperty float z\n"
@@ -160,9 +179,15 @@ class SequencePointCloud:
 
     `push(image, pose, intrinsics, rand=None)` and `flush()` forward to the sequence and return what it returns.  `rand`
     [1,H,W] (or [1,1,H,W]): the dropout numbers of this frame's depth map, used if it is added (`add_depthmap`'s `rand`);
-    uniform random numbers when None and `saver.dropout` > 0."""
+    uniform random numbers when None and `saver.dropout` > 0.
 
-    def __init__(self, seq, saver, buffer_length=5, min_hits=1, mask_fill=32, thresh=0.1):
+    The windows stay inside the sequence: a run over several sequences takes one SequencePointCloud per sequence, into one
+    saver.  One rank's share of the export (see dist.shard_sequences(..., buffer_length=...)): `seq` runs a slice of the
+    sequence (MonoRecSequence(first_frame=slice.frames[0], key_end=slice.run[1])), and only the key frames of `emit`
+    (slice.emit, sequence indices [lo, hi)) are added; the slice's other key frames are run for their keep masks only.
+    `saver.save(file, group)` then writes every rank's vertices into rank 0's file."""
+
+    def __init__(self, seq, saver, buffer_length=5, min_hits=1, mask_fill=32, thresh=0.1, emit=None):
         if buffer_length < 1 or not 1 <= min_hits <= buffer_length:
             raise ValueError(f"buffer_length ({buffer_length}) >= 1 and 1 <= min_hits ({min_hits}) <= buffer_length needed")
         if seq.batch_size > 256:
@@ -172,8 +197,13 @@ class SequencePointCloud:
         self.key_index = buffer_length // 2
         # a batch's windows span its own key frames plus buffer_length - 1 earlier ones
         self.ring_len = seq.batch_size + buffer_length - 1
-        self._keep = None          # [ring_len,1,H,W]: keep mask of the key frame run n-th in slot n % ring_len
-        self._n_run = 0            # key frames run so far
+        self._keep = None          # [ring_len,1,H,W]: keep mask of the key frame at position n in slot n % ring_len
+        self.emit = None if emit is None else (int(emit[0]), int(emit[1]))
+        if self.emit is not None and (self.emit[0] < seq.key_begin
+                                      or (seq.key_end is not None and self.emit[1] > seq.key_end)):
+            raise ValueError(f"SequencePointCloud: emit {self.emit} outside the key frames the sequence runs "
+                             f"({seq.key_begin} ... {seq.key_end})")
+        self._n_run = seq.key_begin - seq.first_key    # position in the sequence's key frames of the next key frame run
         self._waiting = None       # (positions, depth, keyframe, intrinsics, pose) of run key frames whose window is open
         self._rand = {}            # sequence index -> dropout numbers of the key frame
 
@@ -211,8 +241,11 @@ class SequencePointCloud:
             fields = [torch.cat([w, f]) for w, f in zip(self._waiting[2], fields)]
         self._n_run += n
         last_ready = self._n_run - 1 - (self.buffer_length - 1 - self.key_index)
-        lo = sum(1 for p in pos if p < self.key_index)             # never added: their window starts before the sequence
-        hi = sum(1 for p in pos if p <= last_ready)
+        e0, e1 = (index[0], index[-1] + 1) if self.emit is None else self.emit
+        # never added: their window starts before the sequence, or they are before the emitted key frames
+        lo = sum(1 for p, i in zip(pos, index) if p < self.key_index or i < e0)
+        hi = sum(1 for p, i in zip(pos, index) if p <= last_ready and i < e1)
+        end = sum(1 for i in index if i < e1)                        # the key frames after `emit` are never added
         if hi > lo:
             if self.saver.dropout > 0:
                 shape = (1, 1) + tuple(fields[0].shape[-2:])
@@ -225,7 +258,7 @@ class SequencePointCloud:
                                             self.min_hits, rand=rand)
         # the rest waits for the next batch (`fields` are torch.cat copies: the next replay does not overwrite them)
         hi = max(hi, lo)
-        self._waiting = (pos[hi:], index[hi:], [f[hi:] for f in fields]) if hi < len(pos) else None
+        self._waiting = (pos[hi:end], index[hi:end], [f[hi:end] for f in fields]) if hi < end else None
         upto = index[hi - 1] if hi > 0 else None
         if upto is not None:
             self._rand = {i: r for i, r in self._rand.items() if i > upto}

@@ -34,13 +34,21 @@ class MonoRecSequence:
     With `graphed`, these are the CUDA graph's static tensors: they stay valid until the next replay, i.e. the next
     `push` that runs a batch.  Clone what must outlive it.
 
+    One slice of the sequence (one rank's share, see dist.shard_sequences): `first_frame` is the sequence index of the first
+    frame pushed, and key frames from `key_begin` = first_frame + max(0, -min(offsets)) on are run (the first key frame
+    whose earlier neighbours are all pushed); `key_end` ends the key frames run (None: the end of the sequence).  Batches
+    are counted from the first key frame run, and the last one before key_end is run at the push that completes it,
+    eagerly when it is short.  The frames to push are first_frame ... key_end - 1 + max(offsets); `push` refuses a frame
+    after those.  Indices (`n_pushed`, the emitted ones) are sequence indices.  The defaults run the whole sequence.
+
     `model` is a MonoRecModel (or any callable that adds its outputs to the reference's data dict and returns that dict,
     as MonoRecModel.forward does); `device` defaults to the
     device of its parameters.  Stereo frames (`use_stereo`) and `pretrain_mode == 3` (moving-object masks) need inputs a
     frame stream does not carry and raise NotImplementedError.
     """
 
-    def __init__(self, model, frame_count=2, dilation=1, batch_size=8, graphed=True, device=None):
+    def __init__(self, model, frame_count=2, dilation=1, batch_size=8, graphed=True, device=None, first_frame=0,
+                 key_end=None):
         if getattr(model, "use_stereo", False):
             raise NotImplementedError("MonoRecSequence: use_stereo needs stereo frames, which a frame stream does not carry")
         if int(getattr(model, "pretrain_mode", 0)) == 3:
@@ -48,6 +56,8 @@ class MonoRecSequence:
                                       "does not carry")
         if batch_size < 1:
             raise ValueError(f"batch_size ({batch_size}) must be >= 1")
+        if first_frame < 0:
+            raise ValueError(f"first_frame ({first_frame}) must be >= 0")
         self.model = model
         self.offsets = neighbour_offsets(frame_count, dilation)
         self.batch_size = int(batch_size)
@@ -55,8 +65,11 @@ class MonoRecSequence:
         self.device = torch.device(device) if device is not None else next(model.parameters()).device
         lo, self._hi = min(0, min(self.offsets)), max(self.offsets)
         self.ring_len = self._hi - lo + 1 + self.batch_size
-        self.n_pushed = 0
-        self._next = -lo                   # the next key frame to run: the first with all its neighbours in the sequence
+        self.first_key = -lo               # the sequence's first key frame with all its neighbours in the sequence
+        self.key_begin = int(first_frame) - lo
+        self.key_end = None if key_end is None else int(key_end)
+        self.n_pushed = int(first_frame)   # sequence index of the next frame pushed
+        self._next = self.key_begin        # the next key frame to run
         self._rings = None                 # (frames [R,3,H,W], poses [R,4,4], intrinsics [R,4,4])
         self._graph = None
         # ring slots of a batch, relative to its first key frame: row 0 the key frames, row 1 + f their f-th source frames
@@ -67,6 +80,9 @@ class MonoRecSequence:
         if image.dim() != 3 or image.shape[0] != 3 or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
             raise ValueError(f"MonoRecSequence.push: image [3,H,W], pose [4,4], intrinsics [4,4] expected, got "
                              f"{tuple(image.shape)}, {tuple(pose.shape)}, {tuple(intrinsics.shape)}")
+        if self.key_end is not None and self.n_pushed >= self.key_end + self._hi:
+            raise ValueError(f"MonoRecSequence.push: frame {self.n_pushed} is past the last frame the key frames before "
+                             f"key_end={self.key_end} need ({self.key_end + self._hi - 1})")
         if self._rings is None:
             R, (_, H, W) = self.ring_len, image.shape
             self._rings = (torch.empty(R, 3, H, W, device=self.device), torch.empty(R, 4, 4, device=self.device),
@@ -78,8 +94,11 @@ class MonoRecSequence:
         for ring, t in zip(self._rings, (image, pose, intrinsics)):
             ring[slot].copy_(t, non_blocking=True)
         self.n_pushed += 1
-        if self._ready() >= self.batch_size:
+        n = self._ready()
+        if n >= self.batch_size:
             return self._run(self.batch_size, self.graphed)
+        if n > 0 and self.key_end is not None and self.n_pushed == self.key_end + self._hi:
+            return self._run(n, False)                             # the short last batch before key_end
         return []
 
     def flush(self):
@@ -88,8 +107,9 @@ class MonoRecSequence:
         return self._run(n, False) if n > 0 else []
 
     def _ready(self):
-        """Key frames not yet run whose neighbours have all been pushed."""
-        return self.n_pushed - self._hi - self._next
+        """Key frames not yet run (before key_end) whose neighbours have all been pushed."""
+        ready = self.n_pushed - self._hi
+        return (ready if self.key_end is None else min(ready, self.key_end)) - self._next
 
     def _assemble(self, idx, out=None):
         """The batch dict, with the reference's keys and list order, gathered from the rings at slots `idx` [1+F, n];
