@@ -30,7 +30,8 @@ class SequenceSlice(NamedTuple):
     position: int                  # place of emit[0] in the concatenated list of emitted key frames of all sequences
 
 
-def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eval_batch=None, buffer_length=None):
+def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eval_batch=None, buffer_length=None,
+                    keys=None):
     """The slices of sequences of `lengths` frames that `rank` of `world` runs, in sequence order (sequences it does not
     touch are left out; a rank may get none).  Exactly one of:
 
@@ -45,7 +46,13 @@ def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eva
 
     Either way, `run` is made of whole model batches of the one-process run: multiples of `batch_size` from the sequence's
     first key frame, and the short last batch at its end, so every key frame's outputs come from the same batch of the same
-    inputs as in one process."""
+    inputs as in one process.
+
+    `keys`: one key-frame list per sequence (MonoRecSequence's `keys`, e.g. sequence.loader_keys with index masks; None in
+    the list, or keys=None, for every key frame with its neighbours).  Everything above is then counted in listed key
+    frames: positions, evaluater batches, model batches and the vote windows' neighbours.  `run` and `emit` stay sequence
+    indices ([first, last + 1) of the listed key frames in them), and `frames` spans the run's neighbours; a rank passes the
+    frames in it that no listed key frame needs with MonoRecSequence.skip."""
     if (eval_batch is None) == (buffer_length is None):
         raise ValueError("shard_sequences: give exactly one of eval_batch and buffer_length")
     if batch_size < 1 or world < 1 or not 0 <= rank < world:
@@ -53,7 +60,15 @@ def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eva
     from .sequence import neighbour_offsets
     offs = neighbour_offsets(frame_count, dilation)
     lo, hi = min(0, min(offs)), max(offs)
-    n_keys = [max(0, int(n) - hi + lo) for n in lengths]      # key frames -lo .. n - hi - 1 of each sequence
+    if keys is not None and len(keys) != len(lengths):
+        raise ValueError(f"shard_sequences: {len(keys)} key lists for {len(lengths)} sequences")
+    # the key frames of each sequence: the listed ones, or -lo .. n - hi - 1
+    K = [list(range(-lo, int(n) - hi)) if keys is None or keys[s] is None else [int(k) for k in keys[s]]
+         for s, n in enumerate(lengths)]
+    for s, (k, n) in enumerate(zip(K, lengths)):
+        if any(b <= a for a, b in zip(k, k[1:])) or (k and (k[0] < -lo or k[-1] >= int(n) - hi)):
+            raise ValueError(f"shard_sequences: the key frames of sequence {s} must be increasing and in [{-lo}, {n - hi})")
+    n_keys = [len(k) for k in K]
     if eval_batch is not None:
         if eval_batch < 1:
             raise ValueError(f"shard_sequences: eval_batch ({eval_batch}) must be >= 1")
@@ -76,7 +91,9 @@ def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eva
         if a < b:
             r0 = (a - before) // batch_size * batch_size
             r1 = min(k, -(-(b + after) // batch_size) * batch_size)
-            out.append(SequenceSlice(s, (r0, r1 - lo + hi), (r0 - lo, r1 - lo), (a - lo, b - lo), offset + a - p0))
+            key = K[s]
+            out.append(SequenceSlice(s, (key[r0] + lo, key[r1 - 1] + hi + 1), (key[r0], key[r1 - 1] + 1),
+                                     (key[a], key[b - 1] + 1), offset + a - p0))
         offset += p1 - p0
     return out
 

@@ -46,14 +46,19 @@ class SequenceEvaluater:
     `metrics`: reference metric names or this package's functions of those names (the 21 sparse and 12 dense / completeness
     metrics of model/metric.py); `roi` [r0, r1, c0, c1], `max_distance` and `median_scaling` are the evaluater's settings.
 
-    `push(image, pose, intrinsics, target, mvobj_mask=None)` forwards the frame to `seq`; `target` [1,H,W] is the frame's
-    inverse-depth ground truth (host or device), copied once into a ring next to the sequence's.  Every batch of key frames
+    `push(image, pose, intrinsics, target, mvobj_mask=None, stereo=None)` forwards the frame to `seq`; `target` [1,H,W] is
+    the frame's inverse-depth ground truth (host or device), which the sequence copies once, for its key frames, into a ring
+    next to its frames and puts into the batch dict as evaluate.py does.  Every batch of key frames
     the sequence emits is cut into evaluater batches in key-frame order, as the loader's DataLoader batches them with
     shuffle=False; a partial batch waits for the next emitted one.  `next_sequence(seq)` runs the rest of the current
     sequence and continues on the next one with the same totals and the same open batch (the loader's batches run across
     the boundary of concatenated sequences); `flush()` runs the rest of the sequence and closes the last partial batch.
     `push`, `flush` and `next_sequence` return what the sequence returns, and never synchronise with the host once the
-    sequence has captured its graph.  `mvobj_mask` [1,H,W] is needed by the `*_sparse_onlydynamic_metric` names only.
+    sequence has captured its graph.  `mvobj_mask` [1,H,W] is needed by the `*_sparse_onlydynamic_metric` names and by a
+    sequence built with `mvobj_masks=True` (a `pretrain_mode == 3` model): one ring in the sequence serves both.  `stereo`
+    (image, pose, intrinsics) is the right-camera frame of a sequence built with `stereo=True`.  A sequence with a key-frame
+    list (`keys`, e.g. `loader_keys(..., index_masks=...)`) is evaluated over its listed key frames, batched as the
+    DataLoader batches the index-masked dataset; `skip()` passes a frame no listed key frame needs (`seq.needs(n)`).
 
     `add(result, target, mvobj_mask=None)` is the part after the model: the batching and accumulation of results already
     computed ([n,1,H,W] each, key frames in order); `seq` may be None when only `add` is used.
@@ -92,7 +97,6 @@ class SequenceEvaluater:
         self._needs_mvobj = any(key[0] == "sparse" and key[2] for key, _ in self._specs)
         self._state = None         # device float64 [3M+1]: total, valid, running average, num_samples
         self._open = None          # (result, target, mvobj_mask) of the key frames of the open evaluater batch
-        self._rings = None         # device [R,1,H,W] targets (and moving-object masks) of the sequence's frames
         if (group is None) != (shard is None):
             raise ValueError("SequenceEvaluater: group and shard go together (shard: dist.shard_sequences(...)'s slices)")
         self.group, self._slices, self._slice = group, None if shard is None else list(shard), 0
@@ -106,7 +110,7 @@ class SequenceEvaluater:
         self._batch_index = self._slices[0].position // self.batch_size if self._slices else 0
 
     # ---- the sequence side ---------------------------------------------------------------------------------------------
-    def push(self, image, pose, intrinsics, target, mvobj_mask=None):
+    def push(self, image, pose, intrinsics, target, mvobj_mask=None, stereo=None):
         if self.seq is None:
             raise ValueError("SequenceEvaluater.push needs a sequence (seq is None)")
         H, W = image.shape[-2:]
@@ -117,15 +121,15 @@ class SequenceEvaluater:
             if t.numel() != H * W or tuple(t.shape[-2:]) != (H, W):
                 raise ValueError(f"SequenceEvaluater.push: target / mvobj_mask [1,H,W] of the image's size {(H, W)} expected, "
                                  f"got {tuple(t.shape)}")
-        R = self.seq.ring_len
-        if self._rings is None or self._rings[0].shape[0] != R or tuple(self._rings[0].shape[2:]) != (H, W):
-            self._rings = [torch.empty(R, 1, H, W, device=self.seq.device) for _ in maps]
-        slot = self.seq.n_pushed % R
-        for ring, t in zip(self._rings, maps):
-            ring[slot].copy_(t.reshape(1, H, W), non_blocking=True)
-        emitted = self.seq.push(image, pose, intrinsics)
+        keep_mask = self._needs_mvobj or self.seq.mvobj_masks
+        emitted = self.seq.push(image, pose, intrinsics, stereo=stereo, mvobj_mask=mvobj_mask if keep_mask else None,
+                                target=target)
         self._consume(emitted)
         return emitted
+
+    def skip(self):
+        """Passes a frame that no key frame of the sequence needs, without reading it (`MonoRecSequence.skip`)."""
+        self.seq.skip()
 
     def flush(self):
         emitted = self.seq.flush() if self.seq is not None else []
@@ -162,12 +166,9 @@ class SequenceEvaluater:
             emitted = [(i, o) for i, o in emitted if e0 <= i < e1]
         if not emitted:
             return
-        result = torch.cat([o["result"] for _, o in emitted])
-        R, n = self._rings[0].shape[0], len(emitted)
-        first = emitted[0][0] % R                                 # the key frames' slots: at most two contiguous runs
-        k = min(n, R - first)
-        maps = [torch.cat([ring[first:first + k], ring[:n - k]]) for ring in self._rings]
-        self.add(result, *maps)
+        # the key frames' results and the targets (and masks) the sequence gathered into their batch
+        keys = ("result", "target") + (("mvobj_mask",) if self._needs_mvobj else ())
+        self.add(*[torch.cat([o[k] for _, o in emitted]) for k in keys])
 
     # ---- batching and accumulation ---------------------------------------------------------------------------------------
     def add(self, result, target, mvobj_mask=None):

@@ -177,9 +177,12 @@ class SequencePointCloud:
     size 1.  The windows cross batch boundaries: this keeps its own ring of keep masks, and the last buffer_length // 2
     key frames of a batch wait for the next one.  One `mr_pointcloud_add_windows` call per batch.
 
-    `push(image, pose, intrinsics, rand=None)` and `flush()` forward to the sequence and return what it returns.  `rand`
-    [1,H,W] (or [1,1,H,W]): the dropout numbers of this frame's depth map, used if it is added (`add_depthmap`'s `rand`);
-    uniform random numbers when None and `saver.dropout` > 0.
+    `push(image, pose, intrinsics, rand=None, stereo=None, mvobj_mask=None)`, `skip()` and `flush()` forward to the sequence
+    and return what it returns.  `rand` [1,H,W] (or [1,1,H,W]): the dropout numbers of this frame's depth map, used if it is
+    added (`add_depthmap`'s `rand`); uniform random numbers when None and `saver.dropout` > 0.
+
+    With a key-frame list (`MonoRecSequence(keys=...)`, the loader's index masks), the windows run over consecutive listed
+    key frames, as create_pointcloud.py's loop iterates the index-masked dataset.
 
     The windows stay inside the sequence: a run over several sequences takes one SequencePointCloud per sequence, into one
     saver.  One rank's share of the export (see dist.shard_sequences(..., buffer_length=...)): `seq` runs a slice of the
@@ -203,16 +206,20 @@ class SequencePointCloud:
                                       or (seq.key_end is not None and self.emit[1] > seq.key_end)):
             raise ValueError(f"SequencePointCloud: emit {self.emit} outside the key frames the sequence runs "
                              f"({seq.key_begin} ... {seq.key_end})")
-        self._n_run = seq.key_begin - seq.first_key    # position in the sequence's key frames of the next key frame run
+        self._n_run = seq.key_position                 # position in the sequence's key frames of the next key frame run
         self._waiting = None       # (positions, depth, keyframe, intrinsics, pose) of run key frames whose window is open
         self._rand = {}            # sequence index -> dropout numbers of the key frame
 
-    def push(self, image, pose, intrinsics, rand=None):
-        if rand is not None:
+    def push(self, image, pose, intrinsics, rand=None, stereo=None, mvobj_mask=None):
+        if rand is not None and self.seq.runs(self.seq.n_pushed):
             self._rand[self.seq.n_pushed] = rand.to(self.seq.device, torch.float32).reshape(1, 1, *rand.shape[-2:])
-        emitted = self.seq.push(image, pose, intrinsics)
+        emitted = self.seq.push(image, pose, intrinsics, stereo=stereo, mvobj_mask=mvobj_mask)
         self._add(emitted)
         return emitted
+
+    def skip(self):
+        """Passes a frame that no key frame of the sequence needs, without reading it (`MonoRecSequence.skip`)."""
+        self.seq.skip()
 
     def flush(self):
         emitted = self.seq.flush()

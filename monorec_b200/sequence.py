@@ -5,7 +5,13 @@ own copies of the neighbour frames, and create_pointcloud.py runs them at batch 
 one at a time instead: each is copied to the device once, into a ring of frames, poses and intrinsics, and every
 `batch_size` ready key frames are gathered from the ring into one batch dict and run together, by CUDA-graph replay when
 `graphed`.
+
+The reference's KITTI loader can also select the key frames (`use_index_mask`; `loader_keys` restates its list), add the
+right camera's frame (`return_stereo`) and a moving-object mask (`return_mvobj_mask`) to every key frame's dict; the
+sequence takes those as `keys=`, `stereo=True` and `mvobj_masks=True`.
 """
+import bisect
+
 import torch
 
 from .model import GraphedMonoRec
@@ -17,6 +23,25 @@ def neighbour_offsets(frame_count, dilation=1):
     if frame_count < 1 or dilation < 1:
         raise ValueError(f"frame_count ({frame_count}) and dilation ({dilation}) must be >= 1")
     return [i for i in range(-(frame_count // 2) * dilation, ((frame_count + 1) // 2) * dilation + 1, dilation) if i != 0]
+
+
+def loader_keys(length, frame_count=2, dilation=1, lidar_depth=False, annotated_lidar=True, index_masks=None):
+    """The sequence indices (`image_id`) of the loader's key frames of one sequence of `length` frames, in order
+    (kitti_odometry_dataset.py:54-76, 216-219).
+
+    The loader's range is [offset, length + offset - extra_frames) with offset = (frame_count // 2) * dilation and
+    extra_frames = frame_count * dilation, raised to at least 5 and 10 when `lidar_depth` and `annotated_lidar` (the
+    annotated depth maps of eval_monorec.json).  `index_masks`: the loaded JSON dicts of `use_index_mask` (str(index) ->
+    bool); a key frame stays only if every mask lists it as true.  None and () give the same list, as in the loader."""
+    if frame_count < 1 or dilation < 1:
+        raise ValueError(f"frame_count ({frame_count}) and dilation ({dilation}) must be >= 1")
+    offset, extra = (frame_count // 2) * dilation, frame_count * dilation
+    if annotated_lidar and lidar_depth:
+        offset, extra = max(offset, 5), max(extra, 10)
+    keys = range(offset, int(length) + offset - extra)
+    for m in index_masks or ():
+        keys = [k for k in keys if m.get(str(k))]
+    return list(keys)
 
 
 class MonoRecSequence:
@@ -41,19 +66,37 @@ class MonoRecSequence:
     eagerly when it is short.  The frames to push are first_frame ... key_end - 1 + max(offsets); `push` refuses a frame
     after those.  Indices (`n_pushed`, the emitted ones) are sequence indices.  The defaults run the whole sequence.
 
+    `keys`: a sorted list of the sequence indices of the key frames to run (`loader_keys`: the loader's index-masked or
+    annotated-lidar list) instead of every key frame with its neighbours.  Batches are `batch_size` consecutive listed key
+    frames, counted from the first listed key frame run, and the short last batch runs at the push that completes the last
+    listed key frame.  Only the frames a listed key frame needs (`needs(n)`) are copied; `push` accepts the others and
+    copies nothing, and `skip()` passes one without its image, so the caller need not read it.  The ring then holds
+    batch_size * (frame_count + 1) + the neighbour span frames, however far apart the listed key frames are.  With
+    `first_frame` / `key_end`, the listed key frames in [key_begin, key_end) are run.
+
+    `stereo=True`: `push(..., stereo=(image, pose, intrinsics))` takes the frame's right-camera image [3,H,W], pose (the
+    left pose @ the baseline transform) and intrinsics, and the batch dict holds them as `stereoframe`, `stereoframe_pose`,
+    `stereoframe_intrinsics` (kitti_odometry_dataset.py:271-278), as a `use_stereo` model needs.  `mvobj_masks=True`:
+    `push(..., mvobj_mask=[1,H,W])`, and the batch dict holds `mvobj_mask` [B,1,H,W] (:280-282), as `pretrain_mode == 3`
+    needs.  `push(..., target=[1,H,W])` puts the frame's ground truth into the batch dict as `target`, as evaluate.py does
+    (SequenceEvaluater uses it); a mask or target given at the first push that copies a frame is then needed for every key
+    frame.  These are copied for the key frames only, into rings next to the frames', gathered with them into the batch
+    (the CUDA graph's static inputs) and returned in each key frame's outputs.
+
     `model` is a MonoRecModel (or any callable that adds its outputs to the reference's data dict and returns that dict,
-    as MonoRecModel.forward does); `device` defaults to the
-    device of its parameters.  Stereo frames (`use_stereo`) and `pretrain_mode == 3` (moving-object masks) need inputs a
-    frame stream does not carry and raise NotImplementedError.
+    as MonoRecModel.forward does); `device` defaults to the device of its parameters.  A `use_stereo` model without
+    `stereo=True`, and `pretrain_mode == 3` without `mvobj_masks=True`, raise NotImplementedError: a plain frame stream
+    does not carry their inputs.
     """
 
     def __init__(self, model, frame_count=2, dilation=1, batch_size=8, graphed=True, device=None, first_frame=0,
-                 key_end=None):
-        if getattr(model, "use_stereo", False):
-            raise NotImplementedError("MonoRecSequence: use_stereo needs stereo frames, which a frame stream does not carry")
-        if int(getattr(model, "pretrain_mode", 0)) == 3:
-            raise NotImplementedError("MonoRecSequence: pretrain_mode 3 needs moving-object masks, which a frame stream "
-                                      "does not carry")
+                 key_end=None, keys=None, stereo=False, mvobj_masks=False):
+        if getattr(model, "use_stereo", False) and not stereo:
+            raise NotImplementedError("MonoRecSequence: use_stereo needs stereo frames: MonoRecSequence(stereo=True) and "
+                                      "push(..., stereo=(image, pose, intrinsics))")
+        if int(getattr(model, "pretrain_mode", 0)) == 3 and not mvobj_masks:
+            raise NotImplementedError("MonoRecSequence: pretrain_mode 3 needs moving-object masks: "
+                                      "MonoRecSequence(mvobj_masks=True) and push(..., mvobj_mask=...)")
         if batch_size < 1:
             raise ValueError(f"batch_size ({batch_size}) must be >= 1")
         if first_frame < 0:
@@ -62,43 +105,103 @@ class MonoRecSequence:
         self.offsets = neighbour_offsets(frame_count, dilation)
         self.batch_size = int(batch_size)
         self.graphed = bool(graphed)
+        self.stereo, self.mvobj_masks = bool(stereo), bool(mvobj_masks)
         self.device = torch.device(device) if device is not None else next(model.parameters()).device
         lo, self._hi = min(0, min(self.offsets)), max(self.offsets)
-        self.ring_len = self._hi - lo + 1 + self.batch_size
         self.first_key = -lo               # the sequence's first key frame with all its neighbours in the sequence
         self.key_begin = int(first_frame) - lo
         self.key_end = None if key_end is None else int(key_end)
         self.n_pushed = int(first_frame)   # sequence index of the next frame pushed
-        self._next = self.key_begin        # the next key frame to run
         self._rings = None                 # (frames [R,3,H,W], poses [R,4,4], intrinsics [R,4,4])
+        self._maps = None                  # key-frame inputs beside the frames: batch-dict key -> ring [R,...]
         self._graph = None
-        # ring slots of a batch, relative to its first key frame: row 0 the key frames, row 1 + f their f-th source frames
-        rel = torch.tensor([0] + self.offsets).view(-1, 1) + torch.arange(self.batch_size).view(1, -1)
-        self._rel = rel.to(self.device)
+        self._uses = [0] + self.offsets    # a key frame's own frame, then its source frames
+        if keys is None:
+            self.keys = None
+            self.ring_len = self._hi - lo + 1 + self.batch_size
+            self.key_position = self.key_begin - self.first_key
+            self._next = self.key_begin    # the next key frame to run
+            # ring slots of a batch, relative to its first key frame: row 0 the key frames, row 1 + f their f-th sources
+            rel = torch.tensor(self._uses).view(-1, 1) + torch.arange(self.batch_size).view(1, -1)
+            self._rel = rel.to(self.device)
+            return
+        self.keys = [int(k) for k in keys]
+        if any(b <= a for a, b in zip(self.keys, self.keys[1:])) or (self.keys and self.keys[0] < self.first_key):
+            raise ValueError(f"MonoRecSequence: keys must be increasing sequence indices >= {self.first_key} (the first "
+                             f"key frame with all its neighbours)")
+        self.ring_len = self.batch_size * len(self._uses) + self._hi - lo
+        self.key_position = bisect.bisect_left(self.keys, self.key_begin)   # place of the first key frame run in `keys`
+        end = len(self.keys) if self.key_end is None else bisect.bisect_left(self.keys, self.key_end)
+        self._run_keys = self.keys[self.key_position:end]
+        self._run_set = set(self._run_keys)
+        self._next = 0                     # the next key frame to run: its place in _run_keys
+        self._slot = {}                    # sequence index of a copied frame -> (ring slot, last key frame that uses it)
+        self._free = list(range(self.ring_len))[::-1]
 
-    def push(self, image, pose, intrinsics):
+    def needs(self, n):
+        """Whether `push` copies frame n: it is a key frame this sequence runs or a neighbour of one."""
+        if self.keys is None:
+            return self.key_end is None or n < self.key_end + self._hi
+        return any(n - u in self._run_set for u in self._uses)
+
+    def runs(self, n):
+        """Whether key frame n is one this sequence runs (for keys=None: any frame in [key_begin, key_end))."""
+        if self.keys is None:
+            return n >= self.key_begin and (self.key_end is None or n < self.key_end)
+        return n in self._run_set
+
+    def skip(self):
+        """Passes the next frame without its data; only a frame that no key frame run needs (`needs`) can be skipped."""
+        if self.needs(self.n_pushed):
+            raise ValueError(f"MonoRecSequence.skip: frame {self.n_pushed} is needed by a key frame the sequence runs")
+        self.n_pushed += 1
+
+    def push(self, image, pose, intrinsics, stereo=None, mvobj_mask=None, target=None):
         if image.dim() != 3 or image.shape[0] != 3 or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
             raise ValueError(f"MonoRecSequence.push: image [3,H,W], pose [4,4], intrinsics [4,4] expected, got "
                              f"{tuple(image.shape)}, {tuple(pose.shape)}, {tuple(intrinsics.shape)}")
         if self.key_end is not None and self.n_pushed >= self.key_end + self._hi:
             raise ValueError(f"MonoRecSequence.push: frame {self.n_pushed} is past the last frame the key frames before "
                              f"key_end={self.key_end} need ({self.key_end + self._hi - 1})")
+        if stereo is not None and not self.stereo:
+            raise ValueError("MonoRecSequence.push: stereo frames need MonoRecSequence(stereo=True)")
+        n = self.n_pushed
+        if not self.needs(n):
+            self.n_pushed += 1
+            return []
+        H, W = image.shape[1:]
+        maps = self._key_inputs(H, W, stereo, mvobj_mask, target)
         if self._rings is None:
-            R, (_, H, W) = self.ring_len, image.shape
+            R = self.ring_len
             self._rings = (torch.empty(R, 3, H, W, device=self.device), torch.empty(R, 4, 4, device=self.device),
                            torch.empty(R, 4, 4, device=self.device))
+            # the key-frame inputs the sequence is built for, and the optional ones this first push gives
+            shapes = {}
+            if self.stereo:
+                shapes.update(stereoframe=(3, H, W), stereoframe_pose=(4, 4), stereoframe_intrinsics=(4, 4))
+            if self.mvobj_masks or "mvobj_mask" in maps:
+                shapes["mvobj_mask"] = (1, H, W)
+            if "target" in maps:
+                shapes["target"] = (1, H, W)
+            self._maps = {k: torch.empty((R,) + v, device=self.device) for k, v in shapes.items()}
         elif image.shape[1:] != self._rings[0].shape[2:]:
             raise ValueError(f"MonoRecSequence.push: frame size {tuple(image.shape[1:])} differs from the sequence's "
                              f"{tuple(self._rings[0].shape[2:])}")
-        slot = self.n_pushed % self.ring_len
+        slot = self._store(n)
         for ring, t in zip(self._rings, (image, pose, intrinsics)):
             ring[slot].copy_(t, non_blocking=True)
+        if self.runs(n):
+            if set(maps) != set(self._maps):
+                raise ValueError(f"MonoRecSequence.push: key frame {n} comes with {sorted(maps)}, the sequence's key frames "
+                                 f"with {sorted(self._maps)}")
+            for k, t in maps.items():
+                self._maps[k][slot].copy_(t, non_blocking=True)
         self.n_pushed += 1
         n = self._ready()
         if n >= self.batch_size:
             return self._run(self.batch_size, self.graphed)
-        if n > 0 and self.key_end is not None and self.n_pushed == self.key_end + self._hi:
-            return self._run(n, False)                             # the short last batch before key_end
+        if n > 0 and n == self._remaining():
+            return self._run(n, False)                             # the short last batch before key_end / of `keys`
         return []
 
     def flush(self):
@@ -106,10 +209,48 @@ class MonoRecSequence:
         n = self._ready()
         return self._run(n, False) if n > 0 else []
 
+    def _key_inputs(self, H, W, stereo, mvobj_mask, target):
+        """The key-frame inputs given to this push, shaped as one row of their rings."""
+        maps = {}
+        if self.stereo and stereo is not None:
+            image, pose, intrinsics = stereo
+            if tuple(image.shape) != (3, H, W) or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
+                raise ValueError(f"MonoRecSequence.push: stereo image [3,{H},{W}], pose [4,4], intrinsics [4,4] expected, "
+                                 f"got {tuple(image.shape)}, {tuple(pose.shape)}, {tuple(intrinsics.shape)}")
+            maps.update(stereoframe=image, stereoframe_pose=pose, stereoframe_intrinsics=intrinsics)
+        for key, t in (("mvobj_mask", mvobj_mask), ("target", target)):
+            if t is not None:
+                if t.numel() != H * W or tuple(t.shape[-2:]) != (H, W):
+                    raise ValueError(f"MonoRecSequence.push: {key} [1,H,W] of the image's size {(H, W)} expected, got "
+                                     f"{tuple(t.shape)}")
+                maps[key] = t.reshape(1, H, W)
+        if (self.stereo and stereo is None) or (self.mvobj_masks and mvobj_mask is None):
+            if self.runs(self.n_pushed):
+                raise ValueError(f"MonoRecSequence.push: key frame {self.n_pushed} needs "
+                                 f"{'stereo=(image, pose, intrinsics)' if self.stereo and stereo is None else 'mvobj_mask'}")
+        return maps
+
+    def _store(self, n):
+        """The ring slot of frame n."""
+        if self.keys is None:
+            return n % self.ring_len
+        if not self._free:
+            raise RuntimeError("MonoRecSequence: the frame ring is full (a bookkeeping error)")
+        self._slot[n] = (self._free.pop(), max(n - u for u in self._uses if n - u in self._run_set))
+        return self._slot[n][0]
+
     def _ready(self):
         """Key frames not yet run (before key_end) whose neighbours have all been pushed."""
         ready = self.n_pushed - self._hi
+        if self.keys is not None:
+            return bisect.bisect_left(self._run_keys, ready) - self._next
         return (ready if self.key_end is None else min(ready, self.key_end)) - self._next
+
+    def _remaining(self):
+        """Key frames left to run, when the sequence knows where they end."""
+        if self.keys is not None:
+            return len(self._run_keys) - self._next
+        return None if self.key_end is None else self.key_end - self._next
 
     def _assemble(self, idx, out=None):
         """The batch dict, with the reference's keys and list order, gathered from the rings at slots `idx` [1+F, n];
@@ -121,11 +262,19 @@ class MonoRecSequence:
         for key, ring in (("frames", frames), ("poses", poses), ("intrinsics", intrinsics)):
             data[key] = [torch.index_select(ring, 0, idx[1 + f], out=None if out is None else out[key][f])
                          for f in range(len(self.offsets))]
+        for key, ring in self._maps.items():
+            data[key] = torch.index_select(ring, 0, idx[0], out=None if out is None else out[key])
         return data
 
     def _run(self, n, graphed):
-        i0 = self._next
-        idx = torch.remainder(self._rel[:, :n] + i0, self.ring_len)
+        if self.keys is None:
+            index = list(range(self._next, self._next + n))
+            idx = torch.remainder(self._rel[:, :n] + self._next, self.ring_len)
+        else:
+            index = self._run_keys[self._next:self._next + n]
+            idx = torch.tensor([[self._slot[k + u][0] for k in index] for u in self._uses], dtype=torch.int64)
+            # a pinned copy does not synchronise; the host allocator keeps the block until the copy is done
+            idx = idx.pin_memory().to(self.device, non_blocking=True) if self.device.type == "cuda" else idx
         if not graphed:
             out = self.model(self._assemble(idx))
         elif self._graph is None:
@@ -135,10 +284,14 @@ class MonoRecSequence:
             self._assemble(idx, out=self._graph.static_in)
             out = self._graph.replay()
         self._next += n
-        return [(i0 + j, _row(out, j)) for j in range(n)]
+        if self.keys is not None:
+            # frames no later key frame uses go back to the free slots (their next writes follow this batch's gathers)
+            for f in [f for f, (_, last) in self._slot.items() if last <= index[-1]]:
+                self._free.append(self._slot.pop(f)[0])
+        return [(i, _row(out, j)) for j, i in enumerate(index)]
 
-
-_ROW_KEYS = ("result", "cv_mask", "cost_volume", "keyframe", "keyframe_pose", "keyframe_intrinsics")
+_ROW_KEYS = ("result", "cv_mask", "cost_volume", "keyframe", "keyframe_pose", "keyframe_intrinsics", "stereoframe",
+             "stereoframe_pose", "stereoframe_intrinsics", "mvobj_mask", "target")
 
 
 def _row(out, j):
