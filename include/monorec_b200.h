@@ -382,9 +382,12 @@ int mr_eval_accumulate(const float* values, int G, int M, const int* group_sizes
  *     n_masks - min_hits of them are 1 (create_pointcloud.py:93-95); n_masks = 0: no vote;
  *   min_d / max_d: distance range; roi: host int[4] {r0, r1, c0, c1} or NULL; dropout_rand: [B,1,H,W] uniform numbers (a
  *     vertex is kept iff rand > dropout; torch.rand_like in the reference) or NULL;
- *   vertices: device float [capacity][6]; n_before: vertices already stored; n_after: DEVICE long long, the new count, or
- *     minus the needed count if the buffer is too small (then nothing is written);
- *   workspace: device buffer of mr_pointcloud_workspace(B,H,W) bytes. */
+ *   vertices: device float [capacity][6]; n_before: vertices already stored, or any negative value to take the position
+ *     from *n_after as the previous call on the stream left it (the running count stays on the device: the caller needs
+ *     no read-back per call, only a capacity that bounds the count); n_after: DEVICE long long, the new count, or minus the
+ *     needed count if the buffer is too small (then nothing is written; with n_before < 0 a negative count stays negative
+ *     and later calls write nothing);
+ *   workspace: 8-byte aligned device buffer of mr_pointcloud_workspace(B,H,W) bytes. */
 int mr_pointcloud_keep_mask(const float* cv_mask, float* keep, int B, int H, int W, int mask_fill, float thresh, void* stream);
 long long mr_pointcloud_workspace(int B, int H, int W);
 int mr_pointcloud_add(const float* inv_depth, const float* keyframe, const float* K, const float* pose,

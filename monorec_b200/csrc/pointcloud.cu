@@ -77,7 +77,7 @@ struct PcArgs {
     int* counts;              // [B * blocks_per_image] kept vertices per block, then exclusive offsets (in place)
     float* out;               // [capacity][6]
     long long capacity;
-    long long base;           // vertices already in the buffer
+    long long* base;          // device: the buffer position of this call's first vertex (set by pc_scan_kernel)
     long long* total;         // device: number of vertices in the buffer after this call
 };
 
@@ -108,8 +108,11 @@ __global__ void pc_count_kernel(const __grid_constant__ PcArgs<Vote> a) {
     if (threadIdx.x == 0) a.counts[b * gridDim.x + blockIdx.x] = n;
 }
 
-// exclusive scan of the per-block counts (a few thousand entries: one block, sequential chunks per thread + block scan)
-__global__ void pc_scan_kernel(int* counts, int n, long long base, long long capacity, long long* total) {
+// exclusive scan of the per-block counts (a few thousand entries: one block, sequential chunks per thread + block scan).
+// The batch's position is n_before, or (n_before < 0) the count *total left by the previous call on the stream; a negative
+// count (an earlier call overflowed) stays negative and grows by this batch, so nothing more is written.
+__global__ void pc_scan_kernel(int* counts, int n, long long n_before, long long capacity, long long* base_out,
+                               long long* total) {
     __shared__ long long part[1024];
     const int t = threadIdx.x, per = (n + blockDim.x - 1) / blockDim.x;
     const int lo = min(t * per, n), hi = min(lo + per, n);
@@ -120,7 +123,10 @@ __global__ void pc_scan_kernel(int* counts, int n, long long base, long long cap
     if (t == 0) {
         long long run = 0;
         for (int k = 0; k < (int)blockDim.x; ++k) { const long long v = part[k]; part[k] = run; run += v; }
-        *total = (base + run <= capacity) ? base + run : -(base + run);    // negative: the buffer is too small (nothing is written)
+        const long long base = n_before >= 0 ? n_before : *total;
+        *base_out = base;
+        if (base < 0) *total = base - run;
+        else *total = (base + run <= capacity) ? base + run : -(base + run);   // negative: the buffer is too small (nothing is written)
     }
     __syncthreads();
     long long run = part[t];
@@ -171,7 +177,7 @@ __global__ void pc_write_kernel(const __grid_constant__ PcArgs<Vote> a) {
     if (!ok) return;
     int rank = __popc(bal & ((1u << lane) - 1));
     for (int w = 0; w < warp; ++w) rank += wsum[w];
-    const long long at = a.base + a.counts[b * gridDim.x + blockIdx.x] + rank;
+    const long long at = *a.base + a.counts[b * gridDim.x + blockIdx.x] + rank;
     const int y = i / a.W, x = i - y * a.W;
     const float fx = (float)x, fy = (float)y;
     // Backprojection (layers.py:56-58): inv(K)[:3,:3] . (x, y, 1) * depth; then pose . (X, 1)   (ply_utils.py:47-49)
@@ -201,9 +207,10 @@ extern "C" int mr_pointcloud_keep_mask(const float* cv_mask, float* keep, int B,
     return MR_OK;
 }
 
+// workspace: the batch's buffer position (one long long), then the per-block counts
 extern "C" long long mr_pointcloud_workspace(int B, int H, int W) {
     if (B < 1 || H < 1 || W < 1) return 0;
-    return (long long)B * ((H * W + kBlk - 1) / kBlk) * (long long)sizeof(int);
+    return (long long)sizeof(long long) + (long long)B * ((H * W + kBlk - 1) / kBlk) * (long long)sizeof(int);
 }
 
 namespace {
@@ -220,12 +227,13 @@ int add_vertices(PcArgs<Vote>& a, const float* inv_depth, const float* keyframe,
     a.B = B; a.H = H; a.W = W;
     a.use_roi = roi != nullptr;
     if (roi) { a.r0 = roi[0]; a.r1 = roi[1]; a.c0 = roi[2]; a.c1 = roi[3]; }
-    a.counts = static_cast<int*>(workspace);
-    a.out = vertices; a.capacity = capacity; a.base = n_before; a.total = n_after;
+    a.base = static_cast<long long*>(workspace);
+    a.counts = reinterpret_cast<int*>(a.base + 1);
+    a.out = vertices; a.capacity = capacity; a.total = n_after;
     const int nb = (H * W + kBlk - 1) / kBlk;
     pc_count_kernel<<<dim3(nb, B), kBlk, 0, st>>>(a);
     MR_LAUNCH_CHECK("pc_count_kernel");
-    pc_scan_kernel<<<1, 1024, 0, st>>>(a.counts, nb * B, n_before, capacity, n_after);
+    pc_scan_kernel<<<1, 1024, 0, st>>>(a.counts, nb * B, n_before, capacity, a.base, n_after);
     MR_LAUNCH_CHECK("pc_scan_kernel");
     pc_write_kernel<<<dim3(nb, B), kBlk, 0, st>>>(a);
     MR_LAUNCH_CHECK("pc_write_kernel");
@@ -242,7 +250,7 @@ extern "C" int mr_pointcloud_add(const float* inv_depth, const float* keyframe, 
     MR_REQUIRE(inv_depth && keyframe && K && pose && vertices && n_after && workspace, "mr_pointcloud_add: null pointer");
     MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1 && n_masks >= 0 && n_masks <= 16 && (n_masks == 0 || keep_masks != nullptr),
                "mr_pointcloud_add: bad shape or more than 16 masks");
-    MR_REQUIRE(capacity >= 0 && n_before >= 0 && n_before <= capacity, "mr_pointcloud_add: bad buffer position");
+    MR_REQUIRE(capacity >= 0 && n_before <= capacity, "mr_pointcloud_add: bad buffer position");
     if (workspace_bytes < mr_pointcloud_workspace(B, H, W)) {
         mr::set_error("mr_pointcloud_add: workspace too small (%lld < %lld bytes)", workspace_bytes, mr_pointcloud_workspace(B, H, W));
         return MR_ENOMEM;
@@ -282,7 +290,7 @@ extern "C" int mr_pointcloud_add_windows(const float* inv_depth, const float* ke
     for (int b = 0; b < B; ++b)
         MR_REQUIRE(window_start[b] >= 0 && window_start[b] < ring_len,
                    "mr_pointcloud_add_windows: window_start[%d] = %d outside the ring [0, %d)", b, window_start[b], ring_len);
-    MR_REQUIRE(capacity >= 0 && n_before >= 0 && n_before <= capacity,
+    MR_REQUIRE(capacity >= 0 && n_before <= capacity,
                "mr_pointcloud_add_windows: bad buffer position n_before = %lld, capacity = %lld", n_before, capacity);
     if (workspace_bytes < mr_pointcloud_workspace(B, H, W)) {
         mr::set_error("mr_pointcloud_add_windows: workspace too small (%lld < %lld bytes)", workspace_bytes,

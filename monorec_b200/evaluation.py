@@ -75,6 +75,9 @@ class SequenceEvaluater:
     batch's index in the whole run, instead of being folded at once.  `log()` is then a collective: every rank of `group`
     calls it, the rows of all ranks are gathered, and the one-process fold runs over them in global batch order on every
     rank, so every rank returns the one-process log (the same device state, bit for bit).
+
+    `group=LANE` makes the evaluater one lane of a one-process run over several devices (lanes.MultiDeviceEvaluater): it
+    keeps its shard's rows the same way, and its driver collects them (`tagged_rows`) and runs the same fold.
     """
 
     def __init__(self, seq, metrics, batch_size, roi=None, max_distance=None, median_scaling=False, group=None, shard=None):
@@ -233,33 +236,56 @@ class SequenceEvaluater:
         self._row_index += range(self._batch_index, self._batch_index + len(sizes))
         self._batch_index += len(sizes)
 
-    def _gathered_state(self):
-        """The one-process device state from every rank's rows: gathered (a collective), put in global batch order and
-        folded by the same accumulator.  Rows travel as float64, which holds their float32 values (NaN and inf included)
-        and the integer tags exactly."""
-        from .dist import all_gather_rows
+    def tagged_rows(self, device=None):
+        """A sharded evaluater's closed evaluater batches as float64 rows [G, 2 + M] on `device` (default: where they are):
+        global batch index, batch size, then the metric row.  Float64 holds the float32 values (NaN and inf included) and
+        the integer tags exactly."""
         m = len(self.names)
-        dev = self.seq.device if self.seq is not None else (self._rows[0].device if self._rows else
-                                                            torch.device("cuda", torch.cuda.current_device()))
-        rows = torch.cat(self._rows) if self._rows else torch.zeros(0, m, device=dev)
+        dev = device if device is not None else self.seq.device if self.seq is not None else (
+            self._rows[0].device if self._rows else torch.device("cuda", torch.cuda.current_device()))
+        rows = torch.cat(self._rows).to(dev) if self._rows else torch.zeros(0, m, device=dev)
         tags = torch.tensor([self._row_index, self._row_sizes], dtype=torch.float64).reshape(2, len(self._row_index)).t()
-        rows = all_gather_rows(torch.cat([tags.to(rows.device), rows.to(torch.float64)], 1), self.group)
-        if rows.shape[0] == 0:
-            return None
-        rows = rows[torch.argsort(rows[:, 0])]
-        tags = rows[:, :2].cpu().to(torch.int64)
-        if not torch.equal(tags[:, 0], torch.arange(rows.shape[0])):
-            raise RuntimeError(f"SequenceEvaluater.log: the ranks hold evaluater batches {tags[:, 0].tolist()}, not each of "
-                               f"0 ... {rows.shape[0] - 1} once: the ranks' shards do not tile the run")
-        state = torch.zeros(3 * m + 1, dtype=torch.float64, device=rows.device)
-        return M.eval_accumulate_impl(rows[:, 2:].to(torch.float32), tags[:, 1].tolist(), state)
+        return torch.cat([tags.to(dev), rows.to(torch.float64)], 1)
 
     def log(self):
-        m = len(self.names)
-        state = self._state if self._slices is None else self._gathered_state()
-        s = np.zeros(3 * m + 1) if state is None else state.cpu().numpy()
-        total, valid, avg = s[:m], s[m:2 * m], s[2 * m:3 * m]
-        with np.errstate(divide="ignore", invalid="ignore"):
-            metrics = (total / valid).tolist()
-        return {"loss": 0.0, "metrics": metrics, "metrics_correct": avg.tolist(), "valid_batches": valid[0],
-                "loss_loss": 0.0}
+        if self.group is LANE:
+            raise ValueError("SequenceEvaluater.log: a lane's rows are folded by its driver (MultiDeviceEvaluater.log)")
+        if self._slices is None:
+            return log_dict(self._state, len(self.names))
+        from .dist import all_gather_rows
+        return log_dict(fold_rows(all_gather_rows(self.tagged_rows(), self.group), len(self.names)), len(self.names))
+
+
+LANE = "lane"
+"""SequenceEvaluater(group=LANE, shard=...): a lane of lanes.MultiDeviceEvaluater, whose rows its driver folds."""
+
+
+def sort_rows(rows):
+    """Tagged rows of every shard of a run (`SequenceEvaluater.tagged_rows`, in any order) in global batch order, checked to
+    hold each evaluater batch 0 ... G-1 once: (rows, tags [G,2] int64 on the host)."""
+    rows = rows[torch.argsort(rows[:, 0])]
+    tags = rows[:, :2].cpu().to(torch.int64)
+    if not torch.equal(tags[:, 0], torch.arange(rows.shape[0])):
+        raise RuntimeError(f"SequenceEvaluater.log: the shards hold evaluater batches {tags[:, 0].tolist()}, not each of "
+                           f"0 ... {rows.shape[0] - 1} once: the shards do not tile the run")
+    return rows, tags
+
+
+def fold_rows(rows, m):
+    """The one-process device state from every shard's tagged rows (on one device): put in global batch order and folded
+    from zero by the same accumulator as one process.  None when there are no rows."""
+    if rows.shape[0] == 0:
+        return None
+    rows, tags = sort_rows(rows)
+    state = torch.zeros(3 * m + 1, dtype=torch.float64, device=rows.device)
+    return M.eval_accumulate_impl(rows[:, 2:].to(torch.float32), tags[:, 1].tolist(), state)
+
+
+def log_dict(state, m):
+    """Evaluater.eval's dict from the device state of m metrics (None: no batch), with its one device-to-host read."""
+    s = np.zeros(3 * m + 1) if state is None else state.cpu().numpy()
+    total, valid, avg = s[:m], s[m:2 * m], s[2 * m:3 * m]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        metrics = (total / valid).tolist()
+    return {"loss": 0.0, "metrics": metrics, "metrics_correct": avg.tolist(), "valid_batches": valid[0],
+            "loss_loss": 0.0}

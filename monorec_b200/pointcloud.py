@@ -2,9 +2,10 @@
 
 `PLYSaver` keeps the reference's constructor, `add_depthmap(depth, image, intrinsics, extrinsics)` and `save(file)`; the
 vertices stay in one growing device buffer (the reference does `.cpu().tolist()` per frame) and are written in the reference's
-order.  `keep_mask` is the 33x33 dilation of the moving-object mask, `MaskVoter` the sliding-window vote of
-create_pointcloud.py:80-104.  The arithmetic runs in libmonorec_b200.so (csrc/pointcloud.cu); no CPU fallback.
+order, with no host synchronisation until they are read.  `keep_mask` is the 33x33 dilation of the moving-object mask,
+`MaskVoter` the sliding-window vote of create_pointcloud.py:80-104.  The arithmetic runs in libmonorec_b200.so (csrc/pointcloud.cu); no CPU fallback.
 """
+import collections
 import ctypes
 
 import torch
@@ -34,10 +35,18 @@ class PLYSaver(torch.nn.Module):
         self.height, self.width = height, width
         self.min_d, self.max_d, self.roi, self.dropout = min_d, max_d, roi, dropout
         self._buf = None            # device float [capacity, 6]
-        self._count = None          # device int64 [1]: vertices stored (negative: last add did not fit)
+        self._count = None          # device int64 [1]: vertices stored (negative: an add did not fit)
+        self._known = 0             # the count after the last add whose read-back has landed
+        self._in_flight = collections.deque()   # (event, pinned copy of the count, vertex bound) of the later adds
 
     def __len__(self):
-        return 0 if self._count is None else int(self._count.item())
+        """The vertex count: a host synchronisation (as `vertices`, `gather` and `save`)."""
+        if self._count is None:
+            return 0
+        n = int(self._count.item())
+        if n < 0:
+            raise RuntimeError(f"PLYSaver: the vertex buffer of {self._buf.shape[0]} vertices overflowed ({-n} needed)")
+        return n
 
     @property
     def vertices(self):
@@ -60,31 +69,46 @@ class PLYSaver(torch.nn.Module):
         masks = [m.to(torch.float32).contiguous() for m in keep_masks]
         if self.dropout > 0 and rand is None:
             rand = torch.rand_like(d)                                     # ply_utils.py:44-45
-        n_before, ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
         with torch.cuda.device(dev):
+            ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
             _lib.check(lib.mr_pointcloud_add(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(),
                                              _lib.ptr_array(masks) if masks else None, len(masks), int(min_hits), B, H, W,
                                              float(self.min_d), float(self.max_d), roi,
                                              None if rand is None else rand.contiguous().data_ptr(), float(self.dropout),
-                                             self._buf.data_ptr(), self._buf.shape[0], n_before, self._count.data_ptr(),
+                                             self._buf.data_ptr(), self._buf.shape[0], -1, self._count.data_ptr(),
                                              ws.data_ptr(), ws_bytes, torch.cuda.current_stream(dev).cuda_stream),
                        "mr_pointcloud_add")
+            self._track(B * H * W, dev)
 
     def _reserve(self, lib, B, H, W, dev):
-        """Room for B more depth maps: (n_before, workspace, its bytes, roi as a C array)."""
+        """Room for B more depth maps, without waiting for the device: (workspace, its bytes, roi as a C array).
+
+        The kernels take the write position from the device count (n_before = -1).  The host bounds that count by the last
+        count read back (an asynchronous copy per add, see `_track`) plus B*H*W per add since, and grows the buffer, by a
+        copy ordered on the stream after those adds, only when the bound plus this batch's B*H*W would not fit."""
         if self._buf is None:
             self._buf = torch.empty(max(4 * B * H * W, 1 << 20), 6, device=dev)
             self._count = torch.zeros(1, dtype=torch.int64, device=dev)
         ws_bytes = lib.mr_pointcloud_workspace(B, H, W)
-        ws = torch.empty(ws_bytes // 4, dtype=torch.int32, device=dev)
+        ws = torch.empty((ws_bytes + 7) // 8, dtype=torch.int64, device=dev)
         roi = None if self.roi is None else (ctypes.c_int * 4)(*[int(v) for v in self.roi])
-        # the buffer position of this batch is the count so far: one 8-byte D2H per batch (the reference copies every vertex)
-        n_before = int(self._count.item())
-        if n_before + B * H * W > self._buf.shape[0]:
-            grown = torch.empty(2 * (n_before + B * H * W), 6, device=dev)
-            grown[:n_before] = self._buf[:n_before]
+        while self._in_flight and self._in_flight[0][0].query():
+            self._known = abs(int(self._in_flight.popleft()[1]))   # an overflow (< 0) surfaces at the next len()
+        bound = self._known + sum(worst for _, _, worst in self._in_flight)
+        if bound + B * H * W > self._buf.shape[0]:
+            grown = torch.empty(2 * (bound + B * H * W), 6, device=dev)
+            n = min(bound, self._buf.shape[0])
+            grown[:n] = self._buf[:n]
             self._buf = grown
-        return n_before, ws, ws_bytes, roi
+        return ws, ws_bytes, roi
+
+    def _track(self, worst, dev):
+        """After an add of at most `worst` vertices: the count's asynchronous copy to pinned memory, and its event."""
+        seen = torch.empty(1, dtype=torch.int64, pin_memory=True)
+        seen.copy_(self._count, non_blocking=True)
+        done = torch.cuda.Event()
+        done.record(torch.cuda.current_stream(dev))
+        self._in_flight.append((done, seen, worst))
 
     def add_depthmap_windows(self, depth, image, intrinsics, extrinsics, keep_ring, window_start, n_masks, min_hits=1,
                              rand=None):
@@ -108,16 +132,17 @@ class PLYSaver(torch.nn.Module):
         if self.dropout > 0 and rand is None:
             rand = torch.rand_like(d)                                     # ply_utils.py:44-45
         starts = (ctypes.c_int * B)(*[int(v) for v in window_start])
-        n_before, ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
         with torch.cuda.device(dev):
+            ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
             _lib.check(lib.mr_pointcloud_add_windows(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(), ring.data_ptr(),
                                                      ring.shape[0], starts, int(n_masks), int(min_hits), B, H, W,
                                                      float(self.min_d), float(self.max_d), roi,
                                                      None if rand is None else rand.contiguous().data_ptr(),
-                                                     float(self.dropout), self._buf.data_ptr(), self._buf.shape[0], n_before,
+                                                     float(self.dropout), self._buf.data_ptr(), self._buf.shape[0], -1,
                                                      self._count.data_ptr(), ws.data_ptr(), ws_bytes,
                                                      torch.cuda.current_stream(dev).cuda_stream),
                        "mr_pointcloud_add_windows")
+            self._track(B * H * W, dev)
 
     def gather(self, group=None, dst=0):
         """Every rank's vertices, in rank order, on rank `dst` of `group` (a torch.distributed process group; a collective:
@@ -140,13 +165,18 @@ class PLYSaver(torch.nn.Module):
                 return
         else:
             v = self.vertices
-        v = v.detach().to("cpu", torch.float32).contiguous()
-        header = ("ply\nformat binary_little_endian 1.0\n"
-                  f"element vertex {v.shape[0]}\n"
-                  "property float x\nproperty float y\nproperty float z\n"
-                  "property float red\nproperty float green\nproperty float blue\nend_header\n")
-        file.write(header.encode(encoding="ascii"))
-        file.write(v.numpy().tobytes())
+        write_ply(file, v)
+
+
+def write_ply(file, vertices):
+    """Vertices [N, 6] (x, y, z, red, green, blue) as a binary little-endian PLY with the reference's header."""
+    v = vertices.detach().to("cpu", torch.float32).contiguous()
+    header = ("ply\nformat binary_little_endian 1.0\n"
+              f"element vertex {v.shape[0]}\n"
+              "property float x\nproperty float y\nproperty float z\n"
+              "property float red\nproperty float green\nproperty float blue\nend_header\n")
+    file.write(header.encode(encoding="ascii"))
+    file.write(v.numpy().tobytes())
 
 
 class MaskVoter:
