@@ -57,17 +57,14 @@ def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eva
         raise ValueError("shard_sequences: give exactly one of eval_batch and buffer_length")
     if batch_size < 1 or world < 1 or not 0 <= rank < world:
         raise ValueError(f"shard_sequences: batch_size ({batch_size}) >= 1 and 0 <= rank ({rank}) < world ({world}) needed")
-    from .sequence import neighbour_offsets
+    from .sequence import check_keys, neighbour_offsets
     offs = neighbour_offsets(frame_count, dilation)
     lo, hi = min(0, min(offs)), max(offs)
     if keys is not None and len(keys) != len(lengths):
         raise ValueError(f"shard_sequences: {len(keys)} key lists for {len(lengths)} sequences")
     # the key frames of each sequence: the listed ones, or -lo .. n - hi - 1
-    K = [list(range(-lo, int(n) - hi)) if keys is None or keys[s] is None else [int(k) for k in keys[s]]
+    K = [range(-lo, int(n) - hi) if keys is None or keys[s] is None else check_keys(keys[s], offs, n)
          for s, n in enumerate(lengths)]
-    for s, (k, n) in enumerate(zip(K, lengths)):
-        if any(b <= a for a, b in zip(k, k[1:])) or (k and (k[0] < -lo or k[-1] >= int(n) - hi)):
-            raise ValueError(f"shard_sequences: the key frames of sequence {s} must be increasing and in [{-lo}, {n - hi})")
     n_keys = [len(k) for k in K]
     if eval_batch is not None:
         if eval_batch < 1:

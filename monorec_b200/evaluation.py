@@ -4,8 +4,9 @@ The reference's loop takes the loader's batches of key-frame dicts (batch size 2
 an eager forward per batch and turns every metric of every batch into a Python float.  `SequenceEvaluater` takes the frames
 of a sequence and their targets one at a time instead: the model runs through the `MonoRecSequence` (rings, CUDA-graph
 replay), every batch of key frames it emits is cut into the evaluater's batches, and per emitted batch one grouped metric
-pass (`mr_sparse_metrics_grouped` / `mr_dense_metrics_grouped`) and one `mr_eval_accumulate` update the evaluater's float64
-totals on the device.  `log()` reads them back once and returns `Evaluater.eval`'s dict.
+pass (`mr_sparse_metrics_grouped` / `mr_dense_metrics_grouped`) leaves one metric row per evaluater batch on the device.
+`log()` folds the rows with `mr_eval_accumulate` into the evaluater's float64 totals, reads them back once and returns
+`Evaluater.eval`'s dict.
 """
 import numpy as np
 import torch
@@ -63,21 +64,22 @@ class SequenceEvaluater:
     `add(result, target, mvobj_mask=None)` is the part after the model: the batching and accumulation of results already
     computed ([n,1,H,W] each, key frames in order); `seq` may be None when only `add` is used.
 
-    `log()` makes the one device-to-host read and returns the evaluater's dict: `loss` and `loss_loss` 0.0, `metrics` (total
-    over valid batches: NaN for a metric no batch was valid for), `metrics_correct` (the running average over samples) and
-    `valid_batches`.  Batches still open are not in it: call `flush()` first.
+    `log()` folds the closed evaluater batches' metric rows in batch order, makes the one device-to-host read and returns
+    the evaluater's dict: `loss` and `loss_loss` 0.0, `metrics` (total over valid batches: NaN for a metric no batch was
+    valid for), `metrics_correct` (the running average over samples) and `valid_batches`.  Batches still open are not in
+    it: call `flush()` first.
 
     Several processes (one per GPU, or several on one GPU) evaluate one run together with `group` (a torch.distributed
     process group) and `shard`, this rank's slices of the sequences (`dist.shard_sequences(..., eval_batch=batch_size)`):
     `seq` and every sequence given to `next_sequence` run `shard`'s slices in order (MonoRecSequence(first_frame=
     slice.frames[0], key_end=slice.run[1]), fed frames slice.frames[0] ... slice.frames[1] - 1), and only the key frames
-    of each slice's `emit` range are evaluated.  Each evaluater batch's metric row stays on the device, tagged with the
-    batch's index in the whole run, instead of being folded at once.  `log()` is then a collective: every rank of `group`
-    calls it, the rows of all ranks are gathered, and the one-process fold runs over them in global batch order on every
-    rank, so every rank returns the one-process log (the same device state, bit for bit).
+    of each slice's `emit` range are evaluated.  Each evaluater batch's metric row is tagged with the batch's index in the
+    whole run.  `log()` is then a collective: every rank of `group` calls it, the rows of all ranks are gathered, and the
+    one-process fold runs over them in global batch order on every rank, so every rank returns the one-process log (the
+    same device state, bit for bit).
 
-    `group=LANE` makes the evaluater one lane of a one-process run over several devices (lanes.MultiDeviceEvaluater): it
-    keeps its shard's rows the same way, and its driver collects them (`tagged_rows`) and runs the same fold.
+    `group=LANE` makes the evaluater one lane of a one-process run over several devices (lanes.MultiDeviceEvaluater): its
+    driver collects its shard's rows (`tagged_rows`) and runs the same fold.
     """
 
     def __init__(self, seq, metrics, batch_size, roi=None, max_distance=None, median_scaling=False, group=None, shard=None):
@@ -98,7 +100,6 @@ class SequenceEvaluater:
         self.max_distance, self.median_scaling = max_distance, bool(median_scaling)
         self._specs = [METRICS[n] for n in self.names]
         self._needs_mvobj = any(key[0] == "sparse" and key[2] for key, _ in self._specs)
-        self._state = None         # device float64 [3M+1]: total, valid, running average, num_samples
         self._open = None          # (result, target, mvobj_mask) of the key frames of the open evaluater batch
         if (group is None) != (shard is None):
             raise ValueError("SequenceEvaluater: group and shard go together (shard: dist.shard_sequences(...)'s slices)")
@@ -108,7 +109,7 @@ class SequenceEvaluater:
                 raise ValueError(f"SequenceEvaluater: the shard starts at key frame {self._slices[0].position}, inside an "
                                  f"evaluater batch of {self.batch_size} (shard_sequences(..., eval_batch={self.batch_size}))")
             self._check_slice(seq)
-        # sharded: the metric rows of this rank's closed evaluater batches, their sizes and their global batch indices
+        # the metric rows of the closed evaluater batches (device), their sizes and their global batch indices (host)
         self._rows, self._row_sizes, self._row_index = [], [], []
         self._batch_index = self._slices[0].position // self.batch_size if self._slices else 0
 
@@ -206,8 +207,6 @@ class SequenceEvaluater:
         result, target = parts[0], parts[1]
         mvobj_mask = parts[2] if len(parts) > 2 else None
         group = sizes[0]
-        if self._state is None:
-            self._state = torch.zeros(3 * len(self.names) + 1, dtype=torch.float64, device=result.device)
 
         def run(key, pred):
             if key[0] == "dense":
@@ -228,18 +227,15 @@ class SequenceEvaluater:
             for key, col in self._specs:
                 cur = M.median_scaling_impl(cur, target)
                 cols.append(run(key, cur)[:, col])
-        if self._slices is None:
-            M.eval_accumulate_impl(torch.stack(cols, 1), sizes, self._state)
-            return
         self._rows.append(torch.stack(cols, 1).to(torch.float32))
         self._row_sizes += sizes
         self._row_index += range(self._batch_index, self._batch_index + len(sizes))
         self._batch_index += len(sizes)
 
     def tagged_rows(self, device=None):
-        """A sharded evaluater's closed evaluater batches as float64 rows [G, 2 + M] on `device` (default: where they are):
-        global batch index, batch size, then the metric row.  Float64 holds the float32 values (NaN and inf included) and
-        the integer tags exactly."""
+        """The closed evaluater batches as float64 rows [G, 2 + M] on `device` (default: where they are): global batch
+        index, batch size, then the metric row.  Float64 holds the float32 values (NaN and inf included) and the integer
+        tags exactly."""
         m = len(self.names)
         dev = device if device is not None else self.seq.device if self.seq is not None else (
             self._rows[0].device if self._rows else torch.device("cuda", torch.cuda.current_device()))
@@ -250,10 +246,12 @@ class SequenceEvaluater:
     def log(self):
         if self.group is LANE:
             raise ValueError("SequenceEvaluater.log: a lane's rows are folded by its driver (MultiDeviceEvaluater.log)")
-        if self._slices is None:
-            return log_dict(self._state, len(self.names))
+        m = len(self.names)
+        if self.group is None:
+            # its own rows, closed in batch order, with their sizes on the host: folded without reading tags back
+            return log_dict(_accumulate(torch.cat(self._rows), self._row_sizes, m) if self._rows else None, m)
         from .dist import all_gather_rows
-        return log_dict(fold_rows(all_gather_rows(self.tagged_rows(), self.group), len(self.names)), len(self.names))
+        return log_dict(fold_rows(all_gather_rows(self.tagged_rows(), self.group), m), m)
 
 
 LANE = "lane"
@@ -277,8 +275,14 @@ def fold_rows(rows, m):
     if rows.shape[0] == 0:
         return None
     rows, tags = sort_rows(rows)
-    state = torch.zeros(3 * m + 1, dtype=torch.float64, device=rows.device)
-    return M.eval_accumulate_impl(rows[:, 2:].to(torch.float32), tags[:, 1].tolist(), state)
+    return _accumulate(rows[:, 2:], tags[:, 1].tolist(), m)
+
+
+def _accumulate(values, sizes, m):
+    """The device state of evaluater batches of `sizes` images with metric rows `values` [G, M], in batch order: folded
+    from zero by mr_eval_accumulate."""
+    state = torch.zeros(3 * m + 1, dtype=torch.float64, device=values.device)
+    return M.eval_accumulate_impl(values.to(torch.float32), sizes, state)
 
 
 def log_dict(state, m):

@@ -27,7 +27,7 @@ import torch
 from .dist import shard_sequences
 from .evaluation import LANE, SequenceEvaluater, fold_rows, log_dict
 from .pointcloud import PLYSaver, SequencePointCloud, write_ply
-from .sequence import MonoRecSequence, neighbour_offsets
+from .sequence import MonoRecSequence, needs_frame, neighbour_offsets
 
 
 class LanePlan:
@@ -46,18 +46,14 @@ class LanePlan:
         self.lanes, self.keys = int(lanes), keys
         self.slices = [shard_sequences(lengths, frame_count, dilation, batch_size, r, lanes, eval_batch=eval_batch,
                                        buffer_length=buffer_length, keys=keys) for r in range(lanes)]
-        uses = [0] + neighbour_offsets(frame_count, dilation)
+        offsets = neighbour_offsets(frame_count, dilation)
         self.frames = []
         for sl in self.slices:
             mine = []
             for k, s in enumerate(sl):
-                listed = None if keys is None else keys[s.sequence]
-                if listed is None:
-                    need = range(*s.frames)
-                else:
-                    run = [int(x) for x in listed if s.run[0] <= int(x) < s.run[1]]
-                    need = sorted({x + u for x in run for u in uses})
-                mine += [(k, s.sequence, n) for n in need]
+                listed = range(*s.run) if keys is None or keys[s.sequence] is None else keys[s.sequence]
+                run = [int(x) for x in listed if s.run[0] <= int(x) < s.run[1]]
+                mine += [(k, s.sequence, n) for n in range(*s.frames) if needs_frame(run, offsets, n)]
             self.frames.append(mine)
         self.users = {}                    # (sequence, frame) -> the lanes that need it
         for r, mine in enumerate(self.frames):

@@ -57,27 +57,42 @@ class PLYSaver(torch.nn.Module):
     def add_depthmap(self, depth, image, intrinsics, extrinsics, keep_masks=(), min_hits=1, rand=None):
         """depth: inverse depth [B,1,H,W] (the reference's argument name); keep_masks: the voting window's masks (optional:
         the reference multiplies the depth by the voted mask before calling; passing the masks here fuses that product)."""
+        masks = [m.to(torch.float32).contiguous() for m in keep_masks]
+        self._add("mr_pointcloud_add", depth, image, intrinsics, extrinsics, rand,
+                  _lib.ptr_array(masks) if masks else None, len(masks), int(min_hits))
+
+    def add_depthmap_windows(self, depth, image, intrinsics, extrinsics, keep_ring, window_start, n_masks, min_hits=1,
+                             rand=None):
+        """`add_depthmap` of B consecutive key frames, each voted with its own window: key frame b keeps the pixels where
+        more than n_masks - min_hits of the keep masks in ring slots window_start[b], window_start[b] + 1, ...
+        (mod len(keep_ring)) are 1.  The vertices are those of B add_depthmap calls, in the same order.
+        keep_ring: device [R,1,H,W]; window_start: B host ints."""
+        ring = keep_ring.to(torch.float32).contiguous()
+        B, _, H, W = depth.shape
+        if len(window_start) != B or tuple(ring.shape[1:]) != (1, H, W):
+            raise ValueError(f"add_depthmap_windows: {len(window_start)} window starts and a keep ring of "
+                             f"{tuple(ring.shape)} for depth maps {tuple(depth.shape)}")
+        self._add("mr_pointcloud_add_windows", depth, image, intrinsics, extrinsics, rand, ring.data_ptr(), ring.shape[0],
+                  (ctypes.c_int * B)(*[int(v) for v in window_start]), int(n_masks), int(min_hits))
+
+    def _add(self, entry, depth, image, intrinsics, extrinsics, rand, *vote):
+        """One call of the C `entry` (mr_pointcloud_add or mr_pointcloud_add_windows) on B depth maps: `vote` are its
+        arguments between the extrinsics and B, the keep masks and their vote."""
         if not depth.is_cuda:
             raise _lib.MonorecLibraryError("monorec_b200.pointcloud needs CUDA tensors (no CPU fallback)")
         lib = _lib.load()
         dev = depth.device
-        d = depth.to(torch.float32).contiguous()
-        img = image.to(torch.float32).contiguous()
-        K = intrinsics.to(torch.float32).contiguous()
-        P = extrinsics.to(torch.float32).contiguous()
+        d, img, K, P = [t.to(torch.float32).contiguous() for t in (depth, image, intrinsics, extrinsics)]
         B, _, H, W = d.shape
-        masks = [m.to(torch.float32).contiguous() for m in keep_masks]
         if self.dropout > 0 and rand is None:
             rand = torch.rand_like(d)                                     # ply_utils.py:44-45
         with torch.cuda.device(dev):
             ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
-            _lib.check(lib.mr_pointcloud_add(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(),
-                                             _lib.ptr_array(masks) if masks else None, len(masks), int(min_hits), B, H, W,
-                                             float(self.min_d), float(self.max_d), roi,
-                                             None if rand is None else rand.contiguous().data_ptr(), float(self.dropout),
-                                             self._buf.data_ptr(), self._buf.shape[0], -1, self._count.data_ptr(),
-                                             ws.data_ptr(), ws_bytes, torch.cuda.current_stream(dev).cuda_stream),
-                       "mr_pointcloud_add")
+            _lib.check(getattr(lib, entry)(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(), *vote, B, H, W,
+                                           float(self.min_d), float(self.max_d), roi,
+                                           None if rand is None else rand.contiguous().data_ptr(), float(self.dropout),
+                                           self._buf.data_ptr(), self._buf.shape[0], -1, self._count.data_ptr(),
+                                           ws.data_ptr(), ws_bytes, torch.cuda.current_stream(dev).cuda_stream), entry)
             self._track(B * H * W, dev)
 
     def _reserve(self, lib, B, H, W, dev):
@@ -109,40 +124,6 @@ class PLYSaver(torch.nn.Module):
         done = torch.cuda.Event()
         done.record(torch.cuda.current_stream(dev))
         self._in_flight.append((done, seen, worst))
-
-    def add_depthmap_windows(self, depth, image, intrinsics, extrinsics, keep_ring, window_start, n_masks, min_hits=1,
-                             rand=None):
-        """`add_depthmap` of B consecutive key frames, each voted with its own window: key frame b keeps the pixels where
-        more than n_masks - min_hits of the keep masks in ring slots window_start[b], window_start[b] + 1, ...
-        (mod len(keep_ring)) are 1.  The vertices are those of B add_depthmap calls, in the same order.
-        keep_ring: device [R,1,H,W]; window_start: B host ints."""
-        if not depth.is_cuda:
-            raise _lib.MonorecLibraryError("monorec_b200.pointcloud needs CUDA tensors (no CPU fallback)")
-        lib = _lib.load()
-        dev = depth.device
-        d = depth.to(torch.float32).contiguous()
-        img = image.to(torch.float32).contiguous()
-        K = intrinsics.to(torch.float32).contiguous()
-        P = extrinsics.to(torch.float32).contiguous()
-        ring = keep_ring.to(torch.float32).contiguous()
-        B, _, H, W = d.shape
-        if len(window_start) != B or tuple(ring.shape[1:]) != (1, H, W):
-            raise ValueError(f"add_depthmap_windows: {len(window_start)} window starts and a keep ring of "
-                             f"{tuple(ring.shape)} for depth maps {tuple(d.shape)}")
-        if self.dropout > 0 and rand is None:
-            rand = torch.rand_like(d)                                     # ply_utils.py:44-45
-        starts = (ctypes.c_int * B)(*[int(v) for v in window_start])
-        with torch.cuda.device(dev):
-            ws, ws_bytes, roi = self._reserve(lib, B, H, W, dev)
-            _lib.check(lib.mr_pointcloud_add_windows(d.data_ptr(), img.data_ptr(), K.data_ptr(), P.data_ptr(), ring.data_ptr(),
-                                                     ring.shape[0], starts, int(n_masks), int(min_hits), B, H, W,
-                                                     float(self.min_d), float(self.max_d), roi,
-                                                     None if rand is None else rand.contiguous().data_ptr(),
-                                                     float(self.dropout), self._buf.data_ptr(), self._buf.shape[0], -1,
-                                                     self._count.data_ptr(), ws.data_ptr(), ws_bytes,
-                                                     torch.cuda.current_stream(dev).cuda_stream),
-                       "mr_pointcloud_add_windows")
-            self._track(B * H * W, dev)
 
     def gather(self, group=None, dst=0):
         """Every rank's vertices, in rank order, on rank `dst` of `group` (a torch.distributed process group; a collective:

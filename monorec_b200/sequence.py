@@ -11,6 +11,7 @@ right camera's frame (`return_stereo`) and a moving-object mask (`return_mvobj_m
 sequence takes those as `keys=`, `stereo=True` and `mvobj_masks=True`.
 """
 import bisect
+import sys
 
 import torch
 
@@ -42,6 +43,31 @@ def loader_keys(length, frame_count=2, dilation=1, lidar_depth=False, annotated_
     for m in index_masks or ():
         keys = [k for k in keys if m.get(str(k))]
     return list(keys)
+
+
+def check_keys(keys, offsets, length=None):
+    """`keys` as a list of ints, checked to be increasing sequence indices of key frames with all their neighbours (at
+    `offsets`) in the sequence: from -min(offsets) on, and before length - max(offsets) when `length` is given."""
+    keys = [int(k) for k in keys]
+    lo, hi = min(0, min(offsets)), max(offsets)
+    end = None if length is None else int(length) - hi
+    if any(b <= a for a, b in zip(keys, keys[1:])) or (keys and (keys[0] < -lo or (end is not None and keys[-1] >= end))):
+        raise ValueError(f"key frames must be increasing sequence indices in [{-lo}, {'...' if end is None else end}): the "
+                         "key frames with all their neighbours in the sequence")
+    return keys
+
+
+def needs_frame(keys, offsets, n):
+    """Whether frame n is one of the key frames `keys` (sorted: a list or a range) or one of their neighbours at `offsets`."""
+    return any(_listed(keys, n - u) for u in [0] + list(offsets))
+
+
+def _listed(keys, k):
+    """Whether k is in the sorted `keys`: a range answers by arithmetic, a list by bisection."""
+    if isinstance(keys, range):
+        return k in keys
+    i = bisect.bisect_left(keys, k)
+    return i < len(keys) and keys[i] == k
 
 
 class MonoRecSequence:
@@ -117,38 +143,26 @@ class MonoRecSequence:
         self._graph = None
         self._uses = [0] + self.offsets    # a key frame's own frame, then its source frames
         if keys is None:
-            self.keys = None
+            # every key frame: when batch [k, k+B) runs, the live frames are k+lo ... k+B-1+hi (all earlier ones are freed)
+            self.keys, listed = None, range(self.first_key, sys.maxsize)
             self.ring_len = self._hi - lo + 1 + self.batch_size
-            self.key_position = self.key_begin - self.first_key
-            self._next = self.key_begin    # the next key frame to run
-            # ring slots of a batch, relative to its first key frame: row 0 the key frames, row 1 + f their f-th sources
-            rel = torch.tensor(self._uses).view(-1, 1) + torch.arange(self.batch_size).view(1, -1)
-            self._rel = rel.to(self.device)
-            return
-        self.keys = [int(k) for k in keys]
-        if any(b <= a for a, b in zip(self.keys, self.keys[1:])) or (self.keys and self.keys[0] < self.first_key):
-            raise ValueError(f"MonoRecSequence: keys must be increasing sequence indices >= {self.first_key} (the first "
-                             f"key frame with all its neighbours)")
-        self.ring_len = self.batch_size * len(self._uses) + self._hi - lo
-        self.key_position = bisect.bisect_left(self.keys, self.key_begin)   # place of the first key frame run in `keys`
-        end = len(self.keys) if self.key_end is None else bisect.bisect_left(self.keys, self.key_end)
-        self._run_keys = self.keys[self.key_position:end]
-        self._run_set = set(self._run_keys)
+        else:
+            self.keys = listed = check_keys(keys, self.offsets)
+            self.ring_len = self.batch_size * len(self._uses) + self._hi - lo
+        self.key_position = bisect.bisect_left(listed, self.key_begin)   # place of the first key frame run in the list
+        end = len(listed) if self.key_end is None else bisect.bisect_left(listed, self.key_end)
+        self._run_keys = listed[self.key_position:end]
         self._next = 0                     # the next key frame to run: its place in _run_keys
         self._slot = {}                    # sequence index of a copied frame -> (ring slot, last key frame that uses it)
         self._free = list(range(self.ring_len))[::-1]
 
     def needs(self, n):
         """Whether `push` copies frame n: it is a key frame this sequence runs or a neighbour of one."""
-        if self.keys is None:
-            return self.key_end is None or n < self.key_end + self._hi
-        return any(n - u in self._run_set for u in self._uses)
+        return needs_frame(self._run_keys, self.offsets, n)
 
     def runs(self, n):
         """Whether key frame n is one this sequence runs (for keys=None: any frame in [key_begin, key_end))."""
-        if self.keys is None:
-            return n >= self.key_begin and (self.key_end is None or n < self.key_end)
-        return n in self._run_set
+        return _listed(self._run_keys, n)
 
     def skip(self):
         """Passes the next frame without its data; only a frame that no key frame run needs (`needs`) can be skipped."""
@@ -232,25 +246,18 @@ class MonoRecSequence:
 
     def _store(self, n):
         """The ring slot of frame n."""
-        if self.keys is None:
-            return n % self.ring_len
         if not self._free:
             raise RuntimeError("MonoRecSequence: the frame ring is full (a bookkeeping error)")
-        self._slot[n] = (self._free.pop(), max(n - u for u in self._uses if n - u in self._run_set))
+        self._slot[n] = (self._free.pop(), max(n - u for u in self._uses if _listed(self._run_keys, n - u)))
         return self._slot[n][0]
 
     def _ready(self):
         """Key frames not yet run (before key_end) whose neighbours have all been pushed."""
-        ready = self.n_pushed - self._hi
-        if self.keys is not None:
-            return bisect.bisect_left(self._run_keys, ready) - self._next
-        return (ready if self.key_end is None else min(ready, self.key_end)) - self._next
+        return bisect.bisect_left(self._run_keys, self.n_pushed - self._hi) - self._next
 
     def _remaining(self):
-        """Key frames left to run, when the sequence knows where they end."""
-        if self.keys is not None:
-            return len(self._run_keys) - self._next
-        return None if self.key_end is None else self.key_end - self._next
+        """Key frames left to run."""
+        return len(self._run_keys) - self._next
 
     def _assemble(self, idx, out=None):
         """The batch dict, with the reference's keys and list order, gathered from the rings at slots `idx` [1+F, n];
@@ -267,14 +274,10 @@ class MonoRecSequence:
         return data
 
     def _run(self, n, graphed):
-        if self.keys is None:
-            index = list(range(self._next, self._next + n))
-            idx = torch.remainder(self._rel[:, :n] + self._next, self.ring_len)
-        else:
-            index = self._run_keys[self._next:self._next + n]
-            idx = torch.tensor([[self._slot[k + u][0] for k in index] for u in self._uses], dtype=torch.int64)
-            # a pinned copy does not synchronise; the host allocator keeps the block until the copy is done
-            idx = idx.pin_memory().to(self.device, non_blocking=True) if self.device.type == "cuda" else idx
+        index = self._run_keys[self._next:self._next + n]
+        idx = torch.tensor([[self._slot[k + u][0] for k in index] for u in self._uses], dtype=torch.int64)
+        # a pinned copy does not synchronise; the host allocator keeps the block until the copy is done
+        idx = idx.pin_memory().to(self.device, non_blocking=True) if self.device.type == "cuda" else idx
         if not graphed:
             out = self.model(self._assemble(idx))
         elif self._graph is None:
@@ -284,10 +287,9 @@ class MonoRecSequence:
             self._assemble(idx, out=self._graph.static_in)
             out = self._graph.replay()
         self._next += n
-        if self.keys is not None:
-            # frames no later key frame uses go back to the free slots (their next writes follow this batch's gathers)
-            for f in [f for f, (_, last) in self._slot.items() if last <= index[-1]]:
-                self._free.append(self._slot.pop(f)[0])
+        # frames no later key frame uses go back to the free slots (their next writes follow this batch's gathers)
+        for f in [f for f, (_, last) in self._slot.items() if last <= index[-1]]:
+            self._free.append(self._slot.pop(f)[0])
         return [(i, _row(out, j)) for j, i in enumerate(index)]
 
 _ROW_KEYS = ("result", "cv_mask", "cost_volume", "keyframe", "keyframe_pose", "keyframe_intrinsics", "stereoframe",

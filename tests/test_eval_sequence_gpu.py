@@ -277,7 +277,7 @@ def test_push_and_flush_do_not_synchronise(model):
         while not ev.push(images[n], poses[n], Ks[n], target[n]):      # up to the first batch: its graph is captured
             n += 1
         emitted = 4
-        second = MonoRecSequence(model, batch_size=4)                    # (its constructor copies a slot table to the device)
+        second = MonoRecSequence(model, batch_size=4)
         torch.cuda.synchronize()
         torch.cuda.set_sync_debug_mode("error")
         try:

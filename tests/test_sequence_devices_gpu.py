@@ -130,20 +130,26 @@ def _sync_free_after_capture(run, push, sequences):
     return checked
 
 
-@pytest.mark.parametrize("devices", LANES, ids=lambda d: "-".join(map(str, d)))
-def test_lanes_make_no_host_synchronisation(one_process, devices):
+@pytest.mark.parametrize("devices,keyed", [(d, k) for k in (False, True) for d in LANES],
+                         ids=["-".join(map(str, d)) + ("-index_masked" if k else "") for k in (False, True) for d in LANES])
+def test_lanes_make_no_host_synchronisation(one_process, devices, keyed):
+    """Every key frame, or an index-masked key list (key frames 5 ... 7 masked out, so frame 6 is skipped)."""
     from monorec_b200.lanes import MultiDeviceEvaluater, MultiDevicePointCloud
+    from monorec_b200.sequence import loader_keys
     model, pc_model, inputs, _, _ = one_process
     seqs, targets, masks, rands = inputs
     lengths = [seqs[0][0].shape[0]]
+    keys = [loader_keys(lengths[0], index_masks=[{str(k): not 5 <= k <= 7 for k in range(lengths[0])}])] if keyed else None
     with torch.no_grad():
-        ev = MultiDeviceEvaluater(model, devices, lengths, D.NAMES, 2, seq_batch=2, roi=D.ROI, max_distance=D.MAX_D)
+        ev = MultiDeviceEvaluater(model, devices, lengths, D.NAMES, 2, seq_batch=2, keys=keys, roi=D.ROI,
+                                  max_distance=D.MAX_D)
         push = lambda s, n: ev.push(s, n, seqs[s][0][n], seqs[s][1][n], seqs[s][2][n], targets[s][n],  # noqa: E731
                                     mvobj_mask=masks[s][n])
         assert _sync_free_after_capture(ev, push, lambda: [e.seq for e in ev.evaluaters if e is not None])
         assert ev.log()["valid_batches"] > 0
         mov = D._MovingObject(pc_model, step=float(seqs[0][1][1, 2, 3]))
-        pc = MultiDevicePointCloud(mov, devices, lengths, D.H, D.W, seq_batch=2, min_d=3, max_d=20, dropout=0.75)
+        pc = MultiDevicePointCloud(mov, devices, lengths, D.H, D.W, seq_batch=2, keys=keys, min_d=3, max_d=20,
+                                   dropout=0.75)
         push = lambda s, n: pc.push(s, n, seqs[s][0][n], seqs[s][1][n], seqs[s][2][n], rand=rands[s][n])  # noqa: E731
         assert _sync_free_after_capture(pc, push, lambda: [r.seq if r else None
                                                            for r, sl in zip(pc._runner, pc.plan.slices) if sl])
