@@ -9,16 +9,24 @@ create_mask) with model/layers.py:43-71 (Backprojection, point_projection) and :
 
 Parity pin: the reference has no tests or golden vectors of its own ("parity unpinned" by the reference,
 SURVEY.md §4/§8c).  This oracle is pinned instead against outputs of the *reference itself* run on the CPU
-(tests/golden/make_golden.py imports it unmodified from a checkout of the reference and writes
-tests/golden/*.npz); tests/test_oracle_golden.py checks both restatements below against those files.
+(tests/golden/make_golden*.py import it unmodified from a checkout of the reference and write
+tests/golden/*.npz); tests/test_oracle_golden.py, tests/test_cv_pixel_depths.py and tests/test_cv_matching.py check
+both restatements below against those files.
 
-Two independent restatements:
+Two independent restatements, each with every option the kernel implements:
 
 * `cost_volume_torch`  -- same library primitives as the reference (F.grid_sample, avg_pool2d, conv3d), so it
   has the reference's CPU performance characteristics; this is what `bench.py` times as the CPU baseline
   ("port").
 * `cost_volume_closed_form` -- numpy, explicit bilinear gather and box sums following SURVEY.md Appendix C;
   shares no primitive with the first one and can run in float64 (used for tie margins).
+
+The options, with the reference's defaults:
+* the depths: uniform in inverse depth from (inv_depth_min, inv_depth_max, steps), or per pixel from
+  `cv_depths` (B, D, H, W), the reference's data_dict["cv_depths"] (monorec_model.py:181-201);
+* the difference, `use_ssim` (:227-243): True (SSIM), 2 (0.85 SSIM + 0.15 L1), any other truthy value (3x3 box of the
+  L1 difference).  The plain L1 difference of a falsy value is not implemented by the kernel and raises here too;
+* `not_center_cv` (:266-267): the fused volume as sum_f w_f sad_f / sum_f w_f instead of 1 - 2 x that.
 """
 import numpy as np
 import torch
@@ -81,21 +89,40 @@ def _ssim_error(x, y):
     return torch.clamp((1 - num / den) / 2, 0, 1)
 
 
+def _difference(use_ssim, warped, key, n, C, H, W):
+    """The per-pixel, per-channel difference of monorec_model.py:227-243, in its order of comparisons and operations.
+    warped (D, F, C, H, W), key (C, H, W); returns (D*F, C, H, W)."""
+    if use_ssim == True:  # noqa: E712  (the reference's comparison)
+        return _ssim_error(warped.reshape(n, C, H, W) + .5, key.expand(n, -1, -1, -1) + .5)
+    if use_ssim == 2:
+        d = _ssim_error(warped.reshape(n, C, H, W) + .5, key.expand(n, -1, -1, -1) + .5)
+        d = d.view(warped.shape)
+        return (0.85 * d + 0.15 * torch.abs(warped - key)).reshape(n, C, H, W)
+    return F.avg_pool2d(torch.abs(warped - key).reshape(n, C, H, W), kernel_size=3, stride=1, padding=1)
+
+
 @torch.no_grad()
 def cost_volume_torch(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, use_mono=True, use_stereo=False,
-                      patch_size=3, alpha=ALPHA, channel_weights=CHANNEL_WEIGHTS, return_valid=False):
-    """Restates CostVolumeModule.forward (use_ssim=True, sfcv_mult_mask=True, not_center_cv=False).
+                      patch_size=3, alpha=ALPHA, channel_weights=CHANNEL_WEIGHTS, return_valid=False,
+                      cv_depths=None, use_ssim=True, not_center_cv=False):
+    """Restates CostVolumeModule.forward (sfcv_mult_mask=True).  With `cv_depths` (B, D, H, W) the depths come from it
+    and D is its D; otherwise from the planes of (inv_depth_min, inv_depth_max, steps).
 
     Returns (cost_volume (B,D,H,W), [F x (B,D,H,W)] single-frame volumes[, valid (B,F,H,W)]).
     """
+    if not use_ssim:
+        raise NotImplementedError("use_ssim falsy")
     key = data["keyframe"]
     dtype = key.dtype
     frames, intrinsics, poses = collect_frames(data, use_mono, use_stereo)
     B, C, H, W = key.shape
     nF = len(frames)
-    D = int(steps)
+    if cv_depths is None:
+        D = int(steps)
+        z = plane_depths(inv_depth_min, inv_depth_max, D, dtype)        # (D,)
+    else:
+        D = cv_depths.shape[1]                                          # monorec_model.py:196
     border = patch_size // 2 + 1                                        # monorec_model.py:139
-    z = plane_depths(inv_depth_min, inv_depth_max, D, dtype)            # (D,)
     grid_px = _pixel_grid(H, W, dtype)                                  # (3, HW)
     inside = interior_mask(H, W, border, dtype)
     sad_w = (torch.tensor(channel_weights, dtype=dtype) / patch_size ** 2).view(1, C, 1, 1, 1) \
@@ -105,7 +132,8 @@ def cost_volume_torch(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, 
     for b in range(B):                                                  # monorec_model.py:193
         kinv = torch.inverse(data["keyframe_intrinsics"][b])[:3, :3]
         rays = kinv @ grid_px                                           # (3, HW)
-        pts = z.view(D, 1, 1) * rays.unsqueeze(0)                       # (D, 3, HW)   :199-200
+        depth = z.view(D, 1, 1) if cv_depths is None else cv_depths[b].to(dtype).reshape(D, 1, H * W)
+        pts = depth * rays.unsqueeze(0)                                 # (D, 3, HW)   :199-200
         pts = torch.cat([pts, torch.ones(D, 1, H * W, dtype=dtype)], 1)  # homogeneous :201
         warped, valid = [], []
         for f in range(nF):
@@ -123,7 +151,7 @@ def cost_volume_torch(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, 
         warped = torch.stack(warped, 1)                                 # (D, F, C, H, W)
         valid = torch.stack(valid)                                      # (F, 1, H, W)
         n = D * nF
-        err = _ssim_error(warped.reshape(n, C, H, W) + 0.5, key[b:b + 1].expand(n, -1, -1, -1) + 0.5)
+        err = _difference(use_ssim, warped, key[b], n, C, H, W)        # :227-243
         err = err.view(D, nF, C, H, W).permute(1, 2, 0, 3, 4)           # (F, C, D, H, W)
         sad = F.conv3d(err, sad_w, padding=(0, patch_size // 2, patch_size // 2)).squeeze(1)  # (F, D, H, W)
         sfcv = (1 - sad * 2) * valid                                    # :251
@@ -136,7 +164,8 @@ def cost_volume_torch(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, 
         den = wgt.sum(0).squeeze(0)                                     # (H, W)
         nz = den != 0
         cv = torch.zeros_like(num)
-        cv[:, nz] = 1 - 2 * (num[:, nz] / den[nz])                      # :266-269
+        fused = num[:, nz] / den[nz]                                    # :262-264
+        cv[:, nz] = fused if not_center_cv else 1 - 2 * fused           # :266-267
         out_cv.append(cv)
         out_valid.append(valid[:, 0])
     cost_volume = torch.stack(out_cv)
@@ -176,6 +205,20 @@ def _bilinear_zero(img, sx, sy):
     return out
 
 
+def _difference_closed_form(use_ssim, X, Y, mu_y, s_y, dtype):
+    """monorec_model.py:227-243 on X (D,C,H,W) and Y (C,H,W), with the key's box mean and variance.  The box of the L1
+    mode is a zero-padded 3x3 sum / 9 (avg_pool2d with its default count_include_pad); no valid pixel reads the padding."""
+    if use_ssim == True or use_ssim == 2:  # noqa: E712
+        mu_x = _box3(X) / dtype(9)
+        s_x = _box3(X * X) / dtype(9) - mu_x * mu_x
+        s_xy = _box3(X * Y[None]) / dtype(9) - mu_x * mu_y[None]
+        n_ = (2 * mu_x * mu_y[None] + dtype(SSIM_C1)) * (2 * s_xy + dtype(SSIM_C2))
+        d_ = (mu_x * mu_x + (mu_y * mu_y)[None] + dtype(SSIM_C1)) * (s_x + s_y[None] + dtype(SSIM_C2))
+        e = np.clip((1 - n_ / d_) / 2, 0, 1)
+        return e if use_ssim == True else dtype(0.85) * e + dtype(0.15) * np.abs(X - Y[None])  # noqa: E712
+    return _box3(np.abs(X - Y[None])) / dtype(9)
+
+
 def projection_tables(data, use_mono=True, use_stereo=False, dtype=np.float64):
     """proj[b,f] = (K_f . inv(pose_f) . pose_kf)[0:3, 0:4], kinv[b] = inv(K_kf)[0:3, 0:3]  (Appendix C)."""
     frames, intrinsics, poses = collect_frames(data, use_mono, use_stereo)
@@ -191,16 +234,29 @@ def projection_tables(data, use_mono=True, use_stereo=False, dtype=np.float64):
 
 
 def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, use_mono=True,
-                            use_stereo=False, alpha=ALPHA, channel_weights=CHANNEL_WEIGHTS, dtype=np.float32):
-    """Direct evaluation of the Appendix-C formulas.  Returns (cv, [sfcv_f], valid (B,F,H,W), sad (B,F,D,H,W))."""
+                            use_stereo=False, alpha=ALPHA, channel_weights=CHANNEL_WEIGHTS, dtype=np.float32,
+                            cv_depths=None, use_ssim=True, not_center_cv=False):
+    """Direct evaluation of the Appendix-C formulas, with the options of `cost_volume_torch`.  The positions are
+    evaluated in float64 (rounded to fp32 where dtype is float32), the rest in `dtype`.
+
+    Returns (cv, [sfcv_f], valid (B,F,H,W), sad (B,F,D,H,W)).
+    """
+    if not use_ssim:
+        raise NotImplementedError("use_ssim falsy")
     frames, _, _ = collect_frames(data, use_mono, use_stereo)
     key = data["keyframe"].numpy().astype(dtype)
     B, C, H, W = key.shape
-    nF, D = len(frames), int(steps)
+    if cv_depths is not None:
+        z = cv_depths.numpy().astype(np.float64)[:, :, None]                               # (B,D,1,H,W)
+    else:
+        D = int(steps)
+        if dtype == np.float32:
+            z = plane_depths(inv_depth_min, inv_depth_max, D).numpy().astype(np.float64)
+        else:
+            z = 1.0 / np.linspace(float(inv_depth_max), float(inv_depth_min), D, dtype=np.float64)
+        z = np.broadcast_to(z.reshape(1, D, 1, 1, 1), (B, D, 1, 1, 1))
+    nF, D = len(frames), z.shape[1]
     proj, kinv = projection_tables(data, use_mono, use_stereo, dtype=np.float64)
-    z = (1.0 / np.linspace(float(inv_depth_max), float(inv_depth_min), D, dtype=np.float64))
-    if dtype == np.float32:
-        z = plane_depths(inv_depth_min, inv_depth_max, D).numpy().astype(np.float64)
     vv, uu = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
     inside = np.zeros((H, W), dtype=bool)
     inside[2:H - 2, 2:W - 2] = True
@@ -221,10 +277,11 @@ def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, step
             img = frames[f][b].numpy().astype(dtype)
             P = proj[b, f]
             A = np.einsum("ij,jhw->ihw", P[:, :3], ray)                                    # (3,H,W)
-            c = A[None] * z[:, None, None, None] + P[:, 3][None, :, None, None]            # (D,3,H,W)
+            c = A[None] * z[b] + P[:, 3][None, :, None, None]                             # (D,3,H,W)
             c = c.astype(dtype).astype(np.float64) if dtype == np.float32 else c
-            px = c[:, 0] / (c[:, 2] + 1e-7)
-            py = c[:, 1] / (c[:, 2] + 1e-7)
+            with np.errstate(divide="ignore", invalid="ignore"):
+                px = c[:, 0] / (c[:, 2] + 1e-7)
+                py = c[:, 1] / (c[:, 2] + 1e-7)
             gx = np.clip((px / (W - 1) - 0.5) * 2, -2, 2)
             gy = np.clip((py / (H - 1) - 0.5) * 2, -2, 2)
             sx = ((gx + 1) * W - 1) / 2
@@ -234,13 +291,7 @@ def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, step
             X = _bilinear_zero(img, sx, sy) + dtype(0.5)                                   # (3,D,H,W)
             hit = _bilinear_zero(inside[None].astype(dtype), sx, sy)[0] != 0               # (D,H,W)
             valid = inside & hit.all(axis=0)
-            X = np.moveaxis(X, 0, 1)                                                       # (D,3,H,W)
-            mu_x = _box3(X) / dtype(9)
-            s_x = _box3(X * X) / dtype(9) - mu_x * mu_x
-            s_xy = _box3(X * Y[None]) / dtype(9) - mu_x * mu_y[None]
-            n_ = (2 * mu_x * mu_y[None] + dtype(SSIM_C1)) * (2 * s_xy + dtype(SSIM_C2))
-            d_ = (mu_x * mu_x + (mu_y * mu_y)[None] + dtype(SSIM_C1)) * (s_x + s_y[None] + dtype(SSIM_C2))
-            e = np.clip((1 - n_ / d_) / 2, 0, 1)
+            e = _difference_closed_form(use_ssim, np.moveaxis(X, 0, 1), Y, mu_y, s_y, dtype)   # (D,3,H,W)
             sad = _box3((e * cw).sum(axis=1)) / dtype(9)                                   # (D,H,W)
             sads[b, f] = sad
             valids[b, f] = valid
@@ -251,6 +302,6 @@ def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, step
             den += w
         nz = den != 0
         cv = np.zeros((D, H, W), dtype=dtype)
-        cv[:, nz] = 1 - 2 * num[:, nz] / den[nz]
+        cv[:, nz] = num[:, nz] / den[nz] if not_center_cv else 1 - 2 * num[:, nz] / den[nz]
         cvs[b] = cv
     return cvs, [sfs[f] for f in range(nF)], valids, sads

@@ -4,7 +4,7 @@
 
     MONOREC_REFERENCE=<path to the MonoRec checkout> python tests/golden/make_golden_cv_depths.py
 
-The inputs are rebuilt by tests/cv_depths_oracle.make_case (seeded images, depths evaluated in float64 numpy and rounded
+The inputs are rebuilt by tests/cv_cases.make_pixel_case (seeded images, depths evaluated in float64 numpy and rounded
 once to fp32), so only the reference's outputs are stored, in fp32:
   <tag>_cv, <tag>_sf      CostVolumeModule outputs for the cases band, shuffled and wide
   model_<gain>_cv_mask, model_<gain>_depth{1..4}
@@ -22,7 +22,7 @@ sys.path.insert(0, str(HERE.parent.parent))
 
 from make_golden import import_reference  # noqa: E402  (same shims, same reference import)
 from monorec_b200.synthetic import seeded_state_dict  # noqa: E402
-from tests.cv_depths_oracle import CASES, make_case  # noqa: E402
+from tests.cv_cases import PIXEL_CASES, make_pixel_case  # noqa: E402
 
 
 def main():
@@ -30,8 +30,8 @@ def main():
     torch.set_num_threads(8)
     ref_mod = import_reference()
     out = {}
-    for tag in CASES:
-        data, z = make_case(tag)
+    for tag in PIXEL_CASES:
+        data, z = make_pixel_case(tag)
         d = dict(data)
         d["cv_depths"] = z
         with torch.no_grad():
@@ -40,7 +40,7 @@ def main():
         out[f"{tag}_sf"] = np.stack([v.numpy() for v in d["single_frame_cvs"]])
         print(tag, "valid share per frame", [float(1 - (v == 0).all(1).float().mean()) for v in d["single_frame_cvs"]])
     for gain_tag, gain in (("g1", 1.0), ("g07", 0.7)):
-        data, z = make_case("model")
+        data, z = make_pixel_case("model")
         model = ref_mod.MonoRecModel()
         model.load_state_dict(seeded_state_dict(model, seed=7, gain=gain))
         model.eval()

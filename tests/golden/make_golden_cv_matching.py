@@ -4,9 +4,10 @@ options: use_ssim (model/monorec/monorec_model.py:227-243) and not_center_cv (:2
 
     MONOREC_REFERENCE=<path to the MonoRec checkout> python tests/golden/make_golden_cv_matching.py
 
-The inputs are rebuilt by tests/cv_matching_oracle.make_case (seeded images, the default planes or a band of per-pixel
+The inputs are rebuilt by tests/cv_cases.make_matching_case (seeded images, the default planes or a band of per-pixel
 depths), so only the reference's outputs are stored, in fp32:
-  <tag>_cv, <tag>_sf      CostVolumeModule(use_ssim=..., not_center_cv=...) outputs for the cases of cv_matching_oracle.CASES
+  <tag>_cv, <tag>_sf      CostVolumeModule(use_ssim=..., not_center_cv=...) outputs for the cases of
+                          cv_cases.MATCHING_CASES
   model_<gain>_cv_mask, model_<gain>_depth{1..3}
                           a full MonoRecModel(use_ssim=2) forward (seeded weights of model_synth_small.npz, gain 1 and 0.7)
                           on the default planes
@@ -22,7 +23,7 @@ sys.path.insert(0, str(HERE.parent.parent))
 
 from make_golden import import_reference  # noqa: E402  (same shims, same reference import)
 from monorec_b200.synthetic import make_inputs, seeded_state_dict  # noqa: E402
-from tests.cv_matching_oracle import CASES, MODEL_CASE, make_case, with_plane_range  # noqa: E402
+from tests.cv_cases import MATCHING_CASES, MATCHING_MODEL_CASE, make_matching_case, with_plane_range  # noqa: E402
 
 
 def main():
@@ -30,8 +31,8 @@ def main():
     torch.set_num_threads(8)
     ref_mod = import_reference()
     out = {}
-    for tag in CASES:
-        data, z, D, use_ssim, not_center = make_case(tag)
+    for tag in MATCHING_CASES:
+        data, z, D, use_ssim, not_center = make_matching_case(tag)
         d = with_plane_range(data, D)
         if z is not None:
             d["cv_depths"] = z
@@ -40,7 +41,7 @@ def main():
         out[f"{tag}_cv"] = d["cost_volume"].numpy()
         out[f"{tag}_sf"] = np.stack([v.numpy() for v in d["single_frame_cvs"]])
         print(tag, "valid share per frame", [float(1 - (v == 0).all(1).float().mean()) for v in d["single_frame_cvs"]])
-    B, nF, H, W, seed = MODEL_CASE
+    B, nF, H, W, seed = MATCHING_MODEL_CASE
     for gain_tag, gain in (("g1", 1.0), ("g07", 0.7)):
         model = ref_mod.MonoRecModel(use_ssim=2)
         model.load_state_dict(seeded_state_dict(model, seed=7, gain=gain))

@@ -10,8 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cv_depths_oracle as PO
-from tests import cv_matching_oracle as MO
+from tests import cv_cases as CC
 from tests.helpers import GOLDEN, kitti_sample_dict, synth_small_dict
 
 pytestmark = pytest.mark.gpu
@@ -81,7 +80,7 @@ def _unaligned(t):
 
 
 def fuse(sf, centered=True, alpha=10.0):
-    """The reference fusion (oracle/cost_volume_oracle.py:132-139, monorec_model.py:251-269) of single-frame volumes
+    """The reference fusion (oracle/cost_volume_oracle.py:160-168, monorec_model.py:251-269) of single-frame volumes
     sf [F,B,D,H,W] in fp32; a frame is invalid at a pixel whose plane stack is exactly 0.  Returns (cv, min weight of the
     valid frames per pixel)."""
     sf = sf.float()
@@ -132,8 +131,7 @@ def test_half_volumes_against_fp32_path(case):
     abi = _Abi(data, D)
     z = None
     if pix:
-        from tests.cv_depths_oracle import band_depths
-        z = band_depths(B, D, H, W, seed=91, rel=1.1).to(DEV)
+        z = CC.band_depths(B, D, H, W, seed=91, rel=1.1).to(DEV)
     frames = [_unaligned(f) for f in data["frames"]] if gather else None
     nhwc = torch.float16 if D <= 32 and D % 8 == 0 else None
     cv32, sf32, _ = abi.run(torch.float32, m, c, z=z, frames=frames)
@@ -263,21 +261,21 @@ def test_golden_kitti_sample():
                                atol=(1e-4 + HALF_ROUND) * H * W)
 
 
-@pytest.mark.parametrize("tag", list(MO.CASES))
+@pytest.mark.parametrize("tag", list(CC.MATCHING_CASES))
 def test_golden_matching_cases(tag):
     g = np.load(GOLDEN / "cv_matching.npz")
-    data, z, D, use_ssim, not_center = MO.make_case(tag)
+    data, z, D, use_ssim, not_center = CC.make_matching_case(tag)
     if z is None:
-        cv, sf = _run_module(MO.with_plane_range(data, D), D, use_ssim=use_ssim, not_center_cv=not_center)
+        cv, sf = _run_module(CC.with_plane_range(data, D), D, use_ssim=use_ssim, not_center_cv=not_center)
     else:
         cv, sf = _run_module(data, z=z, use_ssim=use_ssim, not_center_cv=not_center)
     print(tag, compare_half(cv, sf, torch.from_numpy(g[f"{tag}_cv"]), [torch.from_numpy(s) for s in g[f"{tag}_sf"]]))
 
 
-@pytest.mark.parametrize("tag", list(PO.CASES))
+@pytest.mark.parametrize("tag", list(CC.PIXEL_CASES))
 def test_golden_pixel_depth_cases(tag):
     g = np.load(GOLDEN / "cv_pixel_depths.npz")
-    data, z = PO.make_case(tag)
+    data, z = CC.make_pixel_case(tag)
     cv, sf = _run_module(data, z=z)
     print(tag, compare_half(cv, sf, torch.from_numpy(g[f"{tag}_cv"]), [torch.from_numpy(s) for s in g[f"{tag}_sf"]]))
 

@@ -11,7 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cv_matching_oracle as MO
+from oracle import cost_volume_oracle as O
+from tests import cv_cases as CC
 from tests.helpers import GOLDEN, compare_volumes
 
 gpu = pytest.mark.gpu
@@ -25,15 +26,15 @@ def _golden():
 
 def _depths(data, z, D):
     B, _, H, W = data["keyframe"].shape
-    return MO.plane_depths(B, D, H, W) if z is None else z
+    return CC.broadcast_planes(B, D, H, W) if z is None else z
 
 
 # ---- CPU --------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("tag", list(MO.CASES))
+@pytest.mark.parametrize("tag", list(CC.MATCHING_CASES))
 def test_torch_restatement_matches_reference(tag):
     g = _golden()
-    data, z, D, use_ssim, not_center = MO.make_case(tag)
-    cv, sf, _ = MO.cost_volume_torch(data, _depths(data, z, D), use_ssim=use_ssim, not_center_cv=not_center)
+    data, z, D, use_ssim, not_center = CC.make_matching_case(tag)
+    cv, sf = O.cost_volume_torch(data, cv_depths=_depths(data, z, D), use_ssim=use_ssim, not_center_cv=not_center)
     # the single-frame volumes at the tolerance of tests/test_oracle_golden.py; the fused volume at the north-star 1e-3, as
     # in tests/test_cv_pixel_depths.py (view weights of flat-cost pixels are differences of nearly equal numbers)
     assert (cv - torch.from_numpy(g[f"{tag}_cv"])).abs().max().item() <= 1e-3
@@ -41,12 +42,12 @@ def test_torch_restatement_matches_reference(tag):
         assert (a - torch.from_numpy(r)).abs().max().item() <= 5e-5
 
 
-@pytest.mark.parametrize("tag", list(MO.CASES))
+@pytest.mark.parametrize("tag", list(CC.MATCHING_CASES))
 def test_closed_form_matches_reference(tag):
     g = _golden()
-    data, z, D, use_ssim, not_center = MO.make_case(tag)
-    cv, sf, _ = MO.cost_volume_closed_form(data, _depths(data, z, D), use_ssim=use_ssim, not_center_cv=not_center,
-                                           dtype=np.float64)
+    data, z, D, use_ssim, not_center = CC.make_matching_case(tag)
+    cv, sf, _, _ = O.cost_volume_closed_form(data, cv_depths=_depths(data, z, D), use_ssim=use_ssim,
+                                             not_center_cv=not_center, dtype=np.float64)
     stats = compare_volumes(torch.from_numpy(cv).float(), [torch.from_numpy(s).float() for s in sf],
                             torch.from_numpy(g[f"{tag}_cv"]), [torch.from_numpy(s) for s in g[f"{tag}_sf"]])
     print(tag, stats)
@@ -102,7 +103,7 @@ def _to(data):
 
 def _module_run(data, D, z=None, nhwc=None, **kw):
     from monorec_b200.cost_volume import CostVolumeModule
-    d = MO.with_plane_range(data, D)
+    d = CC.with_plane_range(data, D)
     if z is not None:
         d["cv_depths"] = z
     if nhwc is not None:
@@ -165,10 +166,10 @@ class _Abi:
 
 
 @gpu
-@pytest.mark.parametrize("tag", list(MO.CASES))
+@pytest.mark.parametrize("tag", list(CC.MATCHING_CASES))
 def test_golden_cases(tag):
     g = _golden()
-    data, z, D, use_ssim, not_center = MO.make_case(tag)
+    data, z, D, use_ssim, not_center = CC.make_matching_case(tag)
     out = _module_run(_to(data), D, None if z is None else z.to(DEV), use_ssim=use_ssim, not_center_cv=not_center)
     stats = compare_volumes(out["cost_volume"].cpu(), [s.cpu() for s in out["single_frame_cvs"]],
                             torch.from_numpy(g[f"{tag}_cv"]), [torch.from_numpy(s) for s in g[f"{tag}_sf"]])
@@ -184,7 +185,7 @@ def test_golden_model(gain_tag, gain):
     from monorec_b200.synthetic import make_inputs, seeded_state_dict
     g = _golden()
     noise = np.load(GOLDEN / "model_fp64.npz")[f"synth_{gain_tag}_noise"]
-    B, nF, H, W, seed = MO.MODEL_CASE
+    B, nF, H, W, seed = CC.MATCHING_MODEL_CASE
     model = MonoRecModel(use_ssim=2)
     model.load_state_dict(seeded_state_dict(model, seed=7, gain=gain))
     model = model.to(DEV).eval()
@@ -224,8 +225,7 @@ def test_mode_properties(mode, centered):
     cvb, sfb, _ = abi.run(m, centered, z=abi.broadcast())
     assert torch.equal(cv, cvb) and torch.equal(sf, sfb), mode
     # a band of per-pixel depths on the TMA windows and on the gather (the per-pixel march of every mode, both paths)
-    from tests.cv_depths_oracle import band_depths
-    z = band_depths(B, D, H, W, seed=78, rel=1.1).to(DEV)
+    z = CC.band_depths(B, D, H, W, seed=78, rel=1.1).to(DEV)
     cvz, sfz, _ = abi.run(m, centered, z=z)
     cvzg, sfzg, _ = abi.run(m, centered, z=z, frames=[_unaligned(f) for f in data["frames"]])
     assert torch.isfinite(cvz).all() and (sfz != 0).any()
@@ -257,10 +257,9 @@ def test_mode_properties(mode, centered):
 def test_nhwc_copy(mode, dtype):
     """The MaskModule's NHWC copy equals the permuted single-frame volumes in every mode, on both depth sources."""
     from monorec_b200.synthetic import make_inputs
-    from tests.cv_depths_oracle import band_depths
     B, F, D, H, W = 2, 2, 32, 64, 128
     abi = _Abi(_to(make_inputs(B, F, H, W, seed=72)), D)
-    for z in (None, band_depths(B, D, H, W, seed=73).to(DEV)):
+    for z in (None, CC.band_depths(B, D, H, W, seed=73).to(DEV)):
         cv, sf, nh = abi.run(MODES[mode], 1, z=z, nhwc_dtype=dtype)
         ref = torch.cat([sf[f].permute(0, 2, 3, 1) for f in range(F)], 0).to(dtype)
         assert torch.equal(nh, ref), mode
@@ -284,7 +283,6 @@ def test_tall_image_on_both_paths(mode):
 @gpu
 def test_ssim_centred_equals_existing_entries():
     from monorec_b200.synthetic import make_inputs
-    from tests.cv_depths_oracle import band_depths
     B, F, D, H, W = 2, 3, 32, 96, 200
     abi = _Abi(_to(make_inputs(B, F, H, W, seed=75)), D)
     cv, sf, _ = abi.run(1, 1)
@@ -294,7 +292,7 @@ def test_ssim_centred_equals_existing_entries():
                                            abi.stream), "mr_cost_volume_fwd")
     torch.cuda.synchronize()
     assert torch.equal(cv, cv0) and torch.equal(sf, sf0)
-    z = band_depths(B, D, H, W, seed=76).to(DEV)
+    z = CC.band_depths(B, D, H, W, seed=76).to(DEV)
     cv, sf, _ = abi.run(1, 1, z=z)
     cv1, sf1, _ = abi.outputs()
     abi.L.check(abi.lib.mr_cost_volume_fwd_depthmap(abi.key.data_ptr(), abi.L.ptr_array(abi.data["frames"]),

@@ -10,7 +10,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests import cv_depths_oracle as PO
+from oracle import cost_volume_oracle as O
+from tests import cv_cases as CC
 from tests.helpers import GOLDEN, compare_volumes
 
 gpu = pytest.mark.gpu
@@ -22,11 +23,11 @@ def _golden():
 
 
 # ---- CPU --------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("tag", list(PO.CASES))
+@pytest.mark.parametrize("tag", list(CC.PIXEL_CASES))
 def test_torch_restatement_matches_reference(tag):
     g = _golden()
-    data, z = PO.make_case(tag)
-    cv, sf, _ = PO.cost_volume_torch(data, z)
+    data, z = CC.make_pixel_case(tag)
+    cv, sf = O.cost_volume_torch(data, cv_depths=z)
     # same primitives, same order as the reference: the single-frame volumes at the tolerance of tests/test_oracle_golden.py.
     # The fused volume of a band has pixels whose view weights are small differences of nearly equal numbers
     # (1 - (sum - 1) / (D - 1) with sum close to D), where a different summation order of the same terms moves it: by
@@ -36,11 +37,11 @@ def test_torch_restatement_matches_reference(tag):
         assert (a - torch.from_numpy(r)).abs().max().item() <= 5e-5
 
 
-@pytest.mark.parametrize("tag", list(PO.CASES))
+@pytest.mark.parametrize("tag", list(CC.PIXEL_CASES))
 def test_closed_form_matches_reference(tag):
     g = _golden()
-    data, z = PO.make_case(tag)
-    cv, sf, _ = PO.cost_volume_closed_form(data, z, dtype=np.float64)
+    data, z = CC.make_pixel_case(tag)
+    cv, sf, _, _ = O.cost_volume_closed_form(data, cv_depths=z, dtype=np.float64)
     stats = compare_volumes(torch.from_numpy(cv).float(), [torch.from_numpy(s).float() for s in sf],
                             torch.from_numpy(g[f"{tag}_cv"]), [torch.from_numpy(s) for s in g[f"{tag}_sf"]])
     print(tag, stats)
@@ -48,12 +49,23 @@ def test_closed_form_matches_reference(tag):
 
 def test_broadcast_planes_are_the_plane_oracle():
     """The default planes as a broadcast depth tensor are the reference's own default (monorec_model.py:184-185)."""
-    from oracle import cost_volume_oracle as O
     from monorec_b200.synthetic import make_inputs
     data = make_inputs(1, 2, 24, 40, seed=3)
     z = O.plane_depths(0.33, 0.0025, 8).view(1, 8, 1, 1).expand(1, 8, 24, 40)
-    cv, sf, _ = PO.cost_volume_torch(data, z)
+    cv, sf = O.cost_volume_torch(data, cv_depths=z)
     ref_cv, ref_sf = O.cost_volume_torch(data, steps=8)
+    assert torch.equal(cv, ref_cv) and all(torch.equal(a, b) for a, b in zip(sf, ref_sf))
+
+
+@pytest.mark.parametrize("not_center_cv", [False, True])
+@pytest.mark.parametrize("use_ssim", [True, 2, 3])
+def test_broadcast_planes_are_the_plane_oracle_in_every_mode(use_ssim, not_center_cv):
+    """The same for every error mode and centring: the depth source and the options are independent in the oracle."""
+    from monorec_b200.synthetic import make_inputs
+    data = make_inputs(1, 2, 24, 40, seed=3)
+    kw = dict(use_ssim=use_ssim, not_center_cv=not_center_cv)
+    cv, sf = O.cost_volume_torch(data, cv_depths=CC.broadcast_planes(1, 8, 24, 40), **kw)
+    ref_cv, ref_sf = O.cost_volume_torch(data, steps=8, **kw)
     assert torch.equal(cv, ref_cv) and all(torch.equal(a, b) for a, b in zip(sf, ref_sf))
 
 
@@ -148,10 +160,10 @@ class _Abi:
 
 
 @gpu
-@pytest.mark.parametrize("tag", list(PO.CASES))
+@pytest.mark.parametrize("tag", list(CC.PIXEL_CASES))
 def test_golden_cases(tag):
     g = _golden()
-    data, z = PO.make_case(tag)
+    data, z = CC.make_pixel_case(tag)
     out = _module_run(_to(data), z.to(DEV))
     stats = compare_volumes(out["cost_volume"].cpu(), [s.cpu() for s in out["single_frame_cvs"]],
                             torch.from_numpy(g[f"{tag}_cv"]), [torch.from_numpy(s) for s in g[f"{tag}_sf"]])
@@ -167,7 +179,7 @@ def test_golden_model(gain_tag, gain):
     from monorec_b200.synthetic import seeded_state_dict
     g = _golden()
     noise = np.load(GOLDEN / "model_fp64.npz")[f"synth_{gain_tag}_noise"]
-    data, z = PO.make_case("model")
+    data, z = CC.make_pixel_case("model")
     model = MonoRecModel()
     model.load_state_dict(seeded_state_dict(model, seed=7, gain=gain))
     model = model.to(DEV).eval()
@@ -217,18 +229,17 @@ def _step_depths(B, D, H, W, z_near=2.0, z_far=30.0, rel=4.0):
 @gpu
 @pytest.mark.parametrize("kind", ["band", "shuffled", "step"])
 def test_against_closed_form(kind):
-    from oracle import cost_volume_oracle as O
     from monorec_b200.synthetic import make_inputs
     B, F, D, H, W = 1, 4, 32, 256, 512
     data = make_inputs(B, F, H, W, seed=100)
     if kind == "band":
-        z = PO.band_depths(B, D, H, W, seed=7, rel=2.0)
+        z = CC.band_depths(B, D, H, W, seed=7, rel=2.0)
     elif kind == "shuffled":
-        z = PO.shuffled_depths(B, D, H, W, seed=8)
+        z = CC.shuffled_depths(B, D, H, W, seed=8)
     else:
         z = _step_depths(B, D, H, W)
     out = _module_run(_to(data), z.to(DEV))
-    ref_cv, ref_sf, _ = PO.cost_volume_closed_form(data, z, dtype=np.float64)
+    ref_cv, ref_sf, _, _ = O.cost_volume_closed_form(data, cv_depths=z, dtype=np.float64)
     ref_cv = torch.from_numpy(ref_cv).float()
     ref_sf = [torch.from_numpy(s).float() for s in ref_sf]
     sf = [s.cpu() for s in out["single_frame_cvs"]]
@@ -257,7 +268,7 @@ def test_unusable_hypotheses_zero_their_pixels():
     B, F, D, H, W = 1, 2, 32, 64, 128
     data = _to(make_inputs(B, F, H, W, seed=12))
     abi = _Abi(data, D)
-    good = PO.band_depths(B, D, H, W, seed=9, rel=1.1).to(DEV)
+    good = CC.band_depths(B, D, H, W, seed=9, rel=1.1).to(DEV)
     bad = good.clone()
     spots = [(20, 30, 5, float("nan")), (40, 70, 0, float("inf")), (30, 100, 31, 0.0), (50, 15, 17, -1.0)]
     for y, x, d, v in spots:
@@ -279,7 +290,7 @@ def test_batch_elements_are_independent():
     from monorec_b200.synthetic import make_inputs
     B, F, D, H, W = 2, 3, 32, 96, 200
     abi = _Abi(_to(make_inputs(B, F, H, W, seed=13)), D)
-    z = PO.band_depths(B, D, H, W, seed=10).to(DEV)
+    z = CC.band_depths(B, D, H, W, seed=10).to(DEV)
     cv0, sf0, _ = abi.depthmap(z)
     z2 = z.clone()
     z2[1] = z2[1].flip(0) * 0.5

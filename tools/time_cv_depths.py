@@ -22,7 +22,7 @@ ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 from monorec_b200 import _lib  # noqa: E402
 from monorec_b200.synthetic import make_inputs, to_device  # noqa: E402
-from tests.cv_depths_oracle import band_depths  # noqa: E402
+from tests.cv_cases import band_depths  # noqa: E402
 
 
 def power_limit():
