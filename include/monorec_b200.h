@@ -279,15 +279,22 @@ long long mr_conv_workspace_bytes(const mr_conv_desc* desc);
 /* sizeof(mr_conv_desc) as compiled into the library (bindings check their mirror of the struct against it). */
 int mr_sizeof_conv_desc(void);
 
-/* NCHW [B,C,H,W] -> channel slice of an NHWC tensor [B,H,W,dst_c]; optional per-pixel multiplier
- * scale[b,h,w] applied as (1 - scale) (monorec_model.py:713: cost_volume * (1 - cv_mask)). */
-int mr_nchw_to_nhwc(const float* src, float* dst, int B, int C, int H, int W, int dst_c, int dst_coff,
+/* Layout, pooling and masking helpers.  Each tensor is stored as MR_DT_F32 (fp32) or MR_DT_F16 (IEEE half) as its dtype
+ * argument says; any other value gives MR_EINVAL before any CUDA call.  The layout change and the masking widen half values,
+ * compute in fp32 and round a half result once (so the half cost volumes of mr_cost_volume_fwd_typed go through them); the
+ * max-pools are exact in either type.
+ *
+ * mr_nchw_to_nhwc: NCHW src [B,C,H,W] (src_dtype) -> channel slice [dst_coff, dst_coff + C) of an NHWC tensor dst [B,H,W,dst_c]
+ *   (dst_dtype); optional per-pixel multiplier one_minus_scale[b,h,w] (fp32) applied as (1 - scale)
+ *   (monorec_model.py:713: cost_volume * (1 - cv_mask)). */
+int mr_nchw_to_nhwc(const void* src, int src_dtype, void* dst, int dst_dtype, int B, int C, int H, int W, int dst_c, int dst_coff,
                     const float* one_minus_scale, void* stream);
-/* The same with a half destination; the layout kernels below have _f16 twins for half NHWC tensors. */
-int mr_nchw_to_nhwc_f16(const float* src, void* dst, int B, int C, int H, int W, int dst_c, int dst_coff,
-                        const float* one_minus_scale, void* stream);
-int mr_maxpool2_nhwc_f16(const void* src, void* dst, int B, int H, int W, int C, void* stream);
-int mr_max_over_frames_f16(const void* src, void* dst, int F, long long n_per_frame, void* stream);
+/* mr_maxpool2_nhwc: nn.MaxPool2d(2) on NHWC (monorec_model.py:304-316): src [B,H,W,C] -> dst [B,H/2,W/2,C]; H and W even,
+ *   C % 4 == 0 (MR_DT_F32) or C % 8 == 0 (MR_DT_F16).
+ * mr_max_over_frames: element-wise max over the leading axis, dst[n] = max_f src[f*n_per_frame + n] (monorec_model.py:362-365);
+ *   n_per_frame % 4 == 0 (MR_DT_F32) or % 8 == 0 (MR_DT_F16). */
+int mr_maxpool2_nhwc(const void* src, void* dst, int dtype, int B, int H, int W, int C, void* stream);
+int mr_max_over_frames(const void* src, void* dst, int dtype, int F, long long n_per_frame, void* stream);
 /* One pass over an encoder level's output x [F*B,H,W,C] (MR_DT_F16: C % 8 == 0, MR_DT_F32: C % 4 == 0; H, W even) that writes both
  * consumers: pooled [F*B,H/2,W/2,C] = nn.MaxPool2d(2) (monorec_model.py:304-316) and frame_max [B,H,W,C] = the element-wise
  * max over the F frames (:362-365). */
@@ -298,35 +305,30 @@ int mr_pool_and_frame_max(const void* src, void* pooled, void* frame_max, int dt
 int mr_maxpool3s2_nhwc(const void* src, void* dst, int dtype, int B, int H, int W, int C, void* stream);
 /* dst[i] = (half) src[i] for n contiguous fp32 values (used for channels-last feature maps). */
 int mr_cast_f32_to_f16(const float* src, void* dst, long long n, void* stream);
-/* nn.MaxPool2d(2) on NHWC (monorec_model.py:304-316). H and W must be even. */
-int mr_maxpool2_nhwc(const float* src, float* dst, int B, int H, int W, int C, void* stream);
-/* Element-wise max over the leading axis: dst[n] = max_f src[f*n_per_frame + n]  (monorec_model.py:362-365). */
-int mr_max_over_frames(const float* src, float* dst, int F, long long n_per_frame, void* stream);
-/* out[b,d,p] = volume[b,d,p] * (1 - mask[b,p])   (monorec_model.py:713, NCHW volume [B,D,HW], mask [B,HW]). */
-int mr_mask_volume(const float* volume, const float* mask, float* out, int B, int D, int HW, void* stream);
-/* The half volumes of mr_cost_volume_fwd_typed (MR_DT_F16): mr_nchw_to_nhwc / mr_nchw_to_nhwc_f16 with a half source,
- * dst_dtype MR_DT_F32 or MR_DT_F16 (the product with 1 - scale in fp32 on the widened value, rounded once for a half
- * destination), and mr_mask_volume with half volume and out (fp32 product, rounded once); mask stays fp32. */
-int mr_nchw_f16_to_nhwc(const void* src, void* dst, int dst_dtype, int B, int C, int H, int W, int dst_c, int dst_coff,
-                        const float* one_minus_scale, void* stream);
-int mr_mask_volume_f16(const void* volume, const float* mask, void* out, int B, int D, int HW, void* stream);
+/* out[b,d,p] = volume[b,d,p] * (1 - mask[b,p])   (monorec_model.py:713, NCHW volume and out [B,D,HW] of type dtype, mask [B,HW]
+ * fp32). */
+int mr_mask_volume(const void* volume, const float* mask, void* out, int dtype, int B, int D, int HW, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Evaluation-side helpers (SURVEY.md section 8f row 2).
  *
  * mr_sparse_metrics: the seven sparse depth metrics of model/metric_functions/sparse_metrics.py:81-251 (a1, a2, a3, rmse,
  * rmse_log, abs_rel, sq_rel with utils/util.py:36-65, :101-118) in one pass; evaluater/evaluater.py:78-112 calls the seven
- * reference functions (~12 elementwise torch kernels each) one after the other.
+ * reference functions (~12 elementwise torch kernels each) one after the other.  The pass covers G = ceil(B / group)
+ * consecutive groups of `group` images at once (the last group may be shorter; group = B gives one row for the whole batch):
+ * row g of out_metrics holds the metrics of images [g * group, min(B, (g + 1) * group)), so that the evaluater's batches of
+ * a run of key frames take one launch pair.
  *   result, target   [B,1,H,W] predicted / ground-truth INVERSE depth (target 0 = no measurement)
+ *   group            >= 1 images per row
  *   mvobj_mask       [B,1,H,W] or NULL: with it, pixels whose mask is <= 0.5 are excluded (the *_onlydynamic variants)
  *   roi              host int[4] {r0, r1, c0, c1} (python slice semantics) or NULL; max_distance <= 0: no clamp
  *   pred_all_valid   0: pixels with result == 0 are excluded (the *_onlyvalid variants)
- *   out_metrics      device float[7]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel; no host synchronisation
+ *   out_metrics      device float[G][7]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel; no host synchronisation
  *   workspace        device buffer of mr_sparse_metrics_workspace(B) bytes, 8-byte aligned
  * mr_images_u8_to_f32: uint8 HWC images [B,Hs,Ws,3] -> float CHW [B,3,H,W] = u / 255 - 0.5 of the crop starting at
  * (crop_top, crop_left) (data_loader/kitti_odometry_dataset.py:121-132 without the PIL resize). */
 long long mr_sparse_metrics_workspace(int B);
-int mr_sparse_metrics(const float* result, const float* target, const float* mvobj_mask, int B, int H, int W,
+int mr_sparse_metrics(const float* result, const float* target, const float* mvobj_mask, int B, int group, int H, int W,
                       const int* roi, float max_distance, int pred_all_valid, float* out_metrics,
                       void* workspace, long long workspace_bytes, void* stream);
 int mr_images_u8_to_f32(const unsigned char* src, float* dst, int B, int Hs, int Ws, int crop_top, int crop_left,
@@ -334,12 +336,12 @@ int mr_images_u8_to_f32(const unsigned char* src, float* dst, int B, int Hs, int
 /* mr_dense_metrics: the twelve dense-ground-truth metrics of model/metric_functions/ in one pass: the seven *_metric functions of
  * sparse_metrics.py:6-78, sc_inv / l1_rel / l1_inv of dense_metrics.py and completeness / covered_gt of
  * completeness_metrics.py.  There is no validity mask: every pixel of the region of interest counts, and a zero depth gives
- * the reference's IEEE outcome (inf / NaN values, a miss in a1-a3).
+ * the reference's IEEE outcome (inf / NaN values, a miss in a1-a3).  Rows of `group` images as in mr_sparse_metrics.
  *   result, target   [B,1,H,W] predicted / ground-truth inverse depth
  *   roi              host int[4] {r0, r1, c0, c1} (python slice semantics) or NULL (completeness and covered_gt ignore it)
  *   min_inv_depth    > 0: inverse depths are clamped from below to it before inverting (1 / max_distance, as the reference's
  *                    `max_distance is not None` branch computes it); <= 0: no clamp
- *   out_metrics      device float[12]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel, sc_inv, l1_rel, l1_inv, completeness,
+ *   out_metrics      device float[G][12]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel, sc_inv, l1_rel, l1_inv, completeness,
  *                    covered_gt; no host synchronisation
  *   workspace        device buffer of mr_dense_metrics_workspace(B) bytes, 8-byte aligned
  * mr_median_scaling: the evaluater's median scaling (utils/util.py:135-142): out[b] = result[b] * (median(target[b][m]) /
@@ -348,26 +350,17 @@ int mr_images_u8_to_f32(const unsigned char* src, float* dst, int B, int Hs, int
  *   [B,1,H,W], out must not alias result; workspace: device buffer of mr_median_scaling_workspace(B,H,W) bytes, 4-byte
  *   aligned.  No host synchronisation. */
 long long mr_dense_metrics_workspace(int B);
-int mr_dense_metrics(const float* result, const float* target, int B, int H, int W, const int* roi, float min_inv_depth,
-                     float* out_metrics, void* workspace, long long workspace_bytes, void* stream);
+int mr_dense_metrics(const float* result, const float* target, int B, int group, int H, int W, const int* roi,
+                     float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes, void* stream);
 long long mr_median_scaling_workspace(int B, int H, int W);
 int mr_median_scaling(const float* result, const float* target, float* out, int B, int H, int W, void* workspace,
                       long long workspace_bytes, void* stream);
-/* mr_sparse_metrics_grouped / mr_dense_metrics_grouped: the same passes over G = ceil(B / group) consecutive groups of `group`
- * images (the last group may be shorter), one row per group: out_metrics is device float[G][7] / [G][12], and row g is what
- * mr_sparse_metrics / mr_dense_metrics return for images [g * group, min(B, (g + 1) * group)) -- the evaluater's batches of
- * a run of key frames in one launch pair.  mr_sparse_metrics / mr_dense_metrics are the case group = B.  Same workspace.
- * mr_eval_accumulate: the evaluater's bookkeeping (evaluater/evaluater.py:45-49, 94-103) on the device, in its float64
+/* mr_eval_accumulate: the evaluater's bookkeeping (evaluater/evaluater.py:45-49, 94-103) on the device, in its float64
  * operation order.  values: device float[G][M], the M metrics of G batches in batch order; group_sizes: host int[G], the
  * images per batch; state: device double[3M + 1] = total[M], valid[M], running_avg[M], num_samples, zero at the start of an
  * evaluation.  Per batch: a row holding a NaN adds zeros to total and running_avg and 0 to valid (else the widened values
  * and 1); the first batch (num_samples == 0) is added to running_avg, a later one of b images sets it to
  * avg * (n / (n + b)) + m * (b / (n + b)); then num_samples += b.  1 <= M <= 1024.  No host synchronisation. */
-int mr_sparse_metrics_grouped(const float* result, const float* target, const float* mvobj_mask, int B, int group, int H, int W,
-                              const int* roi, float max_distance, int pred_all_valid, float* out_metrics,
-                              void* workspace, long long workspace_bytes, void* stream);
-int mr_dense_metrics_grouped(const float* result, const float* target, int B, int group, int H, int W, const int* roi,
-                             float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes, void* stream);
 int mr_eval_accumulate(const float* values, int G, int M, const int* group_sizes, double* state, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------

@@ -54,28 +54,22 @@ SIGNATURES = {
     "mr_conv2d_nhwc_tc": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p]),
     "mr_conv2d_nhwc_tc_phases": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "mr_conv2d_nhwc_tc_plan": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p]),
-    "mr_nchw_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "mr_nchw_to_nhwc_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "mr_maxpool2_nhwc_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "mr_max_over_frames_f16": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p]),
+    "mr_nchw_to_nhwc": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "mr_maxpool2_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "mr_max_over_frames": (c_int, [c_void_p, c_void_p, c_int, c_int, c_longlong, c_void_p]),
     "mr_pool_and_frame_max": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mr_maxpool3s2_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mr_cast_f32_to_f16": (c_int, [c_void_p, c_void_p, c_longlong, c_void_p]),
-    "mr_maxpool2_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
-    "mr_max_over_frames": (c_int, [c_void_p, c_void_p, c_int, c_longlong, c_void_p]),
+    "mr_mask_volume": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "mr_sparse_metrics_workspace": (c_longlong, [c_int]),
-    "mr_sparse_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int), c_float, c_int, c_void_p,
-                                  c_void_p, c_longlong, c_void_p]),
+    "mr_sparse_metrics": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_float, c_int,
+                                  c_void_p, c_void_p, c_longlong, c_void_p]),
     "mr_images_u8_to_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "mr_dense_metrics_workspace": (c_longlong, [c_int]),
-    "mr_dense_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_int), c_float, c_void_p, c_void_p, c_longlong,
-                                 c_void_p]),
+    "mr_dense_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_float, c_void_p, c_void_p,
+                                 c_longlong, c_void_p]),
     "mr_median_scaling_workspace": (c_longlong, [c_int, c_int, c_int]),
     "mr_median_scaling": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_longlong, c_void_p]),
-    "mr_sparse_metrics_grouped": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_float,
-                                          c_int, c_void_p, c_void_p, c_longlong, c_void_p]),
-    "mr_dense_metrics_grouped": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_int), c_float, c_void_p,
-                                         c_void_p, c_longlong, c_void_p]),
     "mr_eval_accumulate": (c_int, [c_void_p, c_int, c_int, POINTER(c_int), c_void_p, c_void_p]),
     "mr_pointcloud_keep_mask": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "mr_pointcloud_workspace": (c_longlong, [c_int, c_int, c_int]),
@@ -89,9 +83,6 @@ SIGNATURES = {
                                          c_void_p, c_void_p, c_void_p]),
     "mr_reprojection_loss_bwd": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                          c_int, c_void_p, c_void_p]),
-    "mr_mask_volume": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "mr_mask_volume_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
-    "mr_nchw_f16_to_nhwc": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
 }
 
 

@@ -131,12 +131,13 @@ def conv2d(srcs, weight, bias, kh, kw, stride=(1, 1), act=ACT_NONE, act_a=0.0, a
 
 
 def nchw_to_nhwc(x, out=None, out_coff=0, one_minus=None, dtype=None):
-    """fp32 or half (B,C,H,W) -> NHWC fp32 / half (optionally into a channel slice of `out`, optionally scaled by
-    (1 - one_minus[b,0,h,w])).  A half source (the half cost volumes) is widened in the kernel."""
+    """(B,C,H,W) -> NHWC fp32 / half (optionally into a channel slice of `out`, optionally scaled by (1 - one_minus[b,0,h,w])).
+    A half source (the half cost volumes) is widened in the kernel; a source of any other type than fp32 or half is widened to
+    fp32 first."""
     lib = _lib.load()
     dtype = (out.dtype if out is not None else dtype) or torch.float32
-    if x.dtype == torch.float16:
-        return _nchw_f16_to_nhwc(lib, x, out, out_coff, one_minus, dtype)
+    if x.dtype != torch.float16:
+        x = x.to(torch.float32)
     if out is None and one_minus is None and x.dim() == 4 and x.dtype == torch.float32 and x.permute(0, 2, 3, 1).is_contiguous():
         v = x.permute(0, 2, 3, 1)             # already channels-last in memory (e.g. cuDNN NHWC output): a view, no kernel
         if dtype == torch.float32:
@@ -153,31 +154,10 @@ def nchw_to_nhwc(x, out=None, out_coff=0, one_minus=None, dtype=None):
     if one_minus is not None:    # the kernel reads fp32 [B,1,H,W]: any other dtype / shape would be read out of bounds
         om_t = one_minus.to(device=x.device, dtype=torch.float32).contiguous()
         assert om_t.numel() == B * H * W, f"one_minus must hold one value per pixel (B,1,H,W), got {tuple(one_minus.shape)}"
-    fn, name = (lib.mr_nchw_to_nhwc_f16, "mr_nchw_to_nhwc_f16") if out.dtype == torch.float16 else (lib.mr_nchw_to_nhwc, "mr_nchw_to_nhwc")
     with torch.cuda.device(x.device):
-        _lib.check(fn(x.data_ptr(), out.data_ptr(), B, C, H, W, out.shape[3], out_coff,
-                      om_t.data_ptr() if om_t is not None else None, _stream(x)), name)
+        _lib.check(lib.mr_nchw_to_nhwc(x.data_ptr(), _dt(x), out.data_ptr(), _dt(out), B, C, H, W, out.shape[3], out_coff,
+                                       om_t.data_ptr() if om_t is not None else None, _stream(x)), "mr_nchw_to_nhwc")
     return out        # (om_t stays referenced until the launch has been queued; the caching allocator is stream-ordered)
-
-
-def _one_minus_f32(one_minus, x):
-    """The kernels read fp32 [B,1,H,W]: any other dtype / shape would be read out of bounds."""
-    om_t = one_minus.to(device=x.device, dtype=torch.float32).contiguous()
-    assert om_t.numel() == x.shape[0] * x.shape[2] * x.shape[3], \
-        f"one_minus must hold one value per pixel (B,1,H,W), got {tuple(one_minus.shape)}"
-    return om_t
-
-
-def _nchw_f16_to_nhwc(lib, x, out, out_coff, one_minus, dtype):
-    x = x.contiguous()
-    B, C, H, W = x.shape
-    if out is None:
-        out = torch.empty(B, H, W, C, device=x.device, dtype=dtype)
-    om_t = None if one_minus is None else _one_minus_f32(one_minus, x)
-    with torch.cuda.device(x.device):
-        _lib.check(lib.mr_nchw_f16_to_nhwc(x.data_ptr(), out.data_ptr(), _dt(out), B, C, H, W, out.shape[3], out_coff,
-                                           om_t.data_ptr() if om_t is not None else None, _stream(x)), "mr_nchw_f16_to_nhwc")
-    return out
 
 
 def as_nhwc(x, dtype):
@@ -192,9 +172,8 @@ def maxpool2(x):
     lib = _lib.load()
     B, H, W, C = x.shape
     out = torch.empty(B, H // 2, W // 2, C, device=x.device, dtype=x.dtype)
-    fn, name = (lib.mr_maxpool2_nhwc_f16, "mr_maxpool2_nhwc_f16") if x.dtype == torch.float16 else (lib.mr_maxpool2_nhwc, "mr_maxpool2_nhwc")
     with torch.cuda.device(x.device):
-        _lib.check(fn(x.data_ptr(), out.data_ptr(), B, H, W, C, _stream(x)), name)
+        _lib.check(lib.mr_maxpool2_nhwc(x.data_ptr(), out.data_ptr(), _dt(x), B, H, W, C, _stream(x)), "mr_maxpool2_nhwc")
     return out
 
 
@@ -205,9 +184,8 @@ def max_over_frames(x, frames):
     lib = _lib.load()
     B = x.shape[0] // frames
     out = torch.empty((B,) + tuple(x.shape[1:]), device=x.device, dtype=x.dtype)
-    fn, name = (lib.mr_max_over_frames_f16, "mr_max_over_frames_f16") if x.dtype == torch.float16 else (lib.mr_max_over_frames, "mr_max_over_frames")
     with torch.cuda.device(x.device):
-        _lib.check(fn(x.data_ptr(), out.data_ptr(), frames, out.numel(), _stream(x)), name)
+        _lib.check(lib.mr_max_over_frames(x.data_ptr(), out.data_ptr(), _dt(x), frames, out.numel(), _stream(x)), "mr_max_over_frames")
     return out
 
 
@@ -251,9 +229,9 @@ def mask_volume_impl(volume: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
     mask = mask.to(torch.float32).contiguous()
     B, D, H, W = volume.shape
     out = torch.empty_like(volume)
-    fn, name = (lib.mr_mask_volume_f16, "mr_mask_volume_f16") if volume.dtype == torch.float16 else (lib.mr_mask_volume, "mr_mask_volume")
     with torch.cuda.device(volume.device):
-        _lib.check(fn(volume.data_ptr(), mask.data_ptr(), out.data_ptr(), B, D, H * W, _stream(volume)), name)
+        _lib.check(lib.mr_mask_volume(volume.data_ptr(), mask.data_ptr(), out.data_ptr(), _dt(volume), B, D, H * W, _stream(volume)),
+                   "mr_mask_volume")
     return out
 
 

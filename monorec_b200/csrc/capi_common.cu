@@ -18,7 +18,7 @@ void count_launch(int n) { g_launches += n; }
 
 }  // namespace mr
 
-extern "C" int mr_version(void) { return (0 << 16) | (2 << 8) | 0; }
+extern "C" int mr_version(void) { return (0 << 16) | (3 << 8) | 0; }
 
 extern "C" const char* mr_last_error(void) { return mr::g_err; }
 

@@ -186,7 +186,7 @@ __device__ __forceinline__ void st1(__half* p, float v) { *p = __float2half_rn(v
 __device__ __forceinline__ float ld1(const float* p) { return __ldg(p); }
 __device__ __forceinline__ float ld1(const __half* p) { return __half2float(__ldg(p)); }
 
-template <typename T, typename S = float>
+template <typename T, typename S>
 __global__ void nchw_to_nhwc_kernel(const S* __restrict__ src, T* __restrict__ dst, int C, int HW, int dst_c,
                                     int dst_coff, const float* __restrict__ oms) {
     // one CTA: 32 pixels x 32 channels tile transposed through shared memory (coalesced on both sides)
@@ -211,7 +211,7 @@ __global__ void nchw_to_nhwc_kernel(const S* __restrict__ src, T* __restrict__ d
 // Half-precision fast path of the layout change (C % 32 == 0, HW % 128 == 0, 16-byte aligned channel slice): a CTA moves
 // 32 channels x 128 pixels; 128-byte coalesced reads per channel row, conflict-free shared-memory transpose (pitch 129),
 // one 16-byte store (8 channels) per thread so that a warp writes 8 pixels x 64 contiguous bytes.
-template <typename S = float>
+template <typename S>
 __global__ void __launch_bounds__(256)
 nchw_to_nhwc_f16_tile_kernel(const S* __restrict__ src, __half* __restrict__ dst, int C, int HW, int dst_c, int dst_coff,
                              const float* __restrict__ oms) {
@@ -241,38 +241,7 @@ nchw_to_nhwc_f16_tile_kernel(const S* __restrict__ src, __half* __restrict__ dst
     }
 }
 
-__global__ void maxpool2_nhwc_kernel(const float4* __restrict__ src, float4* __restrict__ dst, int H, int W, int C4,
-                                     size_t total) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    const int Wo = W / 2, Ho = H / 2;
-    const int c = (int)(i % C4);
-    size_t r = i / C4;
-    const int x = (int)(r % Wo); r /= Wo;
-    const int y = (int)(r % Ho);
-    const size_t b = r / Ho;
-    const float4* p = src + ((b * H + 2 * y) * W + 2 * x) * C4 + c;
-    const float4 a = __ldg(p), bq = __ldg(p + C4), cq = __ldg(p + (size_t)W * C4), dq = __ldg(p + (size_t)W * C4 + C4);
-    float4 o;
-    o.x = fmaxf(fmaxf(a.x, bq.x), fmaxf(cq.x, dq.x));
-    o.y = fmaxf(fmaxf(a.y, bq.y), fmaxf(cq.y, dq.y));
-    o.z = fmaxf(fmaxf(a.z, bq.z), fmaxf(cq.z, dq.z));
-    o.w = fmaxf(fmaxf(a.w, bq.w), fmaxf(cq.w, dq.w));
-    dst[i] = o;
-}
-
-__global__ void max_over_frames_kernel(const float4* __restrict__ src, float4* __restrict__ dst, int F, size_t n4) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n4) return;
-    float4 m = __ldg(src + i);
-    for (int f = 1; f < F; ++f) {
-        const float4 v = __ldg(src + (size_t)f * n4 + i);
-        m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
-    }
-    dst[i] = m;
-}
-
-template <typename T = float>
+template <typename T>
 __global__ void mask_volume_kernel(const T* __restrict__ vol, const float* __restrict__ mask,
                                    T* __restrict__ out, int D, int HW, size_t total) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -282,22 +251,40 @@ __global__ void mask_volume_kernel(const T* __restrict__ vol, const float* __res
     st1(out + i, (1.0f - __ldg(mask + b * HW + p)) * ld1(vol + i));
 }
 
-}  // namespace
-
-extern "C" int mr_mask_volume(const float* volume, const float* mask, float* out, int B, int D, int HW, void* stream) {
-    MR_REQUIRE(volume && mask && out && B >= 1 && D >= 1 && HW >= 1, "mr_mask_volume: bad argument");
-    const size_t total = (size_t)B * D * HW;
-    mask_volume_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(volume, mask, out, D, HW,
-                                                                                          total);
-    MR_LAUNCH_CHECK("mask_volume_kernel");
+// the layout change for a source of type S: the half tile kernel when the destination is half and the slice is aligned for
+// its 16-byte stores, else the generic kernel
+template <typename S>
+int nchw_to_nhwc_launch(const S* src, void* dst, int dst_dtype, int B, int C, int HW, int dst_c, int dst_coff, const float* oms,
+                        cudaStream_t st) {
+    if (dst_dtype == MR_DT_F16 && C % 32 == 0 && HW % 128 == 0 && dst_c % 8 == 0 && dst_coff % 8 == 0 &&
+        (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+        dim3 tgrid(HW / 128, C / 32, B);
+        nchw_to_nhwc_f16_tile_kernel<S><<<tgrid, 256, 0, st>>>(src, static_cast<__half*>(dst), C, HW, dst_c, dst_coff, oms);
+        MR_LAUNCH_CHECK("nchw_to_nhwc_f16_tile_kernel");
+        return MR_OK;
+    }
+    dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
+    if (dst_dtype == MR_DT_F16)
+        nchw_to_nhwc_kernel<__half, S><<<grid, block, 0, st>>>(src, static_cast<__half*>(dst), C, HW, dst_c, dst_coff, oms);
+    else
+        nchw_to_nhwc_kernel<float, S><<<grid, block, 0, st>>>(src, static_cast<float*>(dst), C, HW, dst_c, dst_coff, oms);
+    MR_LAUNCH_CHECK("nchw_to_nhwc_kernel");
     return MR_OK;
 }
 
-extern "C" int mr_mask_volume_f16(const void* volume, const float* mask, void* out, int B, int D, int HW, void* stream) {
-    MR_REQUIRE(volume && mask && out && B >= 1 && D >= 1 && HW >= 1, "mr_mask_volume_f16: bad argument");
+}  // namespace
+
+extern "C" int mr_mask_volume(const void* volume, const float* mask, void* out, int dtype, int B, int D, int HW, void* stream) {
+    MR_REQUIRE(dtype == MR_DT_F32 || dtype == MR_DT_F16, "mr_mask_volume: dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", dtype);
+    MR_REQUIRE(volume && mask && out && B >= 1 && D >= 1 && HW >= 1, "mr_mask_volume: bad argument");
     const size_t total = (size_t)B * D * HW;
-    mask_volume_kernel<__half><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        static_cast<const __half*>(volume), mask, static_cast<__half*>(out), D, HW, total);
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (dtype == MR_DT_F16)
+        mask_volume_kernel<__half><<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const __half*>(volume), mask,
+                                                                           static_cast<__half*>(out), D, HW, total);
+    else
+        mask_volume_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const float*>(volume), mask,
+                                                                          static_cast<float*>(out), D, HW, total);
     MR_LAUNCH_CHECK("mask_volume_kernel");
     return MR_OK;
 }
@@ -347,102 +334,23 @@ extern "C" int mr_conv2d_nhwc(const mr_conv_desc* desc, void* stream) {
     return MR_OK;
 }
 
-extern "C" int mr_nchw_to_nhwc(const float* src, float* dst, int B, int C, int H, int W, int dst_c, int dst_coff,
-                               const float* one_minus_scale, void* stream) {
+extern "C" int mr_nchw_to_nhwc(const void* src, int src_dtype, void* dst, int dst_dtype, int B, int C, int H, int W, int dst_c,
+                               int dst_coff, const float* one_minus_scale, void* stream) {
+    MR_REQUIRE(src_dtype == MR_DT_F32 || src_dtype == MR_DT_F16, "mr_nchw_to_nhwc: src_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)",
+               src_dtype);
+    MR_REQUIRE(dst_dtype == MR_DT_F32 || dst_dtype == MR_DT_F16, "mr_nchw_to_nhwc: dst_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)",
+               dst_dtype);
     MR_REQUIRE(src && dst && B >= 1 && C >= 1 && H >= 1 && W >= 1, "mr_nchw_to_nhwc: bad argument");
     MR_REQUIRE(dst_coff >= 0 && dst_coff + C <= dst_c, "mr_nchw_to_nhwc: channel slice out of range");
-    const int HW = H * W;
-    dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
-    nchw_to_nhwc_kernel<float><<<grid, block, 0, (cudaStream_t)stream>>>(src, dst, C, HW, dst_c, dst_coff, one_minus_scale);
-    MR_LAUNCH_CHECK("nchw_to_nhwc_kernel");
-    return MR_OK;
-}
-
-extern "C" int mr_nchw_to_nhwc_f16(const float* src, void* dst, int B, int C, int H, int W, int dst_c, int dst_coff,
-                                   const float* one_minus_scale, void* stream) {
-    MR_REQUIRE(src && dst && B >= 1 && C >= 1 && H >= 1 && W >= 1, "mr_nchw_to_nhwc_f16: bad argument");
-    MR_REQUIRE(dst_coff >= 0 && dst_coff + C <= dst_c, "mr_nchw_to_nhwc_f16: channel slice out of range");
-    const int HW = H * W;
-    if (C % 32 == 0 && HW % 128 == 0 && dst_c % 8 == 0 && dst_coff % 8 == 0 && (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-        dim3 tgrid(HW / 128, C / 32, B);
-        nchw_to_nhwc_f16_tile_kernel<<<tgrid, 256, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c, dst_coff,
-                                                                           one_minus_scale);
-        MR_LAUNCH_CHECK("nchw_to_nhwc_f16_tile_kernel");
-        return MR_OK;
-    }
-    dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
-    nchw_to_nhwc_kernel<__half><<<grid, block, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c, dst_coff,
-                                                                          one_minus_scale);
-    MR_LAUNCH_CHECK("nchw_to_nhwc_kernel");
-    return MR_OK;
-}
-
-extern "C" int mr_nchw_f16_to_nhwc(const void* src_, void* dst, int dst_dtype, int B, int C, int H, int W, int dst_c,
-                                   int dst_coff, const float* one_minus_scale, void* stream) {
-    MR_REQUIRE(src_ && dst && B >= 1 && C >= 1 && H >= 1 && W >= 1, "mr_nchw_f16_to_nhwc: bad argument");
-    MR_REQUIRE(dst_dtype == MR_DT_F32 || dst_dtype == MR_DT_F16, "mr_nchw_f16_to_nhwc: dst_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)",
-               dst_dtype);
-    MR_REQUIRE(dst_coff >= 0 && dst_coff + C <= dst_c, "mr_nchw_f16_to_nhwc: channel slice out of range");
-    const __half* src = static_cast<const __half*>(src_);
-    const int HW = H * W;
-    if (dst_dtype == MR_DT_F16 && C % 32 == 0 && HW % 128 == 0 && dst_c % 8 == 0 && dst_coff % 8 == 0 &&
-        (reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-        dim3 tgrid(HW / 128, C / 32, B);
-        nchw_to_nhwc_f16_tile_kernel<__half><<<tgrid, 256, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c,
-                                                                                   dst_coff, one_minus_scale);
-        MR_LAUNCH_CHECK("nchw_to_nhwc_f16_tile_kernel");
-        return MR_OK;
-    }
-    dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
-    if (dst_dtype == MR_DT_F16)
-        nchw_to_nhwc_kernel<__half, __half><<<grid, block, 0, (cudaStream_t)stream>>>(src, static_cast<__half*>(dst), C, HW, dst_c,
-                                                                                      dst_coff, one_minus_scale);
-    else
-        nchw_to_nhwc_kernel<float, __half><<<grid, block, 0, (cudaStream_t)stream>>>(src, static_cast<float*>(dst), C, HW, dst_c,
-                                                                                     dst_coff, one_minus_scale);
-    MR_LAUNCH_CHECK("nchw_to_nhwc_kernel");
-    return MR_OK;
+    if (src_dtype == MR_DT_F16)
+        return nchw_to_nhwc_launch(static_cast<const __half*>(src), dst, dst_dtype, B, C, H * W, dst_c, dst_coff, one_minus_scale,
+                                   (cudaStream_t)stream);
+    return nchw_to_nhwc_launch(static_cast<const float*>(src), dst, dst_dtype, B, C, H * W, dst_c, dst_coff, one_minus_scale,
+                               (cudaStream_t)stream);
 }
 
 namespace {
-// half NHWC twins of the pooling kernels: 8 channels (16 bytes) per thread
-__global__ void maxpool2_nhwc_f16_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int H, int W, int C8, size_t total) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    const int Wo = W / 2, Ho = H / 2;
-    const int c = (int)(i % C8);
-    size_t r = i / C8;
-    const int x = (int)(r % Wo); r /= Wo;
-    const int y = (int)(r % Ho);
-    const size_t b = r / Ho;
-    const uint4* p = src + ((b * H + 2 * y) * W + 2 * x) * C8 + c;
-    uint4 q[4] = {__ldg(p), __ldg(p + C8), __ldg(p + (size_t)W * C8), __ldg(p + (size_t)W * C8 + C8)};
-    uint4 o;
-    __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const __half2 a = reinterpret_cast<const __half2*>(&q[0])[k], bq = reinterpret_cast<const __half2*>(&q[1])[k];
-        const __half2 cq = reinterpret_cast<const __half2*>(&q[2])[k], dq = reinterpret_cast<const __half2*>(&q[3])[k];
-        oh[k] = __hmax2(__hmax2(a, bq), __hmax2(cq, dq));
-    }
-    dst[i] = o;
-}
-__global__ void max_over_frames_f16_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, int F, size_t n8) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n8) return;
-    uint4 m = __ldg(src + i);
-    __half2* mh = reinterpret_cast<__half2*>(&m);
-    for (int f = 1; f < F; ++f) {
-        const uint4 v = __ldg(src + (size_t)f * n8 + i);
-        const __half2* vh = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) mh[k] = __hmax2(mh[k], vh[k]);
-    }
-    dst[i] = m;
-}
-// MaskModule encoder, between two levels (monorec_model.py:357-365 with :304-316): the level's output x [F*B,H,W,C] feeds both
-// the element-wise max over the frames (-> decoder skip connection) and the 2x2 max-pool (-> next level).  One pass over x
-// writes both (two kernels read the 268 MB level-0 tensor twice).  VEC = uint4 (8 half) or float4 (4 fp32).
+// element-wise max of two channel vectors: VEC = uint4 (8 half) or float4 (4 fp32)
 template <typename VEC, bool HALF>
 __device__ __forceinline__ VEC vmax(const VEC a, const VEC b) {
     VEC o;
@@ -461,6 +369,32 @@ __device__ __forceinline__ VEC vmax(const VEC a, const VEC b) {
     }
     return o;
 }
+// nn.MaxPool2d(2) (monorec_model.py:304-316) and the element-wise max over the leading frame axis (:362-365) on NHWC tensors
+template <typename VEC, bool HALF>
+__global__ void maxpool2_nhwc_kernel(const VEC* __restrict__ src, VEC* __restrict__ dst, int H, int W, int CV, size_t total) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return;
+    const int Wo = W / 2, Ho = H / 2;
+    const int c = (int)(i % CV);
+    size_t r = i / CV;
+    const int x = (int)(r % Wo); r /= Wo;
+    const int y = (int)(r % Ho);
+    const size_t b = r / Ho;
+    const VEC* p = src + ((b * H + 2 * y) * W + 2 * x) * CV + c;
+    const VEC q0 = __ldg(p), q1 = __ldg(p + CV), q2 = __ldg(p + (size_t)W * CV), q3 = __ldg(p + (size_t)W * CV + CV);
+    dst[i] = vmax<VEC, HALF>(vmax<VEC, HALF>(q0, q1), vmax<VEC, HALF>(q2, q3));
+}
+template <typename VEC, bool HALF>
+__global__ void max_over_frames_kernel(const VEC* __restrict__ src, VEC* __restrict__ dst, int F, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    VEC m = __ldg(src + i);
+    for (int f = 1; f < F; ++f) m = vmax<VEC, HALF>(m, __ldg(src + (size_t)f * n + i));
+    dst[i] = m;
+}
+// MaskModule encoder, between two levels (monorec_model.py:357-365 with :304-316): the level's output x [F*B,H,W,C] feeds both
+// the element-wise max over the frames (-> decoder skip connection) and the 2x2 max-pool (-> next level).  One pass over x
+// writes both (the two kernels above read the 268 MB level-0 tensor twice).
 template <typename VEC, bool HALF>
 __global__ void pool_and_frame_max_kernel(const VEC* __restrict__ src, VEC* __restrict__ pooled, VEC* __restrict__ fmax, int F, int B,
                                           int H, int W, int CV, size_t total) {
@@ -515,26 +449,6 @@ __global__ void cast_f32_to_f16_kernel(const float4* __restrict__ src, uint2* __
 }
 }  // namespace
 
-extern "C" int mr_maxpool2_nhwc_f16(const void* src, void* dst, int B, int H, int W, int C, void* stream) {
-    MR_REQUIRE(src && dst && B >= 1 && C >= 8 && (C % 8) == 0 && H >= 2 && W >= 2 && (H % 2) == 0 && (W % 2) == 0,
-               "mr_maxpool2_nhwc_f16: need even H, W and C %% 8 == 0 (got H=%d W=%d C=%d)", H, W, C);
-    const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-    maxpool2_nhwc_f16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        static_cast<const uint4*>(src), static_cast<uint4*>(dst), H, W, C / 8, total);
-    MR_LAUNCH_CHECK("maxpool2_nhwc_f16_kernel");
-    return MR_OK;
-}
-
-extern "C" int mr_max_over_frames_f16(const void* src, void* dst, int F, long long n_per_frame, void* stream) {
-    MR_REQUIRE(src && dst && F >= 1 && n_per_frame >= 8 && (n_per_frame % 8) == 0,
-               "mr_max_over_frames_f16: n_per_frame must be a positive multiple of 8");
-    const size_t n8 = (size_t)n_per_frame / 8;
-    max_over_frames_f16_kernel<<<(unsigned)((n8 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        static_cast<const uint4*>(src), static_cast<uint4*>(dst), F, n8);
-    MR_LAUNCH_CHECK("max_over_frames_f16_kernel");
-    return MR_OK;
-}
-
 extern "C" int mr_pool_and_frame_max(const void* src, void* pooled, void* frame_max, int dtype, int F, int B, int H, int W, int C,
                                      void* stream) {
     const int v = dtype == MR_DT_F16 ? 8 : 4;
@@ -579,22 +493,39 @@ extern "C" int mr_cast_f32_to_f16(const float* src, void* dst, long long n, void
     return MR_OK;
 }
 
-extern "C" int mr_maxpool2_nhwc(const float* src, float* dst, int B, int H, int W, int C, void* stream) {
-    MR_REQUIRE(src && dst && B >= 1 && C >= 4 && (C % 4) == 0 && H >= 2 && W >= 2 && (H % 2) == 0 && (W % 2) == 0,
-               "mr_maxpool2_nhwc: need even H, W and C %% 4 == 0 (got H=%d W=%d C=%d)", H, W, C);
-    const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 4);
-    maxpool2_nhwc_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), H, W, C / 4, total);
+extern "C" int mr_maxpool2_nhwc(const void* src, void* dst, int dtype, int B, int H, int W, int C, void* stream) {
+    MR_REQUIRE(dtype == MR_DT_F32 || dtype == MR_DT_F16, "mr_maxpool2_nhwc: dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", dtype);
+    const int v = dtype == MR_DT_F16 ? 8 : 4;
+    MR_REQUIRE(B >= 1 && C >= v && (C % v) == 0 && H >= 2 && W >= 2 && (H % 2) == 0 && (W % 2) == 0,
+               "mr_maxpool2_nhwc: need even H, W and C %% %d == 0 (got B=%d H=%d W=%d C=%d)", v, B, H, W, C);
+    MR_REQUIRE(src && dst, "mr_maxpool2_nhwc: null pointer (src, dst)");
+    const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / v);
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    if (dtype == MR_DT_F16)
+        maxpool2_nhwc_kernel<uint4, true><<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const uint4*>(src), static_cast<uint4*>(dst),
+                                                                                  H, W, C / v, total);
+    else
+        maxpool2_nhwc_kernel<float4, false><<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const float4*>(src),
+                                                                                    static_cast<float4*>(dst), H, W, C / v, total);
     MR_LAUNCH_CHECK("maxpool2_nhwc_kernel");
     return MR_OK;
 }
 
-extern "C" int mr_max_over_frames(const float* src, float* dst, int F, long long n_per_frame, void* stream) {
-    MR_REQUIRE(src && dst && F >= 1 && n_per_frame >= 4 && (n_per_frame % 4) == 0,
-               "mr_max_over_frames: n_per_frame must be a positive multiple of 4");
-    const size_t n4 = (size_t)n_per_frame / 4;
-    max_over_frames_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        reinterpret_cast<const float4*>(src), reinterpret_cast<float4*>(dst), F, n4);
+extern "C" int mr_max_over_frames(const void* src, void* dst, int dtype, int F, long long n_per_frame, void* stream) {
+    MR_REQUIRE(dtype == MR_DT_F32 || dtype == MR_DT_F16, "mr_max_over_frames: dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", dtype);
+    const int v = dtype == MR_DT_F16 ? 8 : 4;
+    MR_REQUIRE(F >= 1 && n_per_frame >= v && (n_per_frame % v) == 0,
+               "mr_max_over_frames: need F >= 1 and n_per_frame a positive multiple of %d (got F=%d n_per_frame=%lld)", v, F,
+               n_per_frame);
+    MR_REQUIRE(src && dst, "mr_max_over_frames: null pointer (src, dst)");
+    const size_t n = (size_t)n_per_frame / v;
+    const unsigned grid = (unsigned)((n + 255) / 256);
+    if (dtype == MR_DT_F16)
+        max_over_frames_kernel<uint4, true><<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const uint4*>(src),
+                                                                                    static_cast<uint4*>(dst), F, n);
+    else
+        max_over_frames_kernel<float4, false><<<grid, 256, 0, (cudaStream_t)stream>>>(static_cast<const float4*>(src),
+                                                                                      static_cast<float4*>(dst), F, n);
     MR_LAUNCH_CHECK("max_over_frames_kernel");
     return MR_OK;
 }

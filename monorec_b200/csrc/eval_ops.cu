@@ -1,5 +1,5 @@
-// Evaluation-side helpers of SURVEY.md section 8f row 2 (include/monorec_b200.h: mr_sparse_metrics, mr_dense_metrics and their
-// _grouped forms, mr_eval_accumulate, mr_median_scaling, mr_images_u8_to_f32).
+// Evaluation-side helpers of SURVEY.md section 8f row 2 (include/monorec_b200.h: mr_sparse_metrics, mr_dense_metrics,
+// mr_eval_accumulate, mr_median_scaling, mr_images_u8_to_f32).
 //
 //  * the seven sparse depth metrics of model/metric_functions/sparse_metrics.py:81-251 (a1, a2, a3, rmse, rmse_log, abs_rel,
 //    sq_rel; helpers utils/util.py:36-65, :101-118) in ONE pass over `result` / `target` instead of 7 x ~12 elementwise torch
@@ -379,22 +379,21 @@ extern "C" long long mr_sparse_metrics_workspace(int B) { return B < 1 ? 0 : (lo
 
 extern "C" long long mr_dense_metrics_workspace(int B) { return B < 1 ? 0 : (long long)B * kDenseSums * (long long)sizeof(double); }
 
-static int dense_metrics_run(const char* fn, const float* result, const float* target, int B, int group, int H, int W,
-                             const int* roi, float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes,
-                             void* stream) {
-    MR_REQUIRE(result && target && out_metrics && workspace, "%s: null pointer (result, target, out_metrics, workspace)", fn);
+extern "C" int mr_dense_metrics(const float* result, const float* target, int B, int group, int H, int W, const int* roi,
+                                float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes, void* stream) {
+    MR_REQUIRE(result && target && out_metrics && workspace, "mr_dense_metrics: null pointer (result, target, out_metrics, workspace)");
     MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1 && (long long)H * W <= 0x7fffffffLL,
-               "%s: bad shape B=%d H=%d W=%d", fn, B, H, W);
-    MR_REQUIRE(group >= 1, "%s: group=%d must be >= 1", fn, group);
+               "mr_dense_metrics: bad shape B=%d H=%d W=%d", B, H, W);
+    MR_REQUIRE(group >= 1, "mr_dense_metrics: group=%d must be >= 1", group);
     if (workspace_bytes < mr_dense_metrics_workspace(B)) {
-        mr::set_error("%s: workspace too small (%lld < %lld bytes)", fn, workspace_bytes, mr_dense_metrics_workspace(B));
+        mr::set_error("mr_dense_metrics: workspace too small (%lld < %lld bytes)", workspace_bytes, mr_dense_metrics_workspace(B));
         return MR_ENOMEM;
     }
-    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "%s: workspace must be 8-byte aligned", fn);
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "mr_dense_metrics: workspace must be 8-byte aligned");
     DenseArgs a{};
     a.pred = result; a.gt = target; a.B = B; a.H = H; a.W = W;
     clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
-    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "%s: empty region of interest (roi)", fn);
+    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "mr_dense_metrics: empty region of interest (roi)");
     a.min_inv = min_inv_depth;
     a.sums = static_cast<double*>(workspace);
     cudaStream_t st = (cudaStream_t)stream;
@@ -409,19 +408,6 @@ static int dense_metrics_run(const char* fn, const float* result, const float* t
                                                                (long long)(a.r1 - a.r0) * (a.c1 - a.c0), out_metrics);
     MR_LAUNCH_CHECK("dense_metric_finalize_kernel");
     return MR_OK;
-}
-
-extern "C" int mr_dense_metrics(const float* result, const float* target, int B, int H, int W, const int* roi, float min_inv_depth,
-                                float* out_metrics, void* workspace, long long workspace_bytes, void* stream) {
-    return dense_metrics_run("mr_dense_metrics", result, target, B, B, H, W, roi, min_inv_depth, out_metrics, workspace,
-                             workspace_bytes, stream);
-}
-
-extern "C" int mr_dense_metrics_grouped(const float* result, const float* target, int B, int group, int H, int W, const int* roi,
-                                        float min_inv_depth, float* out_metrics, void* workspace, long long workspace_bytes,
-                                        void* stream) {
-    return dense_metrics_run("mr_dense_metrics_grouped", result, target, B, group, H, W, roi, min_inv_depth, out_metrics,
-                             workspace, workspace_bytes, stream);
 }
 
 extern "C" long long mr_median_scaling_workspace(int B, int H, int W) {
@@ -461,21 +447,21 @@ extern "C" int mr_median_scaling(const float* result, const float* target, float
     return MR_OK;
 }
 
-static int sparse_metrics_run(const char* fn, const float* result, const float* target, const float* mvobj_mask, int B,
-                              int group, int H, int W, const int* roi, float max_distance, int pred_all_valid, float* out_metrics,
-                              void* workspace, long long workspace_bytes, void* stream) {
-    MR_REQUIRE(result && target && out_metrics && workspace, "%s: null pointer", fn);
-    MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1, "%s: bad shape B=%d H=%d W=%d", fn, B, H, W);
-    MR_REQUIRE(group >= 1, "%s: group=%d must be >= 1", fn, group);
+extern "C" int mr_sparse_metrics(const float* result, const float* target, const float* mvobj_mask, int B, int group, int H, int W,
+                                 const int* roi, float max_distance, int pred_all_valid, float* out_metrics, void* workspace,
+                                 long long workspace_bytes, void* stream) {
+    MR_REQUIRE(result && target && out_metrics && workspace, "mr_sparse_metrics: null pointer");
+    MR_REQUIRE(B >= 1 && B <= 65535 && H >= 1 && W >= 1, "mr_sparse_metrics: bad shape B=%d H=%d W=%d", B, H, W);
+    MR_REQUIRE(group >= 1, "mr_sparse_metrics: group=%d must be >= 1", group);
     if (workspace_bytes < mr_sparse_metrics_workspace(B)) {
-        mr::set_error("%s: workspace too small (%lld < %lld bytes)", fn, workspace_bytes, mr_sparse_metrics_workspace(B));
+        mr::set_error("mr_sparse_metrics: workspace too small (%lld < %lld bytes)", workspace_bytes, mr_sparse_metrics_workspace(B));
         return MR_ENOMEM;
     }
-    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "%s: workspace must be 8-byte aligned", fn);
+    MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "mr_sparse_metrics: workspace must be 8-byte aligned");
     MetricArgs a{};
     a.pred = result; a.gt = target; a.mvobj = mvobj_mask; a.B = B; a.H = H; a.W = W;
     clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
-    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "%s: empty region of interest", fn);
+    MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "mr_sparse_metrics: empty region of interest");
     a.inv_max = max_distance > 0.f ? 1.0f / max_distance : 0.f;
     a.pred_all_valid = pred_all_valid;
     a.sums = static_cast<double*>(workspace);
@@ -490,20 +476,6 @@ static int sparse_metrics_run(const char* fn, const float* result, const float* 
     sparse_metric_finalize_kernel<<<(G + 31) / 32, 32, 0, st>>>(a.sums, B, group, G, out_metrics);
     MR_LAUNCH_CHECK("sparse_metric_finalize_kernel");
     return MR_OK;
-}
-
-extern "C" int mr_sparse_metrics(const float* result, const float* target, const float* mvobj_mask, int B, int H, int W,
-                                 const int* roi, float max_distance, int pred_all_valid, float* out_metrics, void* workspace,
-                                 long long workspace_bytes, void* stream) {
-    return sparse_metrics_run("mr_sparse_metrics", result, target, mvobj_mask, B, B, H, W, roi, max_distance, pred_all_valid,
-                              out_metrics, workspace, workspace_bytes, stream);
-}
-
-extern "C" int mr_sparse_metrics_grouped(const float* result, const float* target, const float* mvobj_mask, int B, int group,
-                                         int H, int W, const int* roi, float max_distance, int pred_all_valid,
-                                         float* out_metrics, void* workspace, long long workspace_bytes, void* stream) {
-    return sparse_metrics_run("mr_sparse_metrics_grouped", result, target, mvobj_mask, B, group, H, W, roi, max_distance,
-                              pred_all_valid, out_metrics, workspace, workspace_bytes, stream);
 }
 
 extern "C" int mr_eval_accumulate(const float* values, int G, int M, const int* group_sizes, double* state, void* stream) {

@@ -3,8 +3,9 @@
 The reference's loop takes the loader's batches of key-frame dicts (batch size 2 in configs/evaluate/eval_monorec.json), runs
 an eager forward per batch and turns every metric of every batch into a Python float.  `SequenceEvaluater` takes the frames
 of a sequence and their targets one at a time instead: the model runs through the `MonoRecSequence` (rings, CUDA-graph
-replay), every batch of key frames it emits is cut into the evaluater's batches, and per emitted batch one grouped metric
-pass (`mr_sparse_metrics_grouped` / `mr_dense_metrics_grouped`) leaves one metric row per evaluater batch on the device.
+replay), every batch of key frames it emits is cut into the evaluater's batches, and per emitted batch one metric pass
+(`mr_sparse_metrics` / `mr_dense_metrics` with one group per evaluater batch) leaves one metric row per evaluater batch on
+the device.
 `log()` folds the rows with `mr_eval_accumulate` into the evaluater's float64 totals, reads them back once and returns
 `Evaluater.eval`'s dict.
 """

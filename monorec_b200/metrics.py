@@ -6,7 +6,9 @@ The reference's evaluater (evaluater/evaluater.py:78-112) calls the configured m
 dozen elementwise torch kernels and a few reductions.  Here the 21 `*_sparse*` metrics come out of ONE fused pass
 (`mr_sparse_metrics`) and the 12 dense and completeness metrics out of another (`mr_dense_metrics`); the functions below keep
 the reference's names and signatures and share those passes through a small cache, so `model.metric` can be pointed at this
-module unchanged.  No CPU fallback.
+module unchanged.  Each pass writes one row of metrics per group of `group` consecutive images; the functions below take
+the whole batch as one group, and the sequence evaluation (`evaluation.py`) takes one row per evaluater batch from the
+`*_grouped_impl` functions.  No CPU fallback.
 """
 import ctypes
 import weakref
@@ -42,23 +44,29 @@ def sparse_metrics(data_dict, roi=None, max_distance=None, pred_all_valid=True, 
 
 def sparse_metrics_impl(pred: Tensor, gt: Tensor, mvobj_mask: Optional[Tensor], roi: Optional[List[int]],
                         max_distance: float, pred_all_valid: bool) -> Tensor:
-    """The fused sparse pass (mr_sparse_metrics) -> [7]; max_distance 0 = none.  sparse_metrics calls this directly; under
-    torch.compile it is the implementation of the `monorec_b200::sparse_metrics` op."""
+    """The fused sparse pass over the whole batch -> [7].  sparse_metrics calls this directly; under torch.compile it is the
+    implementation of the `monorec_b200::sparse_metrics` op."""
+    # group = B (an empty batch keeps group 1, so that the library reports it)
+    return sparse_metrics_grouped_impl(pred, gt, mvobj_mask, roi, max_distance, pred_all_valid, max(pred.shape[0], 1))[0]
+
+
+def sparse_metrics_grouped_impl(pred: Tensor, gt: Tensor, mvobj_mask: Optional[Tensor], roi: Optional[List[int]],
+                                max_distance: float, pred_all_valid: bool, group: int) -> Tensor:
+    """The fused sparse pass (mr_sparse_metrics) over groups of `group` images -> [G,7], G = ceil(B / group): row g holds the
+    metrics of images [g * group, (g + 1) * group) (the last group may be shorter); max_distance 0 = none."""
     lib = _lib.load()
     pred = pred.to(torch.float32).contiguous()
     gt = gt.to(device=pred.device, dtype=torch.float32).contiguous()
     B, _, H, W = pred.shape
-    mv = None
-    if mvobj_mask is not None:
-        mv = mvobj_mask.to(device=pred.device, dtype=torch.float32).contiguous()
-    out = torch.empty(7, device=pred.device, dtype=torch.float32)
+    mv = None if mvobj_mask is None else mvobj_mask.to(device=pred.device, dtype=torch.float32).contiguous()
+    out = torch.empty(-(-B // group), 7, device=pred.device, dtype=torch.float32)
     ws_bytes = lib.mr_sparse_metrics_workspace(B)
     ws = torch.empty(ws_bytes // 8, device=pred.device, dtype=torch.float64)
     roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
     with torch.cuda.device(pred.device):
-        _lib.check(lib.mr_sparse_metrics(pred.data_ptr(), gt.data_ptr(), None if mv is None else mv.data_ptr(), B, H, W, roi_c,
-                                         max_distance, 1 if pred_all_valid else 0, out.data_ptr(), ws.data_ptr(), ws_bytes,
-                                         torch.cuda.current_stream(pred.device).cuda_stream), "mr_sparse_metrics")
+        _lib.check(lib.mr_sparse_metrics(pred.data_ptr(), gt.data_ptr(), None if mv is None else mv.data_ptr(), B, int(group),
+                                         H, W, roi_c, max_distance, 1 if pred_all_valid else 0, out.data_ptr(), ws.data_ptr(),
+                                         ws_bytes, torch.cuda.current_stream(pred.device).cuda_stream), "mr_sparse_metrics")
     return out
 
 
@@ -113,19 +121,26 @@ def dense_metrics(depth_prediction, depth_gt, roi=None, max_distance=None):
 
 
 def dense_metrics_impl(pred: Tensor, gt: Tensor, roi: Optional[List[int]], min_inv: float) -> Tensor:
-    """The fused dense pass (mr_dense_metrics) -> [12].  dense_metrics calls this directly; under torch.compile it is the
+    """The fused dense pass over the whole batch -> [12].  dense_metrics calls this directly; under torch.compile it is the
     implementation of the `monorec_b200::dense_metrics` op."""
+    # group = B (an empty batch keeps group 1, so that the library reports it)
+    return dense_metrics_grouped_impl(pred, gt, roi, min_inv, max(pred.shape[0], 1))[0]
+
+
+def dense_metrics_grouped_impl(pred: Tensor, gt: Tensor, roi: Optional[List[int]], min_inv: float, group: int) -> Tensor:
+    """The fused dense pass (mr_dense_metrics) over groups of `group` images -> [G,12]: row g holds the metrics of images
+    [g * group, (g + 1) * group)."""
     lib = _lib.load()
     p = pred.to(torch.float32).contiguous()
     g = gt.to(device=p.device, dtype=torch.float32).contiguous()
     B, _, H, W = p.shape
-    out = torch.empty(len(DENSE_NAMES), device=p.device, dtype=torch.float32)
+    out = torch.empty(-(-B // group), len(DENSE_NAMES), device=p.device, dtype=torch.float32)
     ws_bytes = lib.mr_dense_metrics_workspace(B)
     ws = torch.empty(ws_bytes // 8, device=p.device, dtype=torch.float64)
     roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
     with torch.cuda.device(p.device):
-        _lib.check(lib.mr_dense_metrics(p.data_ptr(), g.data_ptr(), B, H, W, roi_c, min_inv, out.data_ptr(), ws.data_ptr(),
-                                        ws_bytes, torch.cuda.current_stream(p.device).cuda_stream), "mr_dense_metrics")
+        _lib.check(lib.mr_dense_metrics(p.data_ptr(), g.data_ptr(), B, int(group), H, W, roi_c, min_inv, out.data_ptr(),
+                                        ws.data_ptr(), ws_bytes, torch.cuda.current_stream(p.device).cuda_stream), "mr_dense_metrics")
     return out
 
 
@@ -190,45 +205,6 @@ def median_scaling_impl(pred: Tensor, gt: Tensor) -> Tensor:
     with torch.cuda.device(p.device):
         _lib.check(lib.mr_median_scaling(p.data_ptr(), g.data_ptr(), out.data_ptr(), B, H, W, ws.data_ptr(), ws_bytes,
                                          torch.cuda.current_stream(p.device).cuda_stream), "mr_median_scaling")
-    return out
-
-
-def sparse_metrics_grouped_impl(pred: Tensor, gt: Tensor, mvobj_mask: Optional[Tensor], roi: Optional[List[int]],
-                                max_distance: float, pred_all_valid: bool, group: int) -> Tensor:
-    """mr_sparse_metrics_grouped -> [G,7]: row g is sparse_metrics_impl of images [g * group, (g + 1) * group) (the last
-    group may be shorter), from one pass over the whole batch."""
-    lib = _lib.load()
-    pred = pred.to(torch.float32).contiguous()
-    gt = gt.to(device=pred.device, dtype=torch.float32).contiguous()
-    B, _, H, W = pred.shape
-    mv = None if mvobj_mask is None else mvobj_mask.to(device=pred.device, dtype=torch.float32).contiguous()
-    out = torch.empty(-(-B // group), 7, device=pred.device, dtype=torch.float32)
-    ws_bytes = lib.mr_sparse_metrics_workspace(B)
-    ws = torch.empty(ws_bytes // 8, device=pred.device, dtype=torch.float64)
-    roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
-    with torch.cuda.device(pred.device):
-        _lib.check(lib.mr_sparse_metrics_grouped(pred.data_ptr(), gt.data_ptr(), None if mv is None else mv.data_ptr(), B,
-                                                 int(group), H, W, roi_c, max_distance, 1 if pred_all_valid else 0,
-                                                 out.data_ptr(), ws.data_ptr(), ws_bytes,
-                                                 torch.cuda.current_stream(pred.device).cuda_stream),
-                   "mr_sparse_metrics_grouped")
-    return out
-
-
-def dense_metrics_grouped_impl(pred: Tensor, gt: Tensor, roi: Optional[List[int]], min_inv: float, group: int) -> Tensor:
-    """mr_dense_metrics_grouped -> [G,12]: row g is dense_metrics_impl of images [g * group, (g + 1) * group)."""
-    lib = _lib.load()
-    p = pred.to(torch.float32).contiguous()
-    g = gt.to(device=p.device, dtype=torch.float32).contiguous()
-    B, _, H, W = p.shape
-    out = torch.empty(-(-B // group), len(DENSE_NAMES), device=p.device, dtype=torch.float32)
-    ws_bytes = lib.mr_dense_metrics_workspace(B)
-    ws = torch.empty(ws_bytes // 8, device=p.device, dtype=torch.float64)
-    roi_c = None if roi is None else (ctypes.c_int * 4)(*roi)
-    with torch.cuda.device(p.device):
-        _lib.check(lib.mr_dense_metrics_grouped(p.data_ptr(), g.data_ptr(), B, int(group), H, W, roi_c, min_inv, out.data_ptr(),
-                                                ws.data_ptr(), ws_bytes, torch.cuda.current_stream(p.device).cuda_stream),
-                   "mr_dense_metrics_grouped")
     return out
 
 

@@ -364,11 +364,6 @@ class _TrunkFeatures(list):
         return (list, (list(list.__iter__(self)),))
 
 
-def _f32_or_f16(v):
-    """A cost volume as the layout kernels read it: half volumes (volume_dtype=torch.float16) are widened by the kernel."""
-    return v if v.dtype == torch.float16 else v.to(torch.float32)
-
-
 class MaskModule(_PackedSource, nn.Module):
     """Moving-object mask U-Net over the single-frame volumes (monorec_model.py:287-385)."""
 
@@ -440,7 +435,7 @@ class MaskModule(_PackedSource, nn.Module):
             # (standalone call, or a configuration the fused kernel does not write the engine layout for)
             x = torch.empty(nF * B, H, W, D, device=sfcvs[0].device, dtype=C.act_dtype())
             for f, v in enumerate(sfcvs):
-                C.nchw_to_nhwc(_f32_or_f16(v), out=x[f * B:(f + 1) * B])
+                C.nchw_to_nhwc(v, out=x[f * B:(f + 1) * B])
         if not self.use_cv:
             x = torch.zeros_like(x)      # (x may be the caller's buffer: not written)
         cv_feats = []
@@ -577,7 +572,7 @@ class DepthModule(_PackedSource, nn.Module):
         x = torch.empty(B, H, W, D + 3 + cpad, device=cv.device, dtype=C.act_dtype())
         if cpad:
             x[..., D + 3:].zero_()
-        C.nchw_to_nhwc(_f32_or_f16(cv), out=x, out_coff=0, one_minus=cv_mask)
+        C.nchw_to_nhwc(cv, out=x, out_coff=0, one_minus=cv_mask)
         C.nchw_to_nhwc(keyframe.to(torch.float32), out=x, out_coff=D)
         img = [C.as_nhwc(f, C.act_dtype()) for f in feats_nchw[:3]]
         feats = []

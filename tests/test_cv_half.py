@@ -64,16 +64,35 @@ def test_half_host_entry_sizes_and_validation_without_gpu():
     assert b"workspace too small" in lib.mr_last_error()
 
 
-def test_half_volume_helpers_validation_without_gpu():
+def test_typed_layout_pool_mask_validation_without_gpu():
+    """The layout, pooling and masking entries with half tensors (MR_DT_F16 = 1), a dtype argument other than MR_DT_F32 /
+    MR_DT_F16, and the channel-vector width that follows the dtype: MR_EINVAL and a message naming the argument, before any
+    CUDA call (fake, never dereferenced pointers)."""
     lib = _lib()
     src, dst, m = 0x7F0006000000, 0x7F0007000000, 0x7F0008000000
-    assert lib.mr_nchw_f16_to_nhwc(src, dst, 2, 1, 32, 8, 8, 32, 0, None, None) == -1
+    assert lib.mr_nchw_to_nhwc(src, 1, dst, 2, 1, 32, 8, 8, 32, 0, None, None) == -1
     assert b"dst_dtype" in lib.mr_last_error()
-    assert lib.mr_nchw_f16_to_nhwc(src, dst, 1, 1, 32, 8, 8, 32, 4, None, None) == -1
+    assert lib.mr_nchw_to_nhwc(src, 1, dst, 1, 1, 32, 8, 8, 32, 4, None, None) == -1
     assert b"channel slice" in lib.mr_last_error()
-    assert lib.mr_nchw_f16_to_nhwc(None, dst, 0, 1, 32, 8, 8, 32, 0, None, None) == -1
-    assert lib.mr_mask_volume_f16(src, None, dst, 1, 32, 64, None) == -1
-    assert b"mr_mask_volume_f16" in lib.mr_last_error()
+    assert lib.mr_nchw_to_nhwc(None, 1, dst, 0, 1, 32, 8, 8, 32, 0, None, None) == -1
+    assert lib.mr_mask_volume(src, None, dst, 1, 1, 32, 64, None) == -1
+    assert b"mr_mask_volume" in lib.mr_last_error()
+    bad_dtype = [(lambda d: lib.mr_nchw_to_nhwc(src, d, dst, 1, 1, 32, 8, 8, 32, 0, None, None), b"mr_nchw_to_nhwc: src_dtype"),
+                 (lambda d: lib.mr_nchw_to_nhwc(src, 1, dst, d, 1, 32, 8, 8, 32, 0, None, None), b"mr_nchw_to_nhwc: dst_dtype"),
+                 (lambda d: lib.mr_maxpool2_nhwc(src, dst, d, 1, 8, 8, 32, None), b"mr_maxpool2_nhwc: dtype"),
+                 (lambda d: lib.mr_max_over_frames(src, dst, d, 2, 64, None), b"mr_max_over_frames: dtype"),
+                 (lambda d: lib.mr_mask_volume(src, m, dst, d, 1, 32, 64, None), b"mr_mask_volume: dtype")]
+    for call, text in bad_dtype:
+        for d in (2, -1):
+            assert call(d) == -1 and text in lib.mr_last_error(), (text, d, lib.mr_last_error())
+    # 4 channels (values per frame) are one fp32 vector but half a half vector: the fp32 call gets past the width check to
+    # the null destination, the half call stops at the width
+    for dtype, text in ((0, b"null pointer"), (1, b"C % 8")):
+        assert lib.mr_maxpool2_nhwc(src, None, dtype, 1, 8, 8, 4, None) == -1
+        assert text in lib.mr_last_error(), (dtype, lib.mr_last_error())
+    for dtype, text in ((0, b"null pointer"), (1, b"multiple of 8")):
+        assert lib.mr_max_over_frames(src, None, dtype, 2, 4, None) == -1
+        assert text in lib.mr_last_error(), (dtype, lib.mr_last_error())
 
 
 def test_volume_dtype_keyword():
@@ -96,8 +115,9 @@ def test_volume_dtype_keyword():
         MonoRecModel(volume_dtype=torch.bfloat16)
 
 
-def test_c_consumer_of_the_half_entries(tmp_path):
-    """The new declarations compile as C99 (-pedantic) and link; their argument checks answer without a GPU."""
+def test_c_consumer_of_the_typed_entries(tmp_path):
+    """The half-volume declarations and the typed layout / masking entries compile as C99 (-pedantic) and link; their
+    argument checks answer without a GPU."""
     import shutil
     import subprocess
     from pathlib import Path
@@ -118,8 +138,8 @@ def test_c_consumer_of_the_half_entries(tmp_path):
                    '    if (strstr(mr_last_error(), "out_dtype") == 0) return 5;\n'
                    '    if (mr_cost_volume_host_f16(0, 0, 0, 0, 0, 0, 0, 0, 2, 2, 32, 64, 128, 0.0025f, 0.33f, 10.0f, 0, w16)\n'
                    '        != MR_EINVAL) return 6;\n'
-                   '    if (mr_mask_volume_f16(0, 0, 0, 1, 1, 1, 0) != MR_EINVAL) return 7;\n'
-                   '    if (mr_nchw_f16_to_nhwc(0, 0, MR_DT_F16, 1, 1, 1, 1, 1, 0, 0, 0) != MR_EINVAL) return 8;\n'
+                   '    if (mr_mask_volume(0, 0, 0, MR_DT_F16, 1, 1, 1, 0) != MR_EINVAL) return 7;\n'
+                   '    if (mr_nchw_to_nhwc(0, MR_DT_F16, 0, MR_DT_F16, 1, 1, 1, 1, 1, 0, 0, 0) != MR_EINVAL) return 8;\n'
                    '    return 0;\n}\n')
     exe = tmp_path / "consumer_f16"
     libdir = _lib.LIB_PATH.parent

@@ -91,20 +91,20 @@ def _abi():
     return _lib.load()
 
 
-def test_grouped_metrics_validation_without_gpu():
+def test_metric_groups_validation_without_gpu():
     lib = _abi()
     p, t, o, ws = 0x7F0000100000, 0x7F0000200000, 0x7F0000300000, 0x7F0000400000
     for kw, text in ((dict(group=0), "group=0"), (dict(group=-2), "group=-2"), (dict(p=None), "null pointer"),
                      (dict(B=0), "B=0"), (dict(ws=ws + 4), "aligned")):
         a = dict(p=p, B=4, group=2, ws=ws)
         a.update(kw)
-        rc = lib.mr_sparse_metrics_grouped(a["p"], t, None, a["B"], a["group"], 8, 8, None, 80.0, 1, o, a["ws"], 1024, None)
+        rc = lib.mr_sparse_metrics(a["p"], t, None, a["B"], a["group"], 8, 8, None, 80.0, 1, o, a["ws"], 1024, None)
         msg = lib.mr_last_error().decode()
-        assert rc == -1 and msg.startswith("mr_sparse_metrics_grouped") and text in msg, (kw, rc, msg)
-        rc = lib.mr_dense_metrics_grouped(a["p"], t, a["B"], a["group"], 8, 8, None, 0.0, o, a["ws"], 1024, None)
+        assert rc == -1 and msg.startswith("mr_sparse_metrics:") and text in msg, (kw, rc, msg)
+        rc = lib.mr_dense_metrics(a["p"], t, a["B"], a["group"], 8, 8, None, 0.0, o, a["ws"], 1024, None)
         msg = lib.mr_last_error().decode()
-        assert rc == -1 and msg.startswith("mr_dense_metrics_grouped") and text in msg, (kw, rc, msg)
-    assert lib.mr_sparse_metrics_grouped(p, t, None, 4, 2, 8, 8, None, 80.0, 1, o, ws, 8, None) == -3      # MR_ENOMEM
+        assert rc == -1 and msg.startswith("mr_dense_metrics:") and text in msg, (kw, rc, msg)
+    assert lib.mr_sparse_metrics(p, t, None, 4, 2, 8, 8, None, 80.0, 1, o, ws, 8, None) == -3      # MR_ENOMEM
     assert b"workspace too small" in lib.mr_last_error()
 
 

@@ -1,5 +1,5 @@
-"""The sequence form of evaluate.py on the device: the grouped metric passes (`mr_sparse_metrics_grouped`,
-`mr_dense_metrics_grouped`), the evaluater's accumulator (`mr_eval_accumulate`) and SequenceEvaluater, against the ungrouped
+"""The sequence form of evaluate.py on the device: the grouped metric passes (`mr_sparse_metrics` / `mr_dense_metrics` with
+several groups), the evaluater's accumulator (`mr_eval_accumulate`) and SequenceEvaluater, against the one-group
 passes, the float64 restatement (tests/eval_oracle.py), the reference's own logs (tests/golden/eval_sequence.npz) and the
 evaluater's loop over the same key frames."""
 import json

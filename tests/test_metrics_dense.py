@@ -77,21 +77,21 @@ def _abi():
     return _lib.load()
 
 
-def test_dense_metrics_validation_without_gpu():
-    """Bad arguments of mr_dense_metrics give MR_EINVAL and a message naming the field, before any CUDA call (fake, never
-    dereferenced pointers)."""
+def test_dense_metrics_group_validation_without_gpu():
+    """Bad arguments of mr_dense_metrics, the group size included, give MR_EINVAL and a message naming the field, before any
+    CUDA call (fake, never dereferenced pointers)."""
     lib = _abi()
     p, t, o, ws = 0x7F0000100000, 0x7F0000200000, 0x7F0000300000, 0x7F0000400000
     assert lib.mr_dense_metrics_workspace(4) == 4 * 13 * 8 and lib.mr_dense_metrics_workspace(0) == 0
 
-    def call(p=p, t=t, o=o, ws=ws, B=2, H=8, W=8, roi=None, ws_bytes=1024):
-        rc = lib.mr_dense_metrics(p, t, B, H, W, roi, 0.0, o, ws, ws_bytes, None)
+    def call(p=p, t=t, o=o, ws=ws, B=2, group=2, H=8, W=8, roi=None, ws_bytes=1024):
+        rc = lib.mr_dense_metrics(p, t, B, group, H, W, roi, 0.0, o, ws, ws_bytes, None)
         return rc, lib.mr_last_error().decode()
 
     empty = (ctypes.c_int * 4)(5, 5, 0, 8)
     for kw, text in ((dict(p=None), "result"), (dict(t=None), "target"), (dict(o=None), "out_metrics"),
                      (dict(ws=None), "workspace"), (dict(B=0), "B=0"), (dict(H=0), "H=0"), (dict(W=-1), "W=-1"),
-                     (dict(roi=empty), "roi"), (dict(ws=ws + 4), "aligned")):
+                     (dict(roi=empty), "roi"), (dict(ws=ws + 4), "aligned"), (dict(group=0), "group=0")):
         rc, msg = call(**kw)
         assert rc == -1 and text in msg, (kw, rc, msg)
     rc, msg = call(ws_bytes=8)
