@@ -118,6 +118,15 @@ class SequenceEvaluater:
     def push(self, image, pose, intrinsics, target, mvobj_mask=None, stereo=None):
         if self.seq is None:
             raise ValueError("SequenceEvaluater.push needs a sequence (seq is None)")
+        self._check_frame(image, target, mvobj_mask)
+        keep_mask = self._needs_mvobj or self.seq.mvobj_masks
+        emitted = self.seq.push(image, pose, intrinsics, stereo=stereo, mvobj_mask=mvobj_mask if keep_mask else None,
+                                target=target)
+        self._consume(emitted)
+        return emitted
+
+    def _check_frame(self, image, target, mvobj_mask):
+        """push's checks of a frame's target and mask (MultiModelEvaluater.push makes them too)."""
         H, W = image.shape[-2:]
         if self._needs_mvobj and mvobj_mask is None:
             raise ValueError(f"{[n for n in self.names if 'onlydynamic' in n]} need the frame's mvobj_mask")
@@ -126,11 +135,6 @@ class SequenceEvaluater:
             if t.numel() != H * W or tuple(t.shape[-2:]) != (H, W):
                 raise ValueError(f"SequenceEvaluater.push: target / mvobj_mask [1,H,W] of the image's size {(H, W)} expected, "
                                  f"got {tuple(t.shape)}")
-        keep_mask = self._needs_mvobj or self.seq.mvobj_masks
-        emitted = self.seq.push(image, pose, intrinsics, stereo=stereo, mvobj_mask=mvobj_mask if keep_mask else None,
-                                target=target)
-        self._consume(emitted)
-        return emitted
 
     def skip(self):
         """Passes a frame that no key frame of the sequence needs, without reading it (`MonoRecSequence.skip`)."""

@@ -701,6 +701,20 @@ class MonoRecModel(nn.Module):
                                                   strict=False)
 
     def forward(self, data_dict):
+        data_dict = self._stage_cost_volume(data_dict)
+        data_dict = self._stage_trunk(data_dict)
+        return self._stage_heads(data_dict)
+
+    # The forward's three stages.  Each adds its outputs to the dict it is given and returns it; the heads read what the
+    # other two added and write no tensor they produced, so several models can run their own heads on one cost volume and
+    # one trunk output (models_eval.MultiModelEvaluater, which shares them through shallow copies of the dict).
+    def _writes_sfcv_nhwc(self):
+        """Whether the cost-volume stage also writes the MaskModule's NHWC input (a buffer the heads then read)."""
+        return (not self.no_cv and hasattr(self, "att_module") and self.att_module.use_cv and C.MODE in ("tf32", "f16")
+                and self.cv_depth_steps <= 32 and self.cv_depth_steps % 8 == 0)
+
+    def _stage_cost_volume(self, data_dict):
+        """Stage A: the depth-range entries, `cost_volume`, `single_frame_cvs` (and the MaskModule's NHWC copy of them)."""
         keyframe = data_dict["keyframe"]
         lo, hi = float(self.inv_depth_min_max[1]), float(self.inv_depth_min_max[0])
         # 1-element tensors like the reference's (:675-677); torch.full is a fill kernel (CUDA-graph capturable, no H2D copy)
@@ -711,8 +725,7 @@ class MonoRecModel(nn.Module):
 
         with torch.no_grad():
             if not self.no_cv:
-                if hasattr(self, "att_module") and self.att_module.use_cv and C.MODE in ("tf32", "f16") \
-                        and self.cv_depth_steps <= 32 and self.cv_depth_steps % 8 == 0:
+                if self._writes_sfcv_nhwc():
                     # the MaskModule's NHWC input is written by the cost-volume kernel's per-pixel phase (no layout-change launches)
                     nf = (len(data_dict["frames"]) if self.use_mono else 0) + (1 if self.use_stereo else 0)
                     data_dict["_sfcv_nhwc"] = torch.empty(nf * keyframe.shape[0], keyframe.shape[2], keyframe.shape[3],
@@ -723,7 +736,12 @@ class MonoRecModel(nn.Module):
                 s[1] = self.cv_depth_steps
                 data_dict["cost_volume"] = keyframe.new_zeros(s, dtype=self.volume_dtype)
                 data_dict["single_frame_cvs"] = [data_dict["cost_volume"].clone() for _ in data_dict["poses"]]
+        return data_dict
 
+    def _stage_trunk(self, data_dict):
+        """Stage B: `image_features`, the ResNet-18 trunk's levels of the key frame."""
+        keyframe = data_dict["keyframe"]
+        with torch.no_grad():
             # torchvision trunk on cuDNN, fed channels-last; TF32 is allowed there unless the engine runs its fp32 parity mode
             image = (keyframe + .5).contiguous(memory_format=torch.channels_last)
             if torch.compiler.is_compiling():
@@ -735,7 +753,14 @@ class MonoRecModel(nn.Module):
                                                                                   C.MODE != "fp32")
             else:
                 data_dict["image_features"] = trunk_features(self._feature_extractor, image, C.MODE != "fp32")
+        return data_dict
 
+    def _stage_heads(self, data_dict):
+        """Stage C: the Mask and Depth stacks, the masking and the heads -> `cv_mask`, `predicted_inverse_depths`, the
+        masked `cost_volume` (a new tensor), `result`, `mask`."""
+        keyframe = data_dict["keyframe"]
+        lo, hi = float(self.inv_depth_min_max[1]), float(self.inv_depth_min_max[0])
+        with torch.no_grad():
             if self.pretrain_mode == 0 or self.pretrain_mode == 2:
                 data_dict = self.att_module(data_dict)
             elif self.pretrain_mode == 1:

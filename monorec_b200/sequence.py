@@ -300,4 +300,6 @@ def _row(out, j):
     v = {k: out[k][j:j + 1] for k in _ROW_KEYS if k in out}
     if "predicted_inverse_depths" in out:
         v["predicted_inverse_depths"] = [p[j:j + 1] for p in out["predicted_inverse_depths"]]
+    if "models" in out:          # several models over one batch (models_eval): one output dict per model
+        v["models"] = [_row(o, j) for o in out["models"]]
     return v
