@@ -985,7 +985,10 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     // ---- validity pre-pass for every frame: valid_f(v,u) = interior(v,u) & all_d [ sample strictly inside
     //      (1,W-2)x(1,H-2) ]  (monorec_model.py:212-219: bilinear sample of the interior mask != 0 for every plane).
     //      The D samples of a pixel lie on one line and move monotonically with the depth while the denominator keeps
-    //      its sign, so the farthest and the nearest plane decide. -----------------------------------------------------
+    //      its sign, so the farthest and the nearest plane decide.  A denominator < 0 is a point behind the source camera:
+    //      the reference still samples its mirrored projection (layers.py:66 divides by z + 1e-7 whatever its sign), so
+    //      such samples count like any other.  Where the denominator changes sign between the two ends, the ray crosses the
+    //      source camera's plane and its samples do not lie on one segment: every depth of the pixel is checked. -----------
     for (int q = tid; q < F * TH * kTileCols; q += kThreads) {
         const int fr = q >> 6, bc = q & 63;            // fr = f * TH + r
         const int f = fr / TH, r = fr - f * TH;
@@ -998,6 +1001,14 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             const float ay = fmaf(m[4], fu, fmaf(m[5], fv, m[6]));
             const float az = fmaf(m[8], fu, fmaf(m[9], fv, m[10]));
             const float m03 = m[3], m13 = m[7], m23 = m[11];
+            auto inside = [&](const float z, float& den) {
+                den = fmaf(az, z, m23);
+                const float inv = fast_rcp(den);
+                const float sx = fmaf(fmaf(ax, z, m03), inv, -0.5f);
+                const float sy = fmaf(fmaf(ay, z, m13), inv, -0.5f);
+                return (sx > 1.0f) && (sx < fW - 2.0f) && (sy > 1.0f) && (sy < fH - 2.0f);
+            };
+            float den[2] = {1.0f, 1.0f};
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
                 float z;
@@ -1007,11 +1018,14 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
                 } else {
                     z = zs[k ? D - 1 : 0];
                 }
-                const float den = fmaf(az, z, m23);
-                const float inv = fast_rcp(den);
-                const float sx = fmaf(fmaf(ax, z, m03), inv, -0.5f);
-                const float sy = fmaf(fmaf(ay, z, m13), inv, -0.5f);
-                ok = ok && (den > 0.f) && (sx > 1.0f) && (sx < fW - 2.0f) && (sy > 1.0f) && (sy < fH - 2.0f);
+                ok = ok && inside(z, den[k]);
+            }
+            if (ok && ((den[0] > 0.f) != (den[1] > 0.f))) {
+                for (int d = 0; d < D && ok; ++d) {
+                    float dd;
+                    if constexpr (PIX) ok = inside(__ldg(a.depths + ((size_t)b * D + d) * plane + (size_t)v * W + u), dd);
+                    else ok = inside(zs[d], dd);
+                }
             }
         }
         vmask[q] = ok ? 1 : 0;

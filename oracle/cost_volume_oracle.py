@@ -233,6 +233,76 @@ def projection_tables(data, use_mono=True, use_stereo=False, dtype=np.float64):
     return proj, kinv
 
 
+def _closed_form_depths(data, inv_depth_min, inv_depth_max, steps, cv_depths, dtype):
+    """(B, D, 1, H or 1, W or 1) float64 depths of the closed form: `cv_depths`, or the planes of `dtype`."""
+    B = data["keyframe"].shape[0]
+    if cv_depths is not None:
+        return cv_depths.numpy().astype(np.float64)[:, :, None]
+    D = int(steps)
+    if dtype == np.float32:
+        z = plane_depths(inv_depth_min, inv_depth_max, D).numpy().astype(np.float64)
+    else:
+        z = 1.0 / np.linspace(float(inv_depth_max), float(inv_depth_min), D, dtype=np.float64)
+    return np.broadcast_to(z.reshape(1, D, 1, 1, 1), (B, D, 1, 1, 1))
+
+
+def _source_positions(P, ray, z, H, W, dtype):
+    """Source pixel coordinates (sx, sy), each (D, H, W), of the rays `ray` (3, H, W) at depths `z` (D, 1, H|1, W|1) under
+    the projection P (3, 4): layers.py:65-70 and grid_sample's un-normalisation, in float64 (rounded to fp32 where dtype is
+    float32)."""
+    A = np.einsum("ij,jhw->ihw", P[:, :3], ray)                                           # (3,H,W)
+    c = A[None] * z + P[:, 3][None, :, None, None]                                         # (D,3,H,W)
+    c = c.astype(dtype).astype(np.float64) if dtype == np.float32 else c
+    with np.errstate(divide="ignore", invalid="ignore"):
+        px = c[:, 0] / (c[:, 2] + 1e-7)
+        py = c[:, 1] / (c[:, 2] + 1e-7)
+    gx = np.clip((px / (W - 1) - 0.5) * 2, -2, 2)
+    gy = np.clip((py / (H - 1) - 0.5) * 2, -2, 2)
+    sx = ((gx + 1) * W - 1) / 2
+    sy = ((gy + 1) * H - 1) / 2
+    if dtype == np.float32:
+        sx, sy = sx.astype(np.float32), sy.astype(np.float32)
+    return sx, sy
+
+
+def _key_rays(kinv, H, W):
+    vv, uu = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
+    return np.einsum("ij,jhw->ihw", kinv, np.stack([uu, vv, np.ones_like(uu)]))           # (3,H,W)
+
+
+def _interior(H, W):
+    inside = np.zeros((H, W), dtype=bool)
+    inside[2:H - 2, 2:W - 2] = True                                                        # monorec_model.py:282-284
+    return inside
+
+
+def validity_margin(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, use_mono=True, use_stereo=False,
+                    cv_depths=None, dtype=np.float64):
+    """Signed distance (B, F, H, W) float64, in source pixels, from each pixel's nearest sample to the edge of the
+    validity region, at the positions `cost_volume_closed_form` uses with the same arguments.
+
+    The interior mask covers rows and columns 2 .. n-3, so its bilinear sample (zero padding) is non-zero exactly when
+    1 < sx < W-2 and 1 < sy < H-2.  A pixel is valid for a frame when that holds for all of its depths, so the margin is the
+    minimum over the depths of min(sx - 1, W - 2 - sx, sy - 1, H - 2 - sy): `margin > 0` is the closed form's `valid`.
+    It is -inf in the 2-px ring and where a sample is not finite.
+    """
+    frames, _, _ = collect_frames(data, use_mono, use_stereo)
+    B, _, H, W = data["keyframe"].shape
+    z = _closed_form_depths(data, inv_depth_min, inv_depth_max, steps, cv_depths, dtype)
+    proj, kinv = projection_tables(data, use_mono, use_stereo, dtype=np.float64)
+    inside = _interior(H, W)
+    out = np.full((B, len(frames), H, W), -np.inf)
+    for b in range(B):
+        ray = _key_rays(kinv[b], H, W)
+        for f in range(len(frames)):
+            sx, sy = _source_positions(proj[b, f], ray, z[b], H, W, dtype)
+            sx, sy = sx.astype(np.float64), sy.astype(np.float64)
+            m = np.minimum(np.minimum(sx - 1, W - 2 - sx), np.minimum(sy - 1, H - 2 - sy))
+            m = np.where(np.isfinite(m), m, -np.inf).min(axis=0)
+            out[b, f] = np.where(inside, m, -np.inf)
+    return out
+
+
 def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, steps=32, use_mono=True,
                             use_stereo=False, alpha=ALPHA, channel_weights=CHANNEL_WEIGHTS, dtype=np.float32,
                             cv_depths=None, use_ssim=True, not_center_cv=False):
@@ -246,20 +316,10 @@ def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, step
     frames, _, _ = collect_frames(data, use_mono, use_stereo)
     key = data["keyframe"].numpy().astype(dtype)
     B, C, H, W = key.shape
-    if cv_depths is not None:
-        z = cv_depths.numpy().astype(np.float64)[:, :, None]                               # (B,D,1,H,W)
-    else:
-        D = int(steps)
-        if dtype == np.float32:
-            z = plane_depths(inv_depth_min, inv_depth_max, D).numpy().astype(np.float64)
-        else:
-            z = 1.0 / np.linspace(float(inv_depth_max), float(inv_depth_min), D, dtype=np.float64)
-        z = np.broadcast_to(z.reshape(1, D, 1, 1, 1), (B, D, 1, 1, 1))
+    z = _closed_form_depths(data, inv_depth_min, inv_depth_max, steps, cv_depths, dtype)
     nF, D = len(frames), z.shape[1]
     proj, kinv = projection_tables(data, use_mono, use_stereo, dtype=np.float64)
-    vv, uu = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
-    inside = np.zeros((H, W), dtype=bool)
-    inside[2:H - 2, 2:W - 2] = True
+    inside = _interior(H, W)
     cw = np.asarray(channel_weights, dtype=dtype).reshape(1, 3, 1, 1)
 
     cvs = np.zeros((B, D, H, W), dtype=dtype)
@@ -267,7 +327,7 @@ def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, step
     valids = np.zeros((B, nF, H, W), dtype=bool)
     sads = np.zeros((B, nF, D, H, W), dtype=dtype)
     for b in range(B):
-        ray = np.einsum("ij,jhw->ihw", kinv[b], np.stack([uu, vv, np.ones_like(uu)]))      # (3,H,W)
+        ray = _key_rays(kinv[b], H, W)
         Y = key[b] + dtype(0.5)
         mu_y = _box3(Y) / dtype(9)
         s_y = _box3(Y * Y) / dtype(9) - mu_y * mu_y
@@ -275,19 +335,7 @@ def cost_volume_closed_form(data, inv_depth_min=0.33, inv_depth_max=0.0025, step
         den = np.zeros((H, W), dtype=dtype)
         for f in range(nF):
             img = frames[f][b].numpy().astype(dtype)
-            P = proj[b, f]
-            A = np.einsum("ij,jhw->ihw", P[:, :3], ray)                                    # (3,H,W)
-            c = A[None] * z[b] + P[:, 3][None, :, None, None]                             # (D,3,H,W)
-            c = c.astype(dtype).astype(np.float64) if dtype == np.float32 else c
-            with np.errstate(divide="ignore", invalid="ignore"):
-                px = c[:, 0] / (c[:, 2] + 1e-7)
-                py = c[:, 1] / (c[:, 2] + 1e-7)
-            gx = np.clip((px / (W - 1) - 0.5) * 2, -2, 2)
-            gy = np.clip((py / (H - 1) - 0.5) * 2, -2, 2)
-            sx = ((gx + 1) * W - 1) / 2
-            sy = ((gy + 1) * H - 1) / 2
-            if dtype == np.float32:
-                sx, sy = sx.astype(np.float32), sy.astype(np.float32)
+            sx, sy = _source_positions(proj[b, f], ray, z[b], H, W, dtype)
             X = _bilinear_zero(img, sx, sy) + dtype(0.5)                                   # (3,D,H,W)
             hit = _bilinear_zero(inside[None].astype(dtype), sx, sy)[0] != 0               # (D,H,W)
             valid = inside & hit.all(axis=0)

@@ -74,6 +74,17 @@ def wide_depths(B, D, H, W, seed):
     return torch.from_numpy((far ** t).astype(np.float32))
 
 
+def step_depths(B, D, H, W, z_near=2.0, z_far=30.0, rel=4.0):
+    """A x1/rel - x rel band around z_near left of a vertical edge at 0.43 W (through the middle of a 60-column tile) and
+    around z_far right of it, fp32.  (A far side at hundreds of metres has flat costs over the whole band: its view weights
+    vanish and the fused value is a ratio of rounding noise in the reference formula itself; 30 m keeps the fused volume
+    comparable.)"""
+    s = torch.full((B, 1, H, W), z_far)
+    s[..., : int(0.43 * W)] = z_near
+    f = torch.exp(torch.linspace(-np.log(rel), np.log(rel), D, dtype=torch.float64)).float()
+    return (s * f.view(1, D, 1, 1)).contiguous()
+
+
 def broadcast_planes(B, D, H, W):
     """The reference's default planes 1 / linspace(0.0025, 0.33, D) as a (B, D, H, W) broadcast."""
     return O.plane_depths(*INV_RANGE, D).view(1, D, 1, 1).expand(B, D, H, W)

@@ -1,8 +1,9 @@
 """Per-pixel depth hypotheses (data_dict["cv_depths"], monorec_model.py:181-201) through the fused cost-volume kernel.
 
 CPU: the oracle restatements against the reference's outputs (tests/golden/cv_pixel_depths.npz) and the C ABI's argument
-checks.  GPU: the golden cases, bit-for-bit equality with the plane path for broadcast depths, the float64 closed form,
-hypotheses that are not usable, batch independence, the full model, and the module's input checks.
+checks.  GPU: the golden cases, bit-for-bit equality with the plane path for broadcast depths, hypotheses that are not
+usable, batch independence, the full model, and the module's input checks.  The per-pixel path against the float64 closed
+form, at the kernel's own accuracy, is in tests/test_cv_accuracy_gpu.py.
 """
 import ctypes
 
@@ -215,51 +216,6 @@ def test_broadcast_equals_plane_path_bitwise(shape):
         assert torch.equal(sf0, sf1), (shape, dt, (sf0 - sf1).abs().max().item())
         if dt is not None:
             assert torch.equal(nh0, nh1), (shape, dt)
-
-
-def _step_depths(B, D, H, W, z_near=2.0, z_far=30.0, rel=4.0):
-    # (a far side at hundreds of metres has flat costs over the whole band: its view weights vanish and the fused value is
-    # a ratio of rounding noise in the reference formula itself; 30 m keeps the fused volume comparable)
-    s = torch.full((B, 1, H, W), z_far)
-    s[..., : int(0.43 * W)] = z_near       # a vertical edge through the middle of a tile column
-    f = torch.exp(torch.linspace(-np.log(rel), np.log(rel), D, dtype=torch.float64)).float()
-    return (s * f.view(1, D, 1, 1)).contiguous()
-
-
-@gpu
-@pytest.mark.parametrize("kind", ["band", "shuffled", "step"])
-def test_against_closed_form(kind):
-    from monorec_b200.synthetic import make_inputs
-    B, F, D, H, W = 1, 4, 32, 256, 512
-    data = make_inputs(B, F, H, W, seed=100)
-    if kind == "band":
-        z = CC.band_depths(B, D, H, W, seed=7, rel=2.0)
-    elif kind == "shuffled":
-        z = CC.shuffled_depths(B, D, H, W, seed=8)
-    else:
-        z = _step_depths(B, D, H, W)
-    out = _module_run(_to(data), z.to(DEV))
-    ref_cv, ref_sf, _, _ = O.cost_volume_closed_form(data, cv_depths=z, dtype=np.float64)
-    ref_cv = torch.from_numpy(ref_cv).float()
-    ref_sf = [torch.from_numpy(s).float() for s in ref_sf]
-    sf = [s.cpu() for s in out["single_frame_cvs"]]
-    print(kind, compare_volumes(out["cost_volume"].cpu(), sf, ref_cv, ref_sf))
-
-    def sf_err(sf, ref):
-        ds = []
-        for a, r in zip(sf, ref):
-            both = ~((a == 0).all(1) | (r == 0).all(1))
-            ds.append(((a - r).double() * both.unsqueeze(1))[both.unsqueeze(1).expand_as(a)])
-        d = torch.cat(ds)
-        return d.abs().max().item(), d.pow(2).mean().sqrt().item()
-
-    # the plane path on the same frames, for scale
-    abi = _Abi(_to(data), D)
-    _, sfp, _ = abi.plane()
-    pcv, psf, _, _ = O.cost_volume_closed_form(data, steps=D, dtype=np.float64)
-    pm = sf_err([s.cpu() for s in sfp], [torch.from_numpy(s).float() for s in psf])
-    m = sf_err(sf, ref_sf)
-    print(f"{kind}: single-frame max / RMS error per-pixel path {m[0]:.2e} / {m[1]:.2e}, plane path {pm[0]:.2e} / {pm[1]:.2e}")
 
 
 @gpu

@@ -1,5 +1,6 @@
 """Property tests of the oracle itself (SURVEY.md §4 item 3), hypothesis-driven on tiny problems (CPU)."""
 import numpy as np
+import pytest
 import torch
 from hypothesis import given, settings, strategies as st
 
@@ -39,6 +40,49 @@ def test_closed_form_agrees_with_torch_restatement(seed):
     both = ~(za | zb)
     assert int((za != zb).sum()) <= 8
     assert ((cv - torch.from_numpy(cvc)).abs() * both.unsqueeze(1)).max() < 1e-3
+
+
+def _margin_cases():
+    from tests import cv_cases as CC
+    yield "planes", make_inputs(2, 3, 24, 41, seed=17), dict(steps=8)
+    yield "planes_d64", make_inputs(1, 2, 37, 61, seed=31), dict(steps=64)
+    for tag in CC.PIXEL_CASES:
+        data, z = CC.make_pixel_case(tag)
+        yield tag, data, dict(cv_depths=z)
+    data, z, D, _, _ = CC.make_matching_case("ssim_l1_band")
+    yield "ssim_l1_band", data, dict(cv_depths=z)
+
+
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+def test_validity_margin_sign_is_the_closed_form_validity(dtype):
+    """`validity_margin > 0` is exactly the closed form's `valid` (the bilinear sample of the interior mask is non-zero
+    strictly inside 1 < s < n-2) on seeded planes and on the golden per-pixel cases, whose wide spans flip validity inside
+    the band; the float32 mode rounds the positions as the closed form does."""
+    for tag, data, kw in _margin_cases():
+        _, _, valid, _ = O.cost_volume_closed_form(data, dtype=dtype, **kw)
+        margin = O.validity_margin(data, dtype=dtype, **kw)
+        assert margin.dtype == np.float64 and margin.shape == valid.shape, tag
+        assert np.array_equal(margin > 0, valid), (tag, int(((margin > 0) != valid).sum()))
+        assert valid.any() and (~valid[..., 2:-2, 2:-2]).any(), tag        # both sides of the edge are reached
+        assert np.isneginf(margin[..., :2, :]).all() and np.isneginf(margin[..., :, -2:]).all(), tag
+
+
+def test_validity_margin_is_the_distance_to_the_edge():
+    """With the keyframe as its own source frame every depth projects pixel (u, v) onto itself, at the source position
+    sx = u W / (W - 1) - 1/2 (point_projection normalises with W - 1, grid_sample un-normalises with W), so the margin is
+    min(sx - 1, W - 2 - sx, sy - 1, H - 2 - sy) of that position."""
+    data = make_inputs(1, 1, 20, 33, seed=3)
+    data = dict(data, frames=[data["keyframe"].clone()], poses=[data["keyframe_pose"].clone()],
+                intrinsics=[data["keyframe_intrinsics"].clone()])
+    m = O.validity_margin(data, steps=4)[0, 0]
+    H, W = m.shape
+    v, u = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    sx = u * W / (W - 1) - 0.5
+    sy = v * H / (H - 1) - 0.5
+    want = np.minimum(np.minimum(sx - 1, W - 2 - sx), np.minimum(sy - 1, H - 2 - sy))
+    inner = np.zeros((H, W), bool)
+    inner[2:-2, 2:-2] = True
+    assert np.allclose(m[inner], want[inner], rtol=0, atol=1e-5)
 
 
 @settings(max_examples=3, deadline=None)
