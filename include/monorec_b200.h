@@ -147,6 +147,20 @@ int mr_cost_volume_fwd_typed(const float* keyframe, const float* const* frames, 
                              int B, int F, int D, int H, int W,
                              float alpha, const float* chan_w, int matching, int centered, int out_dtype, void* stream);
 
+/* mr_cost_volume_fwd_typed on frames of either channel count:
+ *   channels      3: keyframe and frames are [B,3,H,W] and the results are mr_cost_volume_fwd_typed's bit for bit;
+ *                 1: keyframe and frames are [B,1,H,W] grayscale images (a loader's use_color=False, TUM Mono-VO), read as
+ *                 the three-channel images whose three planes equal them: every output is that of the replicated frames
+ *                 bit for bit, from a third of the frame bytes and of the march's taps and SSIM work.
+ *                 Any other value returns MR_EINVAL.
+ * Every other argument as in mr_cost_volume_fwd_typed.  All arguments are checked before the first CUDA call. */
+int mr_cost_volume_fwd_channels(const float* keyframe, const float* const* frames, const float* proj,
+                                const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv,
+                                void* out_sfcv_nhwc, int nhwc_dtype,
+                                int B, int F, int D, int H, int W,
+                                float alpha, const float* chan_w, int matching, int centered, int out_dtype, int channels,
+                                void* stream);
+
 /* Same path with HOST buffers (pinned or pageable): uploads the images and matrices, runs
  * mr_projection_tables + mr_cost_volume_fwd and downloads both volumes; batch elements are pipelined on
  * internal streams so copies overlap the kernel.  This is the end-to-end entry bench.py times as `e2e`.

@@ -38,6 +38,9 @@ SIGNATURES = {
     "mr_cost_volume_fwd_typed": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_int,
                                          c_int, c_int, c_void_p]),
+    "mr_cost_volume_fwd_channels": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                            c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_float_p, c_int,
+                                            c_int, c_int, c_int, c_void_p]),
     "mr_cost_volume_host_workspace": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
     "mr_cost_volume_host_sfcv_offset": (c_longlong, [c_int, c_int, c_int, c_int, c_int]),
     "mr_cost_volume_host": (c_int, [c_void_p] * 8 + [c_int] * 5 + [c_float] * 3 + [c_void_p, c_longlong]),

@@ -43,6 +43,19 @@ def _as_f32c(t):
     return t
 
 
+def check_channels(keyframe, frames):
+    """The images' channel count C: 3, or 1 for grayscale frames (read as their three-channel replicas).  Another C is a
+    NotImplementedError; a frame (mono or stereo) whose C differs from the keyframe's a ValueError."""
+    C = keyframe.shape[1] if keyframe.dim() == 4 else None
+    if C != 3 and C != 1:
+        raise NotImplementedError(f"monorec_b200: images [B,3,H,W] or grayscale [B,1,H,W] only, got a keyframe "
+                                  f"{tuple(keyframe.shape)}")
+    if any(f.dim() != 4 or f.shape[1] != C for f in frames):
+        raise ValueError(f"CostVolumeModule: a keyframe with {C} channel(s) and frames {[tuple(f.shape) for f in frames]}: "
+                         "the keyframe, the mono frames and the stereo frame must all have 3 channels or all 1")
+    return C
+
+
 def fills_nhwc(nhwc, F, B, D, H, W):
     """Whether the kernel writes the MaskModule's NHWC input [F*B,H,W,D] (fp32 or half) beside the volumes."""
     return nhwc is not None and D <= 32 and D % 8 == 0 and tuple(nhwc.shape) == (F * B, H, W, D) \
@@ -56,10 +69,12 @@ def launch(keyframe: Tensor, frames: List[Tensor], intrinsics: List[Tensor], pos
     """Projection tables and the fused cost-volume kernel on contiguous fp32 CUDA inputs -> (cost_volume [B,D,H,W],
     single-frame volumes [F,B,D,H,W]), half when `half`.  D is cv_depths.shape[1] with per-pixel hypotheses, else `steps`
     planes uniform in inverse depth over [lo, hi].  `sfcv_nhwc`, when given, must satisfy `fills_nhwc` and is filled with
-    the single-frame volumes in the MaskModule's layout.  CostVolumeModule.forward calls this directly; under torch.compile
-    it is the implementation of the `monorec_b200::cost_volume` op (monorec_b200/ops.py)."""
+    the single-frame volumes in the MaskModule's layout.  The keyframe and the frames have C = 3 channels, or C = 1
+    (grayscale: the results are those of the frames replicated to three channels, bit for bit); the caller has checked
+    that they agree.  CostVolumeModule.forward calls this directly; under torch.compile it is the implementation of the
+    `monorec_b200::cost_volume` op (monorec_b200/ops.py)."""
     lib = _lib.load()
-    B, _, H, W = keyframe.shape
+    B, C, H, W = keyframe.shape
     F = len(frames)
     D = steps if cv_depths is None else cv_depths.shape[1]
     vdt = torch.float16 if half else torch.float32
@@ -78,7 +93,14 @@ def launch(keyframe: Tensor, frames: List[Tensor], intrinsics: List[Tensor], pos
                                             None if depths is None else depths.data_ptr(), D, lo, hi, stream),
                    "mr_projection_tables")
         cw = (_lib.c_float * 3)(*channel_weights)
-        if half:
+        if C == 1:
+            # grayscale frames: one entry for every error mode, centring, depth source and storage type
+            _lib.check(lib.mr_cost_volume_fwd_channels(
+                keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
+                None if depths is None else depths.data_ptr(), None if cv_depths is None else cv_depths.data_ptr(),
+                cv.data_ptr(), sfcv.data_ptr(), nhwc.data_ptr() if nhwc is not None else None, nhwc_half,
+                B, F, D, H, W, alpha, cw, matching, centre, 1 if half else 0, 1, stream), "mr_cost_volume_fwd_channels")
+        elif half:
             # half volumes: one entry for every error mode, centring and depth source
             _lib.check(lib.mr_cost_volume_fwd_typed(
                 keyframe.data_ptr(), _lib.ptr_array(frames), proj.data_ptr(),
@@ -164,6 +186,8 @@ class CostVolumeModule(nn.Module):
         compiling = torch.compiler.is_compiling()
         start_time = None if compiling else time.time()
         keyframe = _as_f32c(data_dict["keyframe"])
+        frames, intrinsics, poses = self._gather(data_dict)
+        check_channels(keyframe, frames)
         if not keyframe.is_cuda:
             raise _lib.MonorecLibraryError("monorec_b200.CostVolumeModule needs CUDA tensors (no CPU fallback)")
         pixel_depths = None
@@ -171,7 +195,6 @@ class CostVolumeModule(nn.Module):
             pixel_depths = self._check_cv_depths(data_dict["cv_depths"], keyframe)
         if not compiling:
             _lib.load()
-        frames, intrinsics, poses = self._gather(data_dict)
         frames = [_as_f32c(f) for f in frames]
         intrinsics = [_as_f32c(k) for k in intrinsics]
         poses = [_as_f32c(p) for p in poses]
@@ -179,8 +202,6 @@ class CostVolumeModule(nn.Module):
         kK = _as_f32c(data_dict["keyframe_intrinsics"])
         B, C, H, W = keyframe.shape
         F = len(frames)
-        if C != 3:
-            raise NotImplementedError("monorec_b200: 3-channel images only")
         if pixel_depths is not None:
             lo, hi, D = 0.0, 0.0, pixel_depths.shape[1]
         else:

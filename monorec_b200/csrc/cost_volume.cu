@@ -9,13 +9,14 @@
 //           source frames.  grid = (ceil(W/60), ceil(H/TH), B).
 //   plan  = per tile and source frame the D planes are cut into groups of consecutive planes whose source footprints
 //           (projective image of the tile rectangle: extremes at its 4 corners) share one window of kPitch x kWinRows
-//           pixels.  A window is the [3][rows][kPitch] fp32 copy of that frame region, brought into shared memory by
-//           TMA boxes {kPitch, 8, 1} straight from the NCHW frame (cp.async.bulk.tensor, mbarrier complete_tx, kBuf
+//           pixels.  A window is the [C][rows][kPitch] fp32 copy of that frame region (C = 3, or 1 for grayscale
+//           frames), brought into shared memory by TMA boxes {kPitch, 8, 1} straight from the NCHW frame
+//           (cp.async.bulk.tensor, mbarrier complete_tx, kBuf
 //           buffers in flight); out-of-image box parts are zero-filled by the TMA unit, which is exactly
 //           F.grid_sample(padding_mode="zeros") once integer tap coordinates are clamped to the 2-px zero ring.
 //   unit  = (frame, plane).  Warps claim units from a shared counter (units of one window are consecutive), wait for
 //           the window's mbarrier, and march down the tile rows:
-//             stage 1 (lane = columns l, l+32): homography, floor by magic-number rounding, 12 bilinear taps per
+//             stage 1 (lane = columns l, l+32): homography, floor by magic-number rounding, 4 C bilinear taps per
 //                      sample as conflict-free LDS from the window (immediate offsets), warped row -> smem row buffer;
 //             stage 2 (lane = columns 2l, 2l+1): 3x3 box sums of X, X^2, XY (horizontal in registers, vertical rolling),
 //                      SSIM in 81x-scaled form, channel weights, second 3x3 box -> 1 - 2 sad streamed to HBM.
@@ -49,9 +50,8 @@ constexpr int kMinBlocks = 1;                     // resident CTAs per SM the re
 constexpr int kBuf = 2;                           // source windows in flight per CTA
 constexpr int kPitch = 128;                       // pixels per window row (512 bytes)
 constexpr int kWinRows = 40;                      // rows per window (multiple of 8)
-constexpr int kChanStride = kWinRows * kPitch;    // floats between the channel planes of a window
-constexpr int kWinFloats = 3 * kChanStride;
-constexpr int kBoxRows = 8;                       // rows per TMA box
+constexpr int kChanStride = kWinRows * kPitch;    // floats between the channel planes of a window (NC of them)
+constexpr int kBoxRows = 8;                      // rows per TMA box
 constexpr int kMinGroup = 3;                      // plane groups smaller than this gather from global memory
 constexpr int kTileRows = 16;                     // tile height when shared memory allows it (halved until it fits)
 static_assert(kWinRows % kBoxRows == 0, "window rows must be a multiple of the TMA box height");
@@ -64,8 +64,8 @@ constexpr int kMagicBits = 0x4B400000;
 constexpr int kChunk = 32;                 // planes the per-pixel phase keeps in registers at once
 
 struct CvArgs {
-    const float* key;                    // [B,3,H,W]
-    const float* frames[MR_MAX_FRAMES];  // each [B,3,H,W]
+    const float* key;                    // [B,C,H,W], C = the kernel's channel count NC (3, or 1 for grayscale frames)
+    const float* frames[MR_MAX_FRAMES];  // each [B,C,H,W]
     const float* proj;                   // [B,F,12]
     const float* depths;                 // [D]
     void* cv;                            // [B,D,H,W] in the kernel's storage type OUT (fp32 or IEEE half)
@@ -79,7 +79,7 @@ struct CvArgs {
 };
 
 struct CvMaps {
-    CUtensorMap m[MR_MAX_FRAMES];        // frame f as a (W, H, 3B) fp32 tensor, box {kPitch, kBoxRows, 1}, zero fill
+    CUtensorMap m[MR_MAX_FRAMES];        // frame f as a (W, H, C B) fp32 tensor, box {kPitch, kBoxRows, 1}, zero fill
 };
 
 struct GroupInfo {                       // one window (a run of consecutive planes of one frame)
@@ -97,20 +97,26 @@ struct SmemLayout {
     int total;
 };
 
-constexpr int kXbWarpFloats = 2 * 3 * kRowStride;  // a warp's two warped-row buffers
 constexpr int kLSlotFloats = 3 * 64;              // kErrSsimL1: a warp's carried L1 terms, three float2 per lane (ssim_row)
+
+// Every channel-dependent size is NC (1 or 3) planes of its one-plane size: the windows, the keyframe tile, the hoisted
+// SSIM table and the warped-row buffers.  The geometry (window rows, tile rows) is the same for both channel counts.
+// A warp's two warped-row buffers:
+__host__ __device__ constexpr int xb_warp_floats(int nc) { return 2 * nc * kRowStride; }
 
 // pix: the per-pixel depth source (cv_depths) appends its two depth tables; the plane layout is unchanged.
 // err: the error mode (MR_CV_*).  MR_CV_SSIM_L1 warps keep kLSlotFloats behind their row buffers; MR_CV_BOX_L1 reads no
-// hoisted SSIM table, so its cst region is empty
+// hoisted SSIM table, so its cst region is empty.  NC: the frames' channel count (a template parameter: the kernel's
+// offsets are then the constant expressions of the three-channel layout, which keeps its code unchanged)
+template <int NC>
 __host__ __device__ inline SmemLayout make_layout(int D, int TH, int F, int use_tma, bool pix = false, int err = MR_CV_SSIM) {
     SmemLayout L;
     int off = 0;
     auto take = [&](int bytes, int align) { off = (off + align - 1) / align * align; int o = off; off += bytes; return o; };
-    L.win = take(use_tma ? kBuf * kWinFloats * 4 : 0, 128);
-    L.ytile = take(3 * (TH + 4) * kRowStride * 4, 16);
-    L.cst = take(err == MR_CV_BOX_L1 ? 0 : 3 * (TH + 2) * kTileCols * 8, 16);
-    L.xbuf = take(kWarps * (kXbWarpFloats + (err == MR_CV_SSIM_L1 ? kLSlotFloats : 0)) * 4, 16);
+    L.win = take(use_tma ? kBuf * (NC * kChanStride) * 4 : 0, 128);
+    L.ytile = take(NC * (TH + 4) * kRowStride * 4, 16);
+    L.cst = take(err == MR_CV_BOX_L1 ? 0 : NC * (TH + 2) * kTileCols * 8, 16);
+    L.xbuf = take(kWarps * (xb_warp_floats(NC) + (err == MR_CV_SSIM_L1 ? kLSlotFloats : 0)) * 4, 16);
     L.pjs = take(F * 12 * 4, 16);
     L.zs = take(((D + 3) / 4) * 16, 16);
     L.vmask = take(F * TH * kTileCols, 16);
@@ -241,16 +247,17 @@ __device__ __forceinline__ void sts64(uint32_t a, float2 v) {
     asm volatile("st.shared.v2.f32 [%0+%1], {%2, %3};" ::"r"(a), "n"(OFF), "f"(v.x), "f"(v.y) : "memory");
 }
 
-constexpr int kXbBytes = 3 * kRowStride * 4;      // one warped-row buffer (3 channels)
-constexpr int kYRowBytes = 3 * kRowStride * 4;    // keyframe tile: [row][channel][kRowStride]
-constexpr int kCRowBytes = 3 * (kTileCols / 2) * 16;  // hoisted table: [e-row][channel][32 column pairs] float4
+// per channel plane (NC of them in each):
+constexpr int kXbBytes = kRowStride * 4;          // one warped-row buffer: [channel][kRowStride]
+constexpr int kYRowBytes = kRowStride * 4;        // keyframe tile: [row][channel][kRowStride]
+constexpr int kCRowBytes = (kTileCols / 2) * 16;  // hoisted table: [e-row][channel][32 column pairs] float4
 
-// ---- stage 1 of the march: homography of one tile row (pair = columns lane, lane + 32) and its 24 bilinear taps -------
+// ---- stage 1 of the march: homography of one tile row (pair = columns lane, lane + 32) and its 8 NC bilinear taps -----
 struct Stage1Ctx {
     float2 pzx, pzy, pzz;                // per-lane column part of the projection (already times the plane depth)
     float rax, rbx, ray, rby, raz, rbz;  // per-row part: c = pz(u) + ra * v + rb
     uint32_t kaddr;                      // window modes: shared address of the window minus the unit's constant (see march)
-    const float* img;                    // global mode: source frame of this batch element, [3][H][W]
+    const float* img;                    // global mode: source frame of this batch element, [NC][H][W]
     int W, H, planei;
     float sx_lo, sx_hi, sy_lo, sy_hi;    // == grid clamp(-2, 2) + 0.5, monorec_model.py:208
     // per-pixel depths only: the depth changes from sample to sample, so setup_stage1's products are formed per sample
@@ -298,8 +305,9 @@ __device__ __forceinline__ void bilinear_weights(float ux, float uy, float x0f, 
     w00 = __fmul_rn(wx0, wy0); w01 = __fmul_rn(wx1, wy0); w10 = __fmul_rn(wx0, wy1); w11 = __fmul_rn(wx1, wy1);
 }
 
-struct Taps {                            // the 24 taps and 4 weight pairs of one row step (two samples per lane)
-    float a[3][4], b[3][4];              // [channel][nw, ne, sw, se] of the sample at column lane / lane + 32
+template <int NC>
+struct Taps {                            // the 8 NC taps and 4 weight pairs of one row step (two samples per lane)
+    float a[NC][4], b[NC][4];            // [channel][nw, ne, sw, se] of the sample at column lane / lane + 32
     float2 w00, w01, w10, w11;
 };
 
@@ -307,8 +315,10 @@ struct Taps {                            // the 24 taps and 4 weight pairs of on
 // MODE 1: taps from the window, coordinates clamped to the 2-px zero ring (== zero padding of F.grid_sample)
 // MODE 2: taps from global memory with per-tap zero padding
 // PIX: z = the depths of the lane's two samples in this row (per-pixel depth source); unused for the plane table
-template <int MODE, bool PIX = false>
-__device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float fv, Taps& t, const float2 z = float2{}) {
+// NC: channels of the frames.  The weights do not depend on the channel, so a one-channel frame's taps are those of each
+// plane of its three-channel replica.
+template <int MODE, bool PIX, int NC>
+__device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float fv, Taps<NC>& t, const float2 z = float2{}) {
     float inv[2], ux[2], uy[2];
     if constexpr (!PIX) {
         const float rcx = fmaf(c.rax, fv, c.rbx), rcy = fmaf(c.ray, fv, c.rby), rcz = fmaf(c.raz, fv, c.rbz);
@@ -358,7 +368,7 @@ __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float f
         }
         static_assert(kPitch == 128, "the tap address uses a shift by 7");
 #pragma unroll
-        for (int ch = 0; ch < 3; ++ch) {
+        for (int ch = 0; ch < NC; ++ch) {
             // (ch is a compile-time constant after unrolling: the offsets are immediates)
             if (ch == 0) {
                 t.a[0][0] = lds32<0>(aa); t.a[0][1] = lds32<4>(aa); t.a[0][2] = lds32<kPitch * 4>(aa); t.a[0][3] = lds32<kPitch * 4 + 4>(aa);
@@ -412,7 +422,7 @@ __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float f
             oa = os[0]; ob = os[1]; dxa = dxs[0]; dxb = dxs[1]; dya = dys[0]; dyb = dys[1];
         }
 #pragma unroll
-        for (int ch = 0; ch < 3; ++ch) {
+        for (int ch = 0; ch < NC; ++ch) {
             const float* pa0 = c.img + (oa + ch * c.planei);
             const float* pb0 = c.img + (ob + ch * c.planei);
             t.a[ch][0] = __ldg(pa0); t.a[ch][1] = __ldg(pa0 + dxa); t.a[ch][2] = __ldg(pa0 + dya); t.a[ch][3] = __ldg(pa0 + dya + dxa);
@@ -423,10 +433,11 @@ __device__ __forceinline__ void warp_row_issue(const Stage1Ctx& c, const float f
 
 // interpolation (same order as grid_sample: nw, ne, sw, se; + 0.5: monorec_model.py:231) and the warped row -> row buffer
 // xw = shared address of this lane's first column in the row buffer to fill
-__device__ __forceinline__ void warp_row_finish(const Taps& t, const uint32_t xw) {
-    float va[3], vb[3];
+template <int NC>
+__device__ __forceinline__ void warp_row_finish(const Taps<NC>& t, const uint32_t xw) {
+    float va[NC], vb[NC];
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
+    for (int ch = 0; ch < NC; ++ch) {
         float a = fmaf(t.a[ch][0], t.w00.x, 0.5f), b = fmaf(t.b[ch][0], t.w00.y, 0.5f);
         a = fmaf(t.a[ch][1], t.w01.x, a); b = fmaf(t.b[ch][1], t.w01.y, b);
         a = fmaf(t.a[ch][2], t.w10.x, a); b = fmaf(t.b[ch][2], t.w10.y, b);
@@ -434,8 +445,10 @@ __device__ __forceinline__ void warp_row_finish(const Taps& t, const uint32_t xw
         va[ch] = a; vb[ch] = b;
     }
     sts32<0>(xw, va[0]);                  sts32<128>(xw, vb[0]);
-    sts32<kRowStride * 4>(xw, va[1]);     sts32<kRowStride * 4 + 128>(xw, vb[1]);
-    sts32<2 * kRowStride * 4>(xw, va[2]); sts32<2 * kRowStride * 4 + 128>(xw, vb[2]);
+    if constexpr (NC == 3) {
+        sts32<kRowStride * 4>(xw, va[1]);     sts32<kRowStride * 4 + 128>(xw, vb[1]);
+        sts32<2 * kRowStride * 4>(xw, va[2]); sts32<2 * kRowStride * 4 + 128>(xw, vb[2]);
+    }
 }
 
 // ---- stage 2 of the march: SSIM + patch cost of one row; lane owns buffer columns 2l, 2l+1 (a pair) ---------------------
@@ -454,31 +467,37 @@ struct Stage2Ctx {
 };
 
 // rolling state: horizontal 3-sums of X, X^2, XY per channel for the last rows, indexed by (row step mod 3) so that no
-// register moves are needed.  kErrBoxL1 keeps horizontal 3-sums of |X - Y| instead.
-template <int ERR>
+// register moves are needed.  kErrBoxL1 keeps horizontal 3-sums of |X - Y| instead.  [row slot][channel]
+template <int ERR, int NC>
 struct Stage2State {
-    float2 hs1[3][3], hsx[3][3], hsy[3][3], hE[3];
+    float2 hs1[3][NC], hsx[3][NC], hsy[3][NC], hE[3];
     __device__ __forceinline__ void clear() {
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
             hE[i] = bc2(0.f);
 #pragma unroll
-            for (int c = 0; c < 3; ++c) hs1[i][c] = hsx[i][c] = hsy[i][c] = bc2(0.f);
+            for (int c = 0; c < NC; ++c) hs1[i][c] = hsx[i][c] = hsy[i][c] = bc2(0.f);
         }
     }
 };
-template <>
-struct Stage2State<kErrBoxL1> {
-    float2 hd[3][3], hE[3];
+template <int NC>
+struct Stage2State<kErrBoxL1, NC> {
+    float2 hd[3][NC], hE[3];
     __device__ __forceinline__ void clear() {
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
             hE[i] = bc2(0.f);
 #pragma unroll
-            for (int c = 0; c < 3; ++c) hd[i][c] = bc2(0.f);
+            for (int c = 0; c < NC; ++c) hd[i][c] = bc2(0.f);
         }
     }
 };
+
+// The channel whose error enters the channel-weighted sum with weight k (k = 0, 1, 2).  A one-channel frame stands for
+// three equal planes: its error enters with all three weights, in the three-channel sum's own expression
+// fmaf(w2, e, fmaf(w1, e, w0 * e)), so its cost is the replicated frame's bit for bit.
+template <int NC>
+__host__ __device__ constexpr int wchan(int k) { return NC == 1 ? 0 : k; }
 
 // Patch cost of one row step, common to every error mode: E is the channel-weighted error of the lane's two columns in the
 // row whose error was just finished; its horizontal 3-sum joins the two rows before it in hE (rolling like Stage2State).
@@ -510,45 +529,55 @@ __device__ __forceinline__ void patch_cost_row(float2 (&hE)[3], const Stage2Ctx&
 // ERR: kErrSsim or kErrSsimL1 (kErrBoxL1 is box_l1_row below).  The row buffer and the keyframe tile both hold values
 // + 0.5, so the |X - Y| of kErrSsimL1 and kErrBoxL1 is |(w + .5) - (k + .5)|: it differs from the reference's |w - k| by the
 // rounding of the two additions (of order 1e-7).
-template <int P, int ERR, typename OUT>
-__device__ __forceinline__ void ssim_row(Stage2State<ERR>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
+template <int P, int ERR, int NC, typename OUT>
+__device__ __forceinline__ void ssim_row(Stage2State<ERR, NC>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
                                          const uint32_t cr, OUT* out, const bool store, const uint32_t xb) {
     constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
-    float2 xl[3], xrr[3], yl[3], yrr[3];
-    float4 k4[3];
+    float2 xl[NC], xrr[NC], yl[NC], yrr[NC];
+    float4 k4[NC];
     xl[0] = lds64<0>(xr);                  xrr[0] = lds64<8>(xr);
-    xl[1] = lds64<kRowStride * 4>(xr);     xrr[1] = lds64<kRowStride * 4 + 8>(xr);
-    xl[2] = lds64<2 * kRowStride * 4>(xr); xrr[2] = lds64<2 * kRowStride * 4 + 8>(xr);
+    if constexpr (NC == 3) {
+        xl[1] = lds64<kRowStride * 4>(xr);     xrr[1] = lds64<kRowStride * 4 + 8>(xr);
+        xl[2] = lds64<2 * kRowStride * 4>(xr); xrr[2] = lds64<2 * kRowStride * 4 + 8>(xr);
+    }
     yl[0] = lds64<0>(yr);                  yrr[0] = lds64<8>(yr);
-    yl[1] = lds64<kRowStride * 4>(yr);     yrr[1] = lds64<kRowStride * 4 + 8>(yr);
-    yl[2] = lds64<2 * kRowStride * 4>(yr); yrr[2] = lds64<2 * kRowStride * 4 + 8>(yr);
-    k4[0] = lds128<0>(cr); k4[1] = lds128<512>(cr); k4[2] = lds128<1024>(cr);
+    if constexpr (NC == 3) {
+        yl[1] = lds64<kRowStride * 4>(yr);     yrr[1] = lds64<kRowStride * 4 + 8>(yr);
+        yl[2] = lds64<2 * kRowStride * 4>(yr); yrr[2] = lds64<2 * kRowStride * 4 + 8>(yr);
+        k4[0] = lds128<0>(cr); k4[1] = lds128<512>(cr); k4[2] = lds128<1024>(cr);
+    } else {
+        k4[0] = lds128<0>(cr);
+    }
     // horizontal 3-sums of X, X^2, XY: the middle pair (columns 2l, 2l+1) is shared by both columns of the lane, and every
     // product is folded into an FFMA of its sum
-    float2 h1[3], hx[3], hy[3];
+    float2 h1[NC], hx[NC], hy[NC];
     float2 L;   // kErrSsimL1: sum_c w_c |X - Y|_c of columns 2l, 2l+1, formed channel by channel while their values are loaded
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
+    for (int ch = 0; ch < NC; ++ch) {
         const float2 l = xl[ch], r = xrr[ch], ly = yl[ch], ry = yrr[ch];
         const float m1 = l.y + r.x, mx = fmaf(l.y, l.y, r.x * r.x), my = fmaf(l.y, ly.y, r.x * ry.x);
         h1[ch] = make_float2(l.x + m1, m1 + r.y);
         hx[ch] = make_float2(fmaf(l.x, l.x, mx), fmaf(r.y, r.y, mx));
         hy[ch] = make_float2(fmaf(l.x, ly.x, my), fmaf(r.y, ry.y, my));
         if constexpr (ERR == kErrSsimL1) {
-            const float2 w = ch == 0 ? c.cw0 : ch == 1 ? c.cw1 : c.cw2;
             const float2 d = make_float2(fabsf(l.y - ly.y), fabsf(r.x - ry.x));
-            L = ch == 0 ? make_float2(w.x * d.x, w.y * d.y) : make_float2(fmaf(w.x, d.x, L.x), fmaf(w.y, d.y, L.y));
+            // (one channel: its difference enters with all three weights, see wchan)
+#pragma unroll
+            for (int k = ch; k < (NC == 1 ? 3 : ch + 1); ++k) {
+                const float2 w = k == 0 ? c.cw0 : k == 1 ? c.cw1 : c.cw2;
+                L = k == 0 ? make_float2(w.x * d.x, w.y * d.y) : make_float2(fmaf(w.x, d.x, L.x), fmaf(w.y, d.y, L.y));
+            }
         }
     }
     if constexpr (ERR == kErrSsimL1) {
         // kErrSsimL1: the row's 0.15 L waits one step in the lane's shared memory slot P behind the warp's row buffers,
         // until this row's SSIM is finished.  (Carried in registers, or in one slot that is read before it is rewritten,
         // it pushed the per-pixel gather march into local memory.)
-        sts64<2 * kXbBytes + 256 * P>(xb, make_float2(0.15f * L.x, 0.15f * L.y));
+        sts64<2 * NC * kXbBytes + 256 * P>(xb, make_float2(0.15f * L.x, 0.15f * L.y));
     }
-    float e[3][2];
+    float e[NC][2];
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
+    for (int ch = 0; ch < NC; ++ch) {
         // SSIM with every factor scaled by 81 (layers.py:123-137 through 3x3 box sums s = sum x, sxx, sxy; Y = 9 mu_y,
         // Sg = 81 (sigma_y + C2) hoisted):  n/d = (2 s Y + 81 C1)(2 (9 sxy - s Y) + 81 C2) / ((s^2 + Y^2 + 81 C1)(9 sxx - s^2 + Sg))
         const float Y[2] = {k4[ch].x, k4[ch].y}, Sg[2] = {k4[ch].z, k4[ch].w};
@@ -569,53 +598,59 @@ __device__ __forceinline__ void ssim_row(Stage2State<ERR>& st, const Stage2Ctx& 
         }
     }
     float2 E;
+    constexpr int c1 = wchan<NC>(1), c2 = wchan<NC>(2);
     if constexpr (ERR == kErrSsimL1) {
         // 0.85 SSIM + 0.15 |X - Y| per channel (monorec_model.py:237-241), channel-weighted as sums of their own; the L1
         // sum of the SSIM row is the one the previous step stored
-        const float2 Lp = lds64<2 * kXbBytes + 256 * P2>(xb);
-        E = make_float2(fmaf(0.85f, fmaf(c.cw2.x, e[2][0], fmaf(c.cw1.x, e[1][0], c.cw0.x * e[0][0])), Lp.x),
-                        fmaf(0.85f, fmaf(c.cw2.y, e[2][1], fmaf(c.cw1.y, e[1][1], c.cw0.y * e[0][1])), Lp.y));
+        const float2 Lp = lds64<2 * NC * kXbBytes + 256 * P2>(xb);
+        E = make_float2(fmaf(0.85f, fmaf(c.cw2.x, e[c2][0], fmaf(c.cw1.x, e[c1][0], c.cw0.x * e[0][0])), Lp.x),
+                        fmaf(0.85f, fmaf(c.cw2.y, e[c2][1], fmaf(c.cw1.y, e[c1][1], c.cw0.y * e[0][1])), Lp.y));
     } else {
-        E = make_float2(fmaf(c.cw2.x, e[2][0], fmaf(c.cw1.x, e[1][0], c.cw0.x * e[0][0])),
-                        fmaf(c.cw2.y, e[2][1], fmaf(c.cw1.y, e[1][1], c.cw0.y * e[0][1])));
+        E = make_float2(fmaf(c.cw2.x, e[c2][0], fmaf(c.cw1.x, e[c1][0], c.cw0.x * e[0][0])),
+                        fmaf(c.cw2.y, e[c2][1], fmaf(c.cw1.y, e[c1][1], c.cw0.y * e[0][1])));
     }
     patch_cost_row<P>(st.hE, c, E, out, store);
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) { st.hs1[P][ch] = h1[ch]; st.hsx[P][ch] = hx[ch]; st.hsy[P][ch] = hy[ch]; }
+    for (int ch = 0; ch < NC; ++ch) { st.hs1[P][ch] = h1[ch]; st.hsx[P][ch] = hx[ch]; st.hsy[P][ch] = hy[ch]; }
 }
 
 // kErrBoxL1: horizontal 3-sums of |X - Y| of the new row, their vertical 3-sum over the rolling rows (the 3x3 box of the
 // row above, at the step where the SSIM modes finish that row's SSIM), patch cost of the row above that
-template <int P, typename OUT>
-__device__ __forceinline__ void box_l1_row(Stage2State<kErrBoxL1>& st, const Stage2Ctx& c, const uint32_t xr,
+template <int P, int NC, typename OUT>
+__device__ __forceinline__ void box_l1_row(Stage2State<kErrBoxL1, NC>& st, const Stage2Ctx& c, const uint32_t xr,
                                            const uint32_t yr, OUT* out, const bool store) {
     constexpr int P1 = (P + 1) % 3, P2 = (P + 2) % 3;
-    float2 xl[3], xrr[3], yl[3], yrr[3];
+    float2 xl[NC], xrr[NC], yl[NC], yrr[NC];
     xl[0] = lds64<0>(xr);                  xrr[0] = lds64<8>(xr);
-    xl[1] = lds64<kRowStride * 4>(xr);     xrr[1] = lds64<kRowStride * 4 + 8>(xr);
-    xl[2] = lds64<2 * kRowStride * 4>(xr); xrr[2] = lds64<2 * kRowStride * 4 + 8>(xr);
+    if constexpr (NC == 3) {
+        xl[1] = lds64<kRowStride * 4>(xr);     xrr[1] = lds64<kRowStride * 4 + 8>(xr);
+        xl[2] = lds64<2 * kRowStride * 4>(xr); xrr[2] = lds64<2 * kRowStride * 4 + 8>(xr);
+    }
     yl[0] = lds64<0>(yr);                  yrr[0] = lds64<8>(yr);
-    yl[1] = lds64<kRowStride * 4>(yr);     yrr[1] = lds64<kRowStride * 4 + 8>(yr);
-    yl[2] = lds64<2 * kRowStride * 4>(yr); yrr[2] = lds64<2 * kRowStride * 4 + 8>(yr);
-    float2 hd[3], v[3];
+    if constexpr (NC == 3) {
+        yl[1] = lds64<kRowStride * 4>(yr);     yrr[1] = lds64<kRowStride * 4 + 8>(yr);
+        yl[2] = lds64<2 * kRowStride * 4>(yr); yrr[2] = lds64<2 * kRowStride * 4 + 8>(yr);
+    }
+    float2 hd[NC], v[NC];
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) {
+    for (int ch = 0; ch < NC; ++ch) {
         const float2 l = xl[ch], r = xrr[ch], ly = yl[ch], ry = yrr[ch];
         const float m = fabsf(l.y - ly.y) + fabsf(r.x - ry.x);
         hd[ch] = make_float2(fabsf(l.x - ly.x) + m, m + fabsf(r.y - ry.y));
         v[ch] = make_float2((st.hd[P1][ch].x + st.hd[P2][ch].x) + hd[ch].x, (st.hd[P1][ch].y + st.hd[P2][ch].y) + hd[ch].y);
     }
     // (the box's 1/9 is folded into the channel weights)
-    const float2 E = make_float2(fmaf(c.cw2.x, v[2].x, fmaf(c.cw1.x, v[1].x, c.cw0.x * v[0].x)),
-                                 fmaf(c.cw2.y, v[2].y, fmaf(c.cw1.y, v[1].y, c.cw0.y * v[0].y)));
+    constexpr int c1 = wchan<NC>(1), c2 = wchan<NC>(2);
+    const float2 E = make_float2(fmaf(c.cw2.x, v[c2].x, fmaf(c.cw1.x, v[c1].x, c.cw0.x * v[0].x)),
+                                 fmaf(c.cw2.y, v[c2].y, fmaf(c.cw1.y, v[c1].y, c.cw0.y * v[0].y)));
     patch_cost_row<P>(st.hE, c, E, out, store);
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) st.hd[P][ch] = hd[ch];
+    for (int ch = 0; ch < NC; ++ch) st.hd[P][ch] = hd[ch];
 }
 
 // xb: the lane's address in the warp's first row buffer (xr without the buffer toggle)
-template <int P, int ERR, typename OUT>
-__device__ __forceinline__ void stage2_row(Stage2State<ERR>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
+template <int P, int ERR, int NC, typename OUT>
+__device__ __forceinline__ void stage2_row(Stage2State<ERR, NC>& st, const Stage2Ctx& c, const uint32_t xr, const uint32_t yr,
                                            const uint32_t cr, OUT* out, const bool store, const uint32_t xb) {
     if constexpr (ERR == kErrBoxL1) box_l1_row<P>(st, c, xr, yr, out, store);
     else ssim_row<P, ERR>(st, c, xr, yr, cr, out, store, xb);
@@ -627,17 +662,18 @@ __device__ __forceinline__ void stage2_row(Stage2State<ERR>& st, const Stage2Ctx
 //   xb: shared address of this warp's two row buffers; yr / cr: keyframe row rlo-2 / table row rlo-2 (lane columns);
 //   out: single-frame volume at output row rlo - 4 (advanced every step, stored from the fifth step on); wstride = W
 //   PIX: per-pixel depths, read from image row v0 (= fv0) on; each row's depths are loaded one row step before they are used
-//   ERR: the error mode of stage 2; OUT: the storage type of the single-frame volume
-template <int MODE, bool PIX, int ERR, typename OUT>
+//   ERR: the error mode of stage 2; NC: the channels of the frames; OUT: the storage type of the single-frame volume
+template <int MODE, bool PIX, int ERR, int NC, typename OUT>
 __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx& c2, const uint32_t xb, const int lane,
                                            const float fv0, const int nsteps, uint32_t yr, uint32_t cr, OUT* out,
                                            const int wstride, const int v0 = 0) {
-    Stage2State<ERR> st;
+    constexpr uint32_t kXb = NC * kXbBytes;   // one warped-row buffer
+    Stage2State<ERR, NC> st;
     st.clear();
     if constexpr (ERR == kErrSsimL1) {   // the L1 slots start at 0 like st
-        sts64<2 * kXbBytes>(xb + 8 * lane, bc2(0.f));
-        sts64<2 * kXbBytes + 256>(xb + 8 * lane, bc2(0.f));
-        sts64<2 * kXbBytes + 512>(xb + 8 * lane, bc2(0.f));
+        sts64<2 * kXb>(xb + 8 * lane, bc2(0.f));
+        sts64<2 * kXb + 256>(xb + 8 * lane, bc2(0.f));
+        sts64<2 * kXb + 512>(xb + 8 * lane, bc2(0.f));
     }
     float fv = fv0;
     uint32_t off = 0;                      // byte offset of the row buffer stage 2 reads next
@@ -646,13 +682,13 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
     float2 zn{};
     if constexpr (PIX) zn = load_row_depths(c1, v0);
     {
-        Taps t;
+        Taps<NC> t;
         if constexpr (PIX) {
             const float2 zc = zn;
             zn = load_row_depths(c1, zv);
             warp_row_issue<MODE, true>(c1, fv, t, zc);
         } else {
-            warp_row_issue<MODE>(c1, fv, t);
+            warp_row_issue<MODE, false>(c1, fv, t);
         }
         warp_row_finish(t, xw);
     }
@@ -662,22 +698,22 @@ __device__ __forceinline__ void march_unit(const Stage1Ctx& c1, const Stage2Ctx&
     int done = 0;                          // rows stage 2 has consumed
     auto both = [&](auto tag) {
         fv += 1.0f;
-        Taps tp;
+        Taps<NC> tp;
         if constexpr (PIX) {
             const float2 zc = zn;
             zn = load_row_depths(c1, ++zv);
             warp_row_issue<MODE, true>(c1, fv, tp, zc);
         } else {
-            warp_row_issue<MODE>(c1, fv, tp);
+            warp_row_issue<MODE, false>(c1, fv, tp);
         }
         // stage 1 of row t+1 completes before stage 2 of row t: measured faster than keeping the taps in flight across
         // stage 2 (1.07 against 1.12 ms)
-        warp_row_finish(tp, xw + (kXbBytes - off));
+        warp_row_finish(tp, xw + (kXb - off));
         stage2_row<decltype(tag)::value, ERR>(st, c2, xr + off, yr, cr, out, done >= 4, xr);
         __syncwarp();
-        off = kXbBytes - off;
-        yr += kYRowBytes;
-        cr += kCRowBytes;
+        off = kXb - off;
+        yr += NC * kYRowBytes;
+        cr += NC * kCRowBytes;
         // (kErrSsimL1: the stride as an unsigned step, whose high word is the constant 0: the signed step's high word held a
         // register across the loop, and the per-pixel gather march spilled it)
         if constexpr (ERR == kErrSsimL1) out += (size_t)(uint32_t)wstride;
@@ -851,11 +887,14 @@ __device__ __forceinline__ void pixel_phase(const PixelPhase& c) {
 // per plane and pixel (a.depths = cv_depths [B,D,H,W]).  ERR is the error mode of stage 2 (use_ssim), CENTER false stores the
 // uncentred fused volume (not_center_cv).  OUT is the storage type of both volumes: float, or __half (the march and the
 // per-pixel phase compute in fp32 either way; only the stores round, and the per-pixel phase widens what it reads back).
-template <bool PIX, int ERR, bool CENTER, typename OUT>
+// NC is the channel count of the keyframe and the frames: 3, or 1 for a grayscale stream, whose outputs are those of its
+// three-channel replica bit for bit (see wchan).
+template <bool PIX, int ERR, bool CENTER, typename OUT, int NC>
 __global__ void __launch_bounds__(kThreads, kMinBlocks)
 cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
+    static_assert(NC == 1 || NC == 3, "frames have 1 or 3 channels");
     extern __shared__ __align__(128) unsigned char smem[];
-    const SmemLayout L = make_layout(a.D, a.TH, a.F, a.use_tma, PIX, ERR);
+    const SmemLayout L = make_layout<NC>(a.D, a.TH, a.F, a.use_tma, PIX, ERR);
     float* win = reinterpret_cast<float*>(smem + L.win);
     float* ytile = reinterpret_cast<float*>(smem + L.ytile);
     float* cst = reinterpret_cast<float*>(smem + L.cst);
@@ -881,12 +920,12 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     const int v0 = blockIdx.y * TH;            // image row of tile row 0
     const size_t plane = (size_t)H * W;
     const int planei = H * W;
-    float* xbuf = reinterpret_cast<float*>(smem + L.xbuf) + warp * (kXbWarpFloats + (ERR == kErrSsimL1 ? kLSlotFloats : 0));
+    float* xbuf = reinterpret_cast<float*>(smem + L.xbuf) + warp * (xb_warp_floats(NC) + (ERR == kErrSsimL1 ? kLSlotFloats : 0));
 
     // ---- keyframe tile (+0.5, monorec_model.py:232) and hoisted SSIM terms -------------------------------------
-    const float* key = a.key + (size_t)b * 3 * plane;
-    for (int line = warp; line < 3 * (TH + 4); line += kWarps) {      // line = (tile row + 2) * 3 + channel
-        const int rr = line / 3, ch = line - 3 * rr;
+    const float* key = a.key + (size_t)b * NC * plane;
+    for (int line = warp; line < NC * (TH + 4); line += kWarps) {     // line = (tile row + 2) * NC + channel
+        const int rr = line / NC, ch = line - NC * rr;
         const int v = v0 - 2 + rr;
         const float* src = key + ch * plane + (size_t)v * W;
 #pragma unroll
@@ -943,10 +982,10 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             if (lane == 0) zrow[line] = bad ? make_float2(__int_as_float(0x7fc00000), __int_as_float(0x7fc00000)) : make_float2(lo, hi);
         }
     }
-    if (lane < 6) {   // columns -1 and 64 of both row buffers stay zero
-        const int rb = lane / 3, ch = lane % 3;
-        xbuf[(rb * 3 + ch) * kRowStride] = 0.f;
-        xbuf[(rb * 3 + ch) * kRowStride + kTileCols + 1] = 0.f;
+    if (lane < 2 * NC) {   // columns -1 and 64 of both row buffers stay zero
+        const int rb = lane / NC, ch = lane % NC;
+        xbuf[(rb * NC + ch) * kRowStride] = 0.f;
+        xbuf[(rb * NC + ch) * kRowStride + kTileCols + 1] = 0.f;
     }
     if (tid < 2 * F) rowrng[tid] = (tid & 1) ? -1 : TH;
     if (tid < 12 * F) pjs[tid] = __ldg(a.proj + (size_t)b * F * 12 + tid);
@@ -958,7 +997,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     __syncthreads();
     // table entry for the column pair (2j, 2j+1) of e-row er, channel ch: (Y[2j], Y[2j+1], Sg[2j], Sg[2j+1]) with
     // Y = 9 mu_y = sum y, Sg = 81 (sigma_y + C2) = 9 sum y^2 - Y^2 + 81 C2 (kErrBoxL1 reads no table)
-    for (int line = warp; line < (ERR == kErrBoxL1 ? 0 : 3 * (TH + 2)); line += kWarps) {      // line = e-row * 3 + channel
+    for (int line = warp; line < (ERR == kErrBoxL1 ? 0 : NC * (TH + 2)); line += kWarps) {     // line = e-row * NC + channel
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
             const int bc = lane + 32 * k;
@@ -968,7 +1007,7 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             for (int dy = 0; dy < 3; ++dy)
 #pragma unroll
                 for (int dx = 0; dx < 3; ++dx) {
-                    float q = y[dy * 3 * kRowStride + dx];
+                    float q = y[dy * NC * kRowStride + dx];
                     s1 += q;
                     s2 = fmaf(q, q, s2);
                 }
@@ -1140,17 +1179,17 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
     }
     __syncthreads();
 
-    // window `seq` -> buffer seq % kBuf: 3 channel planes of nrows rows, TMA boxes of kBoxRows rows
+    // window `seq` -> buffer seq % kBuf: NC channel planes of nrows rows, TMA boxes of kBoxRows rows
     auto issue_window = [&](int seq) {
         const GroupInfo gi = ginfo[seq2g[seq]];
         const int buf = seq % kBuf;
         const uint32_t bar = bars + 8 * buf;
-        const uint32_t dst = smem_u32(win + (size_t)buf * kWinFloats);
+        const uint32_t dst = smem_u32(win + (size_t)buf * (NC * kChanStride));
         atomicExch(&ctr[2 + kBuf + buf], seq);   // (an atomic, like its readers: a flag, not a data race)
-        mbar_expect_tx(bar, (uint32_t)(3 * gi.nrows * kPitch * 4));
-        for (int ch = 0; ch < 3; ++ch)
+        mbar_expect_tx(bar, (uint32_t)(NC * gi.nrows * kPitch * 4));
+        for (int ch = 0; ch < NC; ++ch)
             for (int r8 = 0; r8 < gi.nrows; r8 += kBoxRows)
-                tma_load_3d(dst + (uint32_t)((ch * kWinRows + r8) * kPitch * 4), &maps.m[gi.f], bar, gi.wx0, gi.wy0 + r8, b * 3 + ch);
+                tma_load_3d(dst + (uint32_t)((ch * kWinRows + r8) * kPitch * 4), &maps.m[gi.f], bar, gi.wx0, gi.wy0 + r8, b * NC + ch);
     };
     if (tid == 0 && a.use_tma) {
         const int nw = ctr[1];
@@ -1194,10 +1233,10 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
         else setup_stage1(c1, pjs + 12 * f, zs[d], fu2);
         const int nsteps = rhi - rlo + 5;
         const float fv0 = (float)(v0 + rlo - 2);
-        const uint32_t yr = ys_s + rlo * kYRowBytes;          // tile row rlo-2 is keyframe-tile row rlo
+        const uint32_t yr = ys_s + rlo * (NC * kYRowBytes);   // tile row rlo-2 is keyframe-tile row rlo
         // the SSIM row of step t is tile row rlo-3+t, whose table row is rlo-2+t (t = 0, 1 read throw-away rows, possibly
         // in front of the table: still inside this CTA's shared memory, see make_layout)
-        const uint32_t cr = cs_s + (rlo - 2) * kCRowBytes;
+        const uint32_t cr = cs_s + (rlo - 2) * (NC * kCRowBytes);
         OUT* out = static_cast<OUT*>(a.sfcv) + (((size_t)f * a.B + b) * D + d) * plane + ((ptrdiff_t)(v0 + rlo - 4) * W + ucol);
         const unsigned g = gid[unit];
         if (g != 0xFFFFu) {
@@ -1212,14 +1251,14 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
                 if (spin > (1u << 22)) __trap();
             }
             mbar_wait(bars + 8 * buf, (uint32_t)((gi.seq / kBuf) & 1));
-            const uint32_t wb = win_s + (uint32_t)buf * (kWinFloats * 4);
+            const uint32_t wb = win_s + (uint32_t)buf * (NC * kChanStride * 4);
             if (uflag[unit] & 2) {
                 // tap address = wb + 4 ((bits(ty) - kMagicBits - wy0) kPitch + bits(tx) - kMagicBits - wx0), mod 2^32
                 c1.kaddr = wb - 4u * ((uint32_t)(kMagicBits + gi.wy0) * kPitch + (uint32_t)(kMagicBits + gi.wx0));
-                march_unit<0, PIX, ERR>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
+                march_unit<0, PIX, ERR, NC>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
             } else {
                 c1.kaddr = wb - 4u * ((uint32_t)(int)gi.wy0 * kPitch + (uint32_t)(int)gi.wx0);
-                march_unit<1, PIX, ERR>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
+                march_unit<1, PIX, ERR, NC>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
             }
             // hand the buffer on: the last unit of the window re-arms it with the window after next
             if (lane == 0) {
@@ -1236,8 +1275,8 @@ cost_volume_kernel(const CvArgs a, const __grid_constant__ CvMaps maps) {
             }
             __syncwarp();
         } else {
-            c1.img = a.frames[f] + (size_t)b * 3 * plane;
-            march_unit<2, PIX, ERR>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
+            c1.img = a.frames[f] + (size_t)b * NC * plane;
+            march_unit<2, PIX, ERR, NC>(c1, c2, xb_s, lane, fv0, nsteps, yr, cr, out, W, v0 + rlo - 2);
         }
     }
     __syncthreads();  // the marching warps' global stores are visible to the whole CTA from here on
@@ -1334,14 +1373,19 @@ __global__ void projection_tables_kernel(const float* kf_pose, const float* kf_K
     }
 }
 
-int pick_tile_rows(int D, int F, int use_tma, bool pix, int err) {
+// the launch's layout for nc channels
+SmemLayout layout_for(int nc, int D, int TH, int F, int use_tma, bool pix, int err) {
+    return nc == 1 ? make_layout<1>(D, TH, F, use_tma, pix, err) : make_layout<3>(D, TH, F, use_tma, pix, err);
+}
+
+int pick_tile_rows(int D, int F, int use_tma, bool pix, int err, int nc) {
     const int limit = 227 * 1024;
     for (int th = kTileRows; th >= 2; th >>= 1)
-        if (make_layout(D, th, F, use_tma, pix, err).total <= limit) return th;
+        if (layout_for(nc, D, th, F, use_tma, pix, err).total <= limit) return th;
     return 0;
 }
 
-template <bool PIX, int ERR, bool CENTER, typename OUT>
+template <bool PIX, int ERR, bool CENTER, typename OUT, int NC>
 int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
     // The opt-in is per function and per device context, so it is remembered per device (bit d: device d; devices from 64 on
     // set it before every launch).  Two threads that both find the bit clear both set the attribute: harmless.
@@ -1350,26 +1394,37 @@ int launch_kernel(dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, con
     MR_CUDA(cudaGetDevice(&dev));
     const unsigned long long bit = dev < 64 ? 1ull << dev : 0ull;
     if ((opted_in.load(std::memory_order_acquire) & bit) == 0) {
-        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX, ERR, CENTER, OUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     227 * 1024));
+        MR_CUDA(cudaFuncSetAttribute(cost_volume_kernel<PIX, ERR, CENTER, OUT, NC>,
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         opted_in.fetch_or(bit, std::memory_order_release);
     }
-    cost_volume_kernel<PIX, ERR, CENTER, OUT><<<grid, kThreads, smem, stream>>>(a, maps);
+    cost_volume_kernel<PIX, ERR, CENTER, OUT, NC><<<grid, kThreads, smem, stream>>>(a, maps);
     MR_LAUNCH_CHECK("cost_volume_kernel");
     return MR_OK;
 }
 
 // the instantiation for (error mode, centring); matching was checked by the caller
-template <bool PIX, typename OUT>
+template <bool PIX, typename OUT, int NC>
 int launch_variant(int matching, int centered, dim3 grid, int smem, cudaStream_t stream, const CvArgs& a, const CvMaps& maps) {
     if (matching == kErrSsimL1)
-        return centered ? launch_kernel<PIX, kErrSsimL1, true, OUT>(grid, smem, stream, a, maps)
-                        : launch_kernel<PIX, kErrSsimL1, false, OUT>(grid, smem, stream, a, maps);
+        return centered ? launch_kernel<PIX, kErrSsimL1, true, OUT, NC>(grid, smem, stream, a, maps)
+                        : launch_kernel<PIX, kErrSsimL1, false, OUT, NC>(grid, smem, stream, a, maps);
     if (matching == kErrBoxL1)
-        return centered ? launch_kernel<PIX, kErrBoxL1, true, OUT>(grid, smem, stream, a, maps)
-                        : launch_kernel<PIX, kErrBoxL1, false, OUT>(grid, smem, stream, a, maps);
-    return centered ? launch_kernel<PIX, kErrSsim, true, OUT>(grid, smem, stream, a, maps)
-                    : launch_kernel<PIX, kErrSsim, false, OUT>(grid, smem, stream, a, maps);
+        return centered ? launch_kernel<PIX, kErrBoxL1, true, OUT, NC>(grid, smem, stream, a, maps)
+                        : launch_kernel<PIX, kErrBoxL1, false, OUT, NC>(grid, smem, stream, a, maps);
+    return centered ? launch_kernel<PIX, kErrSsim, true, OUT, NC>(grid, smem, stream, a, maps)
+                    : launch_kernel<PIX, kErrSsim, false, OUT, NC>(grid, smem, stream, a, maps);
+}
+
+// the instantiation for (depth source, storage type, channels)
+template <int NC>
+int launch_channels(bool pix, int out_dtype, int matching, int centered, dim3 grid, int smem, cudaStream_t stream,
+                    const CvArgs& a, const CvMaps& maps) {
+    if (out_dtype == MR_DT_F16)
+        return pix ? launch_variant<true, __half, NC>(matching, centered, grid, smem, stream, a, maps)
+                   : launch_variant<false, __half, NC>(matching, centered, grid, smem, stream, a, maps);
+    return pix ? launch_variant<true, float, NC>(matching, centered, grid, smem, stream, a, maps)
+               : launch_variant<false, float, NC>(matching, centered, grid, smem, stream, a, maps);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1415,9 +1470,10 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
                            const float* depths, void* out_cv, void* out_sfcv, int B, int F, int D, int H, int W,
                            float alpha, const float* chan_w, int b_begin, int b_count, int gather_only,
                            cudaStream_t stream, void* sf_nhwc, int sf_nhwc_dtype, int per_pixel_depths, int matching,
-                           int centered, int out_dtype) {
+                           int centered, int out_dtype, int channels) {
     MR_REQUIRE(keyframe && frames && proj && depths && out_cv && out_sfcv, "mr_cost_volume_fwd: null pointer");
     MR_REQUIRE(out_dtype == MR_DT_F32 || out_dtype == MR_DT_F16, "mr_cost_volume_fwd: unknown out_dtype %d", out_dtype);
+    MR_REQUIRE(channels == 1 || channels == 3, "mr_cost_volume_fwd: channels must be 1 or 3 (got %d)", channels);
     MR_REQUIRE(b_begin >= 0 && b_count >= 1 && b_begin + b_count <= B, "mr_cost_volume_fwd: bad batch range");
     MR_REQUIRE(B >= 1 && B <= 21845, "mr_cost_volume_fwd: batch %d out of range", B);
     MR_REQUIRE(F >= 1 && F <= MR_MAX_FRAMES, "mr_cost_volume_fwd: 1 <= F <= %d required (got %d)", MR_MAX_FRAMES, F);
@@ -1437,7 +1493,7 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
                "mr_cost_volume_fwd_nhwc: the NHWC copy needs D <= %d, D %% 8 == 0, a 16-byte aligned buffer and an fp32 / half type", kChunk);
     a.sf_nhwc = sf_nhwc; a.sf_nhwc_half = (sf_nhwc_dtype == MR_DT_F16) ? 1 : 0;
     a.B = B; a.F = F; a.D = D; a.H = H; a.W = W; a.b0 = b_begin;
-    // TMA addresses the frames as (W, H, 3B) tensors: the row pitch must be a multiple of 16 bytes and the base 16-byte
+    // TMA addresses the frames as (W, H, C B) tensors: the row pitch must be a multiple of 16 bytes and the base 16-byte
     // aligned; otherwise (ragged widths) every unit takes the global gather of the same kernel.
     CvMaps local{};       // by-value kernel parameter (__grid_constant__): one tensor map per source frame
     a.use_tma = 0;
@@ -1446,7 +1502,7 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
         bool ok = true;
         for (int f = 0; f < F && ok; ++f) {
             if (reinterpret_cast<uintptr_t>(frames[f]) & 15) { ok = false; break; }
-            const cuuint64_t gdim[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)3 * B};
+            const cuuint64_t gdim[3] = {(cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)channels * B};
             const cuuint64_t gstr[2] = {(cuuint64_t)W * 4, (cuuint64_t)H * W * 4};
             const cuuint32_t box[3] = {(cuuint32_t)kPitch, (cuuint32_t)kBoxRows, 1};
             const cuuint32_t estr[3] = {1, 1, 1};
@@ -1461,20 +1517,17 @@ int mr::launch_cost_volume(const float* keyframe, const float* const* frames, co
         }
     }
     const bool pix = per_pixel_depths != 0;
-    a.TH = pick_tile_rows(D, F, a.use_tma, pix, matching);
+    a.TH = pick_tile_rows(D, F, a.use_tma, pix, matching, channels);
     MR_REQUIRE(a.TH > 0, "mr_cost_volume_fwd: no tile height fits shared memory for D=%d F=%d", D, F);
     a.alpha = alpha;
     a.inv_dm1 = (float)(1.0 / (double)(D - 1));
     const float def_w[3] = {5.f / 32.f, 16.f / 32.f, 11.f / 32.f};  // monorec_model.py:133
     const float* cw = chan_w ? chan_w : def_w;
     a.cw0 = cw[0] / 9.f; a.cw1 = cw[1] / 9.f; a.cw2 = cw[2] / 9.f;  // monorec_model.py:141 (weights / patch_size^2)
-    const SmemLayout L = make_layout(D, a.TH, F, a.use_tma, pix, matching);
+    const SmemLayout L = layout_for(channels, D, a.TH, F, a.use_tma, pix, matching);
     dim3 grid((W + kOutCols - 1) / kOutCols, (H + a.TH - 1) / a.TH, b_count);
-    if (out_dtype == MR_DT_F16)
-        return pix ? launch_variant<true, __half>(matching, centered, grid, L.total, stream, a, local)
-                   : launch_variant<false, __half>(matching, centered, grid, L.total, stream, a, local);
-    return pix ? launch_variant<true, float>(matching, centered, grid, L.total, stream, a, local)
-               : launch_variant<false, float>(matching, centered, grid, L.total, stream, a, local);
+    return channels == 1 ? launch_channels<1>(pix, out_dtype, matching, centered, grid, L.total, stream, a, local)
+                         : launch_channels<3>(pix, out_dtype, matching, centered, grid, L.total, stream, a, local);
 }
 
 extern "C" int mr_cost_volume_fwd(const float* keyframe, const float* const* frames, const float* proj,
@@ -1547,11 +1600,13 @@ extern "C" int mr_cost_volume_fwd_matching(const float* keyframe, const float* c
                                   chan_w, 0, B, 0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, pix, matching, centered);
 }
 
-extern "C" int mr_cost_volume_fwd_typed(const float* keyframe, const float* const* frames, const float* proj,
-                                        const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv,
-                                        void* out_sfcv_nhwc, int nhwc_dtype, int B, int F, int D, int H, int W, float alpha,
-                                        const float* chan_w, int matching, int centered, int out_dtype, void* stream) {
-    const char* fn = "mr_cost_volume_fwd_typed";
+namespace {
+// mr_cost_volume_fwd_typed on frames of `channels` channels; fn names the entry in the messages
+int cost_volume_typed(const char* fn, const float* keyframe, const float* const* frames, const float* proj,
+                      const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv, void* out_sfcv_nhwc,
+                      int nhwc_dtype, int B, int F, int D, int H, int W, float alpha, const float* chan_w, int matching,
+                      int centered, int out_dtype, int channels, void* stream) {
+    MR_REQUIRE(channels == 1 || channels == 3, "%s: channels must be 1 or 3 (got %d)", fn, channels);
     MR_REQUIRE(out_dtype == MR_DT_F32 || out_dtype == MR_DT_F16, "%s: out_dtype must be MR_DT_F32 or MR_DT_F16 (got %d)", fn,
                out_dtype);
     const int rc = check_general_args(fn, depths, pixel_depths, nhwc_dtype, F, D, matching, centered);
@@ -1565,5 +1620,24 @@ extern "C" int mr_cost_volume_fwd_typed(const float* keyframe, const float* cons
     const int pix = pixel_depths != nullptr;
     return mr::launch_cost_volume(keyframe, frames, proj, pix ? pixel_depths : depths, out_cv, out_sfcv, B, F, D, H, W, alpha,
                                   chan_w, 0, B, 0, (cudaStream_t)stream, out_sfcv_nhwc, nhwc_dtype, pix, matching, centered,
-                                  out_dtype);
+                                  out_dtype, channels);
+}
+}  // namespace
+
+extern "C" int mr_cost_volume_fwd_typed(const float* keyframe, const float* const* frames, const float* proj,
+                                        const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv,
+                                        void* out_sfcv_nhwc, int nhwc_dtype, int B, int F, int D, int H, int W, float alpha,
+                                        const float* chan_w, int matching, int centered, int out_dtype, void* stream) {
+    return cost_volume_typed("mr_cost_volume_fwd_typed", keyframe, frames, proj, depths, pixel_depths, out_cv, out_sfcv,
+                             out_sfcv_nhwc, nhwc_dtype, B, F, D, H, W, alpha, chan_w, matching, centered, out_dtype, 3, stream);
+}
+
+extern "C" int mr_cost_volume_fwd_channels(const float* keyframe, const float* const* frames, const float* proj,
+                                           const float* depths, const float* pixel_depths, void* out_cv, void* out_sfcv,
+                                           void* out_sfcv_nhwc, int nhwc_dtype, int B, int F, int D, int H, int W,
+                                           float alpha, const float* chan_w, int matching, int centered, int out_dtype,
+                                           int channels, void* stream) {
+    return cost_volume_typed("mr_cost_volume_fwd_channels", keyframe, frames, proj, depths, pixel_depths, out_cv, out_sfcv,
+                             out_sfcv_nhwc, nhwc_dtype, B, F, D, H, W, alpha, chan_w, matching, centered, out_dtype, channels,
+                             stream);
 }

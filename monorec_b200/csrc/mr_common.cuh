@@ -12,12 +12,12 @@ void count_launch(int n = 1);
 
 // cost_volume.cu: launches the fused kernel for batch elements [b_begin, b_begin + b_count) of a B-element problem;
 // depths is the plane table [D], or with per_pixel_depths != 0 one depth per plane and pixel [B,D,H,W]; out_cv / out_sfcv
-// are fp32 (out_dtype MR_DT_F32) or IEEE half (MR_DT_F16)
+// are fp32 (out_dtype MR_DT_F32) or IEEE half (MR_DT_F16); keyframe and frames have `channels` (3 or 1) planes
 int launch_cost_volume(const float* keyframe, const float* const* frames, const float* proj, const float* depths,
                        void* out_cv, void* out_sfcv, int B, int F, int D, int H, int W, float alpha,
                        const float* chan_w, int b_begin, int b_count, int gather_only, cudaStream_t stream,
                        void* sf_nhwc = nullptr, int sf_nhwc_dtype = 0, int per_pixel_depths = 0,
-                       int matching = MR_CV_SSIM, int centered = 1, int out_dtype = MR_DT_F32);
+                       int matching = MR_CV_SSIM, int centered = 1, int out_dtype = MR_DT_F32, int channels = 3);
 
 inline int check_cuda(cudaError_t e, const char* what) {
     if (e == cudaSuccess) return MR_OK;

@@ -168,19 +168,20 @@ class MultiDeviceEvaluater(_Lanes):
     Lane r runs `shard_sequences(lengths, frame_count, dilation, seq_batch, r, len(devices), eval_batch=batch_size,
     keys=keys)` on devices[r]: a `MonoRecSequence(first_frame=, key_end=, keys=)` per slice, with `graphed` CUDA-graph
     replay (each lane captures its own graph), under a `SequenceEvaluater(group=LANE, shard=)`.  `metrics`, `batch_size`,
-    `roi`, `max_distance` and `median_scaling` are the evaluater's; `stereo` / `mvobj_masks` the sequences'.
+    `roi`, `max_distance` and `median_scaling` are the evaluater's; `stereo` / `mvobj_masks` / `use_color` the sequences'.
 
     `push(sequence, frame, image, pose, intrinsics, target, mvobj_mask=None, stereo=None)` in `order`, then `flush()`.
     `log()` brings every lane's closed evaluater-batch rows to devices[0], sorts them by global batch index and runs the
     one-process fold (`evaluation.fold_rows`, as the `torchrun` path): `Evaluater.eval`'s dict, equal to one process's."""
 
     def __init__(self, model, devices, lengths, metrics, batch_size, frame_count=2, dilation=1, seq_batch=8, keys=None,
-                 roi=None, max_distance=None, median_scaling=False, graphed=True, stereo=False, mvobj_masks=False):
+                 roi=None, max_distance=None, median_scaling=False, graphed=True, stereo=False, mvobj_masks=False,
+                 use_color=True):
         plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), eval_batch=batch_size, keys=keys)
         super().__init__(plan, devices)
         self._models = _replicas(model, self.devices)
         self._seq_kw = dict(frame_count=frame_count, dilation=dilation, batch_size=seq_batch, graphed=graphed,
-                            stereo=stereo, mvobj_masks=mvobj_masks)
+                            stereo=stereo, mvobj_masks=mvobj_masks, use_color=use_color)
         self.evaluaters = [SequenceEvaluater(None, metrics, batch_size, roi=roi, max_distance=max_distance,
                                              median_scaling=median_scaling, group=LANE, shard=sl) if sl else None
                            for sl in plan.slices]
@@ -210,8 +211,8 @@ class MultiDevicePointCloud(_Lanes):
     entry of `devices`.
 
     Lane r runs `shard_sequences(..., r, len(devices), buffer_length=buffer_length, keys=keys)` on devices[r]: per slice a
-    `MonoRecSequence` and a `SequencePointCloud(emit=slice.emit)` into the lane's own `PLYSaver(height, width, min_d,
-    max_d, roi=roi, dropout=dropout)`.
+    `MonoRecSequence` (with `stereo`, `mvobj_masks`, `use_color`) and a `SequencePointCloud(emit=slice.emit)` into the
+    lane's own `PLYSaver(height, width, min_d, max_d, roi=roi, dropout=dropout)`.
 
     `push(sequence, frame, image, pose, intrinsics, rand=None, stereo=None, mvobj_mask=None)` in `order`, then `flush()`;
     `rand` are the frame's dropout numbers, keyed by sequence index as in `SequencePointCloud`.  `vertices` (on
@@ -219,12 +220,12 @@ class MultiDevicePointCloud(_Lanes):
 
     def __init__(self, model, devices, lengths, height, width, frame_count=2, dilation=1, seq_batch=8, keys=None,
                  buffer_length=5, min_hits=1, mask_fill=32, min_d=3, max_d=400, roi=None, dropout=0, graphed=True,
-                 stereo=False, mvobj_masks=False):
+                 stereo=False, mvobj_masks=False, use_color=True):
         plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), buffer_length=buffer_length, keys=keys)
         super().__init__(plan, devices)
         self._models = _replicas(model, self.devices)
         self._seq_kw = dict(frame_count=frame_count, dilation=dilation, batch_size=seq_batch, graphed=graphed,
-                            stereo=stereo, mvobj_masks=mvobj_masks)
+                            stereo=stereo, mvobj_masks=mvobj_masks, use_color=use_color)
         self._pc_kw = dict(buffer_length=buffer_length, min_hits=min_hits, mask_fill=mask_fill)
         self.savers = [PLYSaver(height, width, min_d=min_d, max_d=max_d, roi=roi, dropout=dropout)
                        for _ in self.devices]

@@ -546,7 +546,7 @@ class DepthModule(_PackedSource, nn.Module):
         if self.training:
             raise NotImplementedError("monorec_b200.DepthModule: inference only")
         out_range = tuple(self.out_range if out_range is None else out_range)
-        keyframe = data_dict["keyframe"]
+        keyframe = data_dict.get("_keyframe_rgb", data_dict["keyframe"])   # see rgb_keyframe
         cv = data_dict["cost_volume"]
         feats_nchw = data_dict["image_features"]
         cv_mask = data_dict.get("_cv_mask_for_depth")
@@ -598,6 +598,19 @@ class DepthModule(_PackedSource, nn.Module):
     def predict_depth(self, x, scale):
         """API parity with the reference (:554-557); x is NHWC inside this implementation."""
         return self._head(x, self._packs(self._build)["heads"][scale], tuple(self.out_range))
+
+
+def rgb_keyframe(data_dict):
+    """The keyframe as three channels: data_dict["keyframe"] itself, or for a grayscale keyframe [B,1,H,W] its replica
+    [B,3,H,W], made at the first call and kept in the dict as `_keyframe_rgb` for the later ones (the trunk and the
+    DepthModule read it; MonoRecModel's heads stage drops it)."""
+    key = data_dict["keyframe"]
+    if key.shape[1] != 1:
+        return key
+    rgb = data_dict.get("_keyframe_rgb")
+    if rgb is None:
+        rgb = data_dict["_keyframe_rgb"] = key.expand(-1, 3, -1, -1).contiguous()
+    return rgb
 
 
 class MonoRecModel(nn.Module):
@@ -701,6 +714,11 @@ class MonoRecModel(nn.Module):
                                                   strict=False)
 
     def forward(self, data_dict):
+        """The reference's forward on its data dict.  The images may also be grayscale, [B,1,H,W] (a loader's
+        use_color=False, TUM Mono-VO): they mean the three-channel images whose three planes equal them, and every output is
+        that of those replicas bit for bit.  The cost volume reads the one-channel frames; the trunk and the DepthModule read
+        one three-channel copy of the keyframe, made once here."""
+        rgb_keyframe(data_dict)
         data_dict = self._stage_cost_volume(data_dict)
         data_dict = self._stage_trunk(data_dict)
         return self._stage_heads(data_dict)
@@ -740,7 +758,7 @@ class MonoRecModel(nn.Module):
 
     def _stage_trunk(self, data_dict):
         """Stage B: `image_features`, the ResNet-18 trunk's levels of the key frame."""
-        keyframe = data_dict["keyframe"]
+        keyframe = rgb_keyframe(data_dict)
         with torch.no_grad():
             # torchvision trunk on cuDNN, fed channels-last; TF32 is allowed there unless the engine runs its fp32 parity mode
             image = (keyframe + .5).contiguous(memory_format=torch.channels_last)
@@ -773,6 +791,7 @@ class MonoRecModel(nn.Module):
                 # cost_volume * (1 - cv_mask) (:713): the product is fused into the depth module's layout change and
                 # the masked volume is also materialised for callers that read data_dict["cost_volume"]
                 data_dict["_cv_mask_for_depth"] = data_dict["cv_mask"]
+                rgb_keyframe(data_dict)     # (the DepthModule reads the three-channel copy of a grayscale keyframe)
                 # (1-p)*lo + p*hi (:717-718) in the heads' epilogue; a standalone DepthModule call returns the raw |tanh| heads
                 data_dict = self.depth_module(data_dict, out_range=(lo, hi - lo))
                 del data_dict["_cv_mask_for_depth"]
@@ -786,6 +805,7 @@ class MonoRecModel(nn.Module):
         data_dict.pop("_cv_range", None)
         data_dict.pop("_sfcv_nhwc", None)
         data_dict.pop("_sfcv_nhwc_filled", None)
+        data_dict.pop("_keyframe_rgb", None)
         return data_dict
 
 

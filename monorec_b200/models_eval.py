@@ -18,6 +18,7 @@ import numpy as np
 import torch
 
 from .evaluation import SequenceEvaluater
+from .model import rgb_keyframe
 from .sequence import MonoRecSequence
 
 __all__ = ["MultiModelEvaluater", "cost_volume_key", "same_trunk", "share_groups"]
@@ -69,6 +70,8 @@ class _SharedForward:
         self.models, self.cv_groups, self.trunk_groups = models, cv_groups, trunk_groups
 
     def __call__(self, batch):
+        batch = dict(batch)
+        rgb_keyframe(batch)                   # a grayscale keyframe's three-channel copy: one for every stage and model
         cv, feats = {}, {}
         for g in self.cv_groups:
             d = self.models[g[0]]._stage_cost_volume(dict(batch))
@@ -109,9 +112,9 @@ class MultiModelEvaluater:
     """`Evaluater.eval` of every model of `models` (MonoRecModels in eval mode on one device) over one frame stream.
 
     `metrics`, `batch_size`, `roi`, `max_distance`, `median_scaling` are SequenceEvaluater's (the same for every model, as
-    in evaluate.py); `frame_count`, `dilation`, `seq_batch` (the key frames per forward), `keys`, `stereo`, `mvobj_masks`
-    and `device` build the MonoRecSequence the models run over.  A `use_stereo` model needs `stereo=True`, a
-    `pretrain_mode == 3` model `mvobj_masks=True`; the stereo frames and masks are copied to the device once, and only if
+    in evaluate.py); `frame_count`, `dilation`, `seq_batch` (the key frames per forward), `keys`, `stereo`, `mvobj_masks`,
+    `device` and `use_color` (False: grayscale [1,H,W] frames) build the MonoRecSequence the models run over.  A
+    `use_stereo` model needs `stereo=True`, a `pretrain_mode == 3` model `mvobj_masks=True`; the stereo frames and masks are copied to the device once, and only if
     a model (or an `*_onlydynamic` metric, for the masks) reads them.
 
     `push(image, pose, intrinsics, target, mvobj_mask=None, stereo=None)`, `skip()` and `flush()` are SequenceEvaluater's
@@ -129,7 +132,7 @@ class MultiModelEvaluater:
     """
 
     def __init__(self, models, metrics, batch_size, roi=None, max_distance=None, median_scaling=False, frame_count=2,
-                 dilation=1, seq_batch=8, keys=None, stereo=False, mvobj_masks=False, device=None):
+                 dilation=1, seq_batch=8, keys=None, stereo=False, mvobj_masks=False, device=None, use_color=True):
         self.models = list(models)
         if not self.models:
             raise ValueError("MultiModelEvaluater: models is empty")
@@ -150,6 +153,7 @@ class MultiModelEvaluater:
         self.cv_groups, self.trunk_groups = share_groups(self.models)
         self._forward = _SharedForward(self.models, self.cv_groups, self.trunk_groups)
         self._seq_args = dict(frame_count=frame_count, dilation=dilation, batch_size=seq_batch, device=self.device,
+                              use_color=use_color,
                               stereo=self.stereo and any(m.use_stereo for m in self.models),
                               mvobj_masks=bool(mvobj_masks) and any(int(m.pretrain_mode) == 3 for m in self.models))
         self.seq = MonoRecSequence(self._forward, keys=keys, **self._seq_args)

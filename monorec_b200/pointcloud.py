@@ -55,7 +55,8 @@ class PLYSaver(torch.nn.Module):
         return self._buf[:n] if n else torch.empty(0, 6)
 
     def add_depthmap(self, depth, image, intrinsics, extrinsics, keep_masks=(), min_hits=1, rand=None):
-        """depth: inverse depth [B,1,H,W] (the reference's argument name); keep_masks: the voting window's masks (optional:
+        """depth: inverse depth [B,1,H,W] (the reference's argument name); image: the key frames [B,3,H,W], or grayscale
+        [B,1,H,W], whose vertices are coloured with the replicated value; keep_masks: the voting window's masks (optional:
         the reference multiplies the depth by the voted mask before calling; passing the masks here fuses that product)."""
         masks = [m.to(torch.float32).contiguous() for m in keep_masks]
         self._add("mr_pointcloud_add", depth, image, intrinsics, extrinsics, rand,
@@ -82,6 +83,8 @@ class PLYSaver(torch.nn.Module):
             raise _lib.MonorecLibraryError("monorec_b200.pointcloud needs CUDA tensors (no CPU fallback)")
         lib = _lib.load()
         dev = depth.device
+        if image.shape[1] == 1:       # grayscale key frames: the colours are the replicated value, as for their RGB replica
+            image = image.expand(-1, 3, -1, -1)
         d, img, K, P = [t.to(torch.float32).contiguous() for t in (depth, image, intrinsics, extrinsics)]
         B, _, H, W = d.shape
         if self.dropout > 0 and rand is None:

@@ -109,6 +109,11 @@ class MonoRecSequence:
     frame.  These are copied for the key frames only, into rings next to the frames', gathered with them into the batch
     (the CUDA graph's static inputs) and returned in each key frame's outputs.
 
+    `use_color=False` (the KITTI loader's name for its grayscale cameras; TUM Mono-VO is grayscale too): `push` takes
+    one-channel images [1,H,W], and stereo images [1,H,W] too, and the frame rings hold one plane.  The model reads them as
+    the three-channel images whose planes equal them (MonoRecModel.forward), so the outputs are those of a colour sequence
+    fed the replicated frames, bit for bit; the key frame's `keyframe` output is the one-channel image.
+
     `model` is a MonoRecModel (or any callable that adds its outputs to the reference's data dict and returns that dict,
     as MonoRecModel.forward does); `device` defaults to the device of its parameters.  A `use_stereo` model without
     `stereo=True`, and `pretrain_mode == 3` without `mvobj_masks=True`, raise NotImplementedError: a plain frame stream
@@ -116,7 +121,7 @@ class MonoRecSequence:
     """
 
     def __init__(self, model, frame_count=2, dilation=1, batch_size=8, graphed=True, device=None, first_frame=0,
-                 key_end=None, keys=None, stereo=False, mvobj_masks=False):
+                 key_end=None, keys=None, stereo=False, mvobj_masks=False, use_color=True):
         if getattr(model, "use_stereo", False) and not stereo:
             raise NotImplementedError("MonoRecSequence: use_stereo needs stereo frames: MonoRecSequence(stereo=True) and "
                                       "push(..., stereo=(image, pose, intrinsics))")
@@ -132,6 +137,8 @@ class MonoRecSequence:
         self.batch_size = int(batch_size)
         self.graphed = bool(graphed)
         self.stereo, self.mvobj_masks = bool(stereo), bool(mvobj_masks)
+        self.use_color = bool(use_color)
+        self.channels = 3 if self.use_color else 1
         self.device = torch.device(device) if device is not None else next(model.parameters()).device
         lo, self._hi = min(0, min(self.offsets)), max(self.offsets)
         self.first_key = -lo               # the sequence's first key frame with all its neighbours in the sequence
@@ -171,8 +178,9 @@ class MonoRecSequence:
         self.n_pushed += 1
 
     def push(self, image, pose, intrinsics, stereo=None, mvobj_mask=None, target=None):
-        if image.dim() != 3 or image.shape[0] != 3 or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
-            raise ValueError(f"MonoRecSequence.push: image [3,H,W], pose [4,4], intrinsics [4,4] expected, got "
+        C = self.channels
+        if image.dim() != 3 or image.shape[0] != C or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
+            raise ValueError(f"MonoRecSequence.push: image [{C},H,W], pose [4,4], intrinsics [4,4] expected, got "
                              f"{tuple(image.shape)}, {tuple(pose.shape)}, {tuple(intrinsics.shape)}")
         if self.key_end is not None and self.n_pushed >= self.key_end + self._hi:
             raise ValueError(f"MonoRecSequence.push: frame {self.n_pushed} is past the last frame the key frames before "
@@ -187,12 +195,12 @@ class MonoRecSequence:
         maps = self._key_inputs(H, W, stereo, mvobj_mask, target)
         if self._rings is None:
             R = self.ring_len
-            self._rings = (torch.empty(R, 3, H, W, device=self.device), torch.empty(R, 4, 4, device=self.device),
+            self._rings = (torch.empty(R, self.channels, H, W, device=self.device), torch.empty(R, 4, 4, device=self.device),
                            torch.empty(R, 4, 4, device=self.device))
             # the key-frame inputs the sequence is built for, and the optional ones this first push gives
             shapes = {}
             if self.stereo:
-                shapes.update(stereoframe=(3, H, W), stereoframe_pose=(4, 4), stereoframe_intrinsics=(4, 4))
+                shapes.update(stereoframe=(self.channels, H, W), stereoframe_pose=(4, 4), stereoframe_intrinsics=(4, 4))
             if self.mvobj_masks or "mvobj_mask" in maps:
                 shapes["mvobj_mask"] = (1, H, W)
             if "target" in maps:
@@ -228,8 +236,9 @@ class MonoRecSequence:
         maps = {}
         if self.stereo and stereo is not None:
             image, pose, intrinsics = stereo
-            if tuple(image.shape) != (3, H, W) or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
-                raise ValueError(f"MonoRecSequence.push: stereo image [3,{H},{W}], pose [4,4], intrinsics [4,4] expected, "
+            C = self.channels
+            if tuple(image.shape) != (C, H, W) or tuple(pose.shape) != (4, 4) or tuple(intrinsics.shape) != (4, 4):
+                raise ValueError(f"MonoRecSequence.push: stereo image [{C},{H},{W}], pose [4,4], intrinsics [4,4] expected, "
                                  f"got {tuple(image.shape)}, {tuple(pose.shape)}, {tuple(intrinsics.shape)}")
             maps.update(stereoframe=image, stereoframe_pose=pose, stereoframe_intrinsics=intrinsics)
         for key, t in (("mvobj_mask", mvobj_mask), ("target", target)):

@@ -8,10 +8,11 @@ call site of march_unit<MODE> or pixel_phase<T> when the inlining chains of its 
 line.  For each march mode it prints the largest such loop, the row loop (three row steps per body), and for the
 per-pixel phase its loops; counts are per row step for the march and per loop iteration otherwise.
 
-The kernel is instantiated as cost_volume_kernel<PIX, ERR, CENTER, OUT>: depth source (plane table / per-pixel cv_depths),
-error mode (1 SSIM, 2 SSIM + L1, 3 box L1: MR_CV_*), centred or uncentred fused volume, and the volumes' storage type (float
-or __half).  The twelve fp32 instantiations come first (the two default ones, SSIM centred, plane depths then per-pixel
-depths, lead), the twelve half ones after them in the same order.  A source from before the volume type was a template
+The kernel is instantiated as cost_volume_kernel<PIX, ERR, CENTER, OUT, NC>: depth source (plane table / per-pixel
+cv_depths), error mode (1 SSIM, 2 SSIM + L1, 3 box L1: MR_CV_*), centred or uncentred fused volume, the volumes' storage
+type (float or __half) and the frames' channel count (3, or 1 for grayscale frames).  The twelve fp32 three-channel
+instantiations come first (the two default ones, SSIM centred, plane depths then per-pixel depths, lead), the twelve half
+ones after them in the same order, then the same twenty-four with one channel.  A source from before the volume type was a template
 parameter is reported under the fp32 titles; one from before the error mode was has only cost_volume_kernel<PIX>, reported
 under the first two titles.
 """
@@ -56,21 +57,24 @@ def disassemble(src):
 
 ERR_NAMES = {1: "SSIM", 2: "SSIM + L1", 3: "box L1"}
 OUT_TYPES = (("f", "float", "fp32"), ("6__half", "__half", "half"))
-# (label, mangled template arguments of cost_volume_kernel<PIX, ERR, CENTER, OUT>, those of a source from before the volume
-# type was a template parameter (fp32 only), those of a source with only <PIX>)
+# (label, mangled template arguments of cost_volume_kernel<PIX, ERR, CENTER, OUT, NC>, then those of older sources: without
+# the channel count (three channels), without the volume type (fp32 only), with only <PIX>)
 INSTANTIATIONS = [
-    (f"{'per-pixel' if pix else 'plane'} depths, {ERR_NAMES[err]}, {'centred' if ctr else 'uncentred'}, {oname} volumes "
-     f"(cost_volume_kernel<{'true' if pix else 'false'}, {err}, {'true' if ctr else 'false'}, {otype}>)",
-     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}E{omangled}EE",
-     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}EE" if omangled == "f" else None,
-     f"cost_volume_kernelILb{pix}EE" if err == 1 and ctr and omangled == "f" else None)
+    (f"{'per-pixel' if pix else 'plane'} depths, {ERR_NAMES[err]}, {'centred' if ctr else 'uncentred'}, {oname} volumes, "
+     f"{nc} channel{'s' if nc > 1 else ''} "
+     f"(cost_volume_kernel<{'true' if pix else 'false'}, {err}, {'true' if ctr else 'false'}, {otype}, {nc}>)",
+     f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}E{omangled}Li{nc}EEE",
+     [f for f in (f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}E{omangled}EE" if nc == 3 else None,
+                  f"cost_volume_kernelILb{pix}ELi{err}ELb{ctr}EE" if nc == 3 and omangled == "f" else None,
+                  f"cost_volume_kernelILb{pix}EE" if nc == 3 and err == 1 and ctr and omangled == "f" else None) if f])
+    for nc in (3, 1)
     for omangled, otype, oname in OUT_TYPES
     for err, ctr, pix in [(1, 1, 0), (1, 1, 1)] + [(e, c, p) for e in (1, 2, 3) for c in (1, 0) for p in (0, 1)
                                                     if (e, c) != (1, 1)]
 ]
 
 
-def kernel_instructions(dis, name="cost_volume_kernelILb0ELi1ELb1EfEE"):
+def kernel_instructions(dis, name="cost_volume_kernelILb0ELi1ELb1EfLi3EEE"):
     """[(addr, opcode, text, source lines of the inlining chain)] and {label: addr} of the kernel whose .text section
     name contains `name` (default: the plane instantiation)."""
     ins, labels, cur, inside, pending = [], {}, [], False, []
@@ -108,12 +112,11 @@ def main():
         if m and "__device__" not in l and "void" not in l:
             sites[f"{m.group(1)}<{m.group(2)}>"] = i
     dis = disassemble(src)
-    for k, (title, name, old3, old) in enumerate(INSTANTIATIONS):
+    for k, (title, name, older) in enumerate(INSTANTIATIONS):
         if name not in dis:
-            if old3 is not None and old3 in dis:     # (a source from before the volume type became a template parameter)
-                name = old3
-            elif old is not None and old in dis:     # (a source from before the error mode became a template parameter)
-                name = old
+            found = [o for o in older if o in dis]   # (a source from before a template parameter was added)
+            if found:
+                name = found[0]
             elif k == 0 and "cost_volume_kernelILb" not in dis:   # (from before the depth source became one)
                 report(src, "cost_volume_kernel", *kernel_instructions(dis, "cost_volume_kernel"), sites)
                 continue
