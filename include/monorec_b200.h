@@ -337,7 +337,9 @@ int mr_mask_volume(const void* volume, const float* mask, void* out, int dtype, 
  *   mvobj_mask       [B,1,H,W] or NULL: with it, pixels whose mask is <= 0.5 are excluded (the *_onlydynamic variants)
  *   roi              host int[4] {r0, r1, c0, c1} (python slice semantics) or NULL; max_distance <= 0: no clamp
  *   pred_all_valid   0: pixels with result == 0 are excluded (the *_onlyvalid variants)
- *   out_metrics      device float[G][7]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel; no host synchronisation
+ *   out_metrics      device float[G][7]: a1, a2, a3, rmse, rmse_log, abs_rel, sq_rel; no host synchronisation.  A NaN in
+ *                    result or target at a pixel that is not excluded gives the reference's NaN in rmse, rmse_log, abs_rel
+ *                    and sq_rel of its row (a miss in a1-a3); NaN at excluded pixels does not show
  *   workspace        device buffer of mr_sparse_metrics_workspace(B) bytes, 8-byte aligned
  * mr_images_u8_to_f32: uint8 HWC images [B,Hs,Ws,3] -> float CHW [B,3,H,W] = u / 255 - 0.5 of the crop starting at
  * (crop_top, crop_left) (data_loader/kitti_odometry_dataset.py:121-132 without the PIL resize). */
@@ -387,8 +389,9 @@ int mr_eval_accumulate(const float* values, int G, int M, const int* group_sizes
  *   inv_depth [B,1,H,W] (data_dict["result"]); keyframe [B,3,H,W]; K, pose [B,4,4];
  *   keep_masks: host array of n_masks device pointers [B,1,H,W] (the window's keep masks) -- a pixel survives iff more than
  *     n_masks - min_hits of them are 1 (create_pointcloud.py:93-95); n_masks = 0: no vote;
- *   min_d / max_d: distance range; roi: host int[4] {r0, r1, c0, c1} or NULL; dropout_rand: [B,1,H,W] uniform numbers (a
- *     vertex is kept iff rand > dropout; torch.rand_like in the reference) or NULL;
+ *   min_d / max_d: distance range; roi: host int[4] {r0, r1, c0, c1} with python slice semantics (negative bounds count
+ *     from the end, bounds past the edge are clipped, an empty region adds no vertex) or NULL; dropout_rand: [B,1,H,W]
+ *     uniform numbers (a vertex is kept iff rand > dropout; torch.rand_like in the reference) or NULL;
  *   vertices: device float [capacity][6]; n_before: vertices already stored, or any negative value to take the position
  *     from *n_after as the previous call on the stream left it (the running count stays on the device: the caller needs
  *     no read-back per call, only a capacity that bounds the count); n_after: DEVICE long long, the new count, or minus the

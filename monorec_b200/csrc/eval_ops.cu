@@ -17,6 +17,13 @@ namespace {
 
 constexpr int kSums = 8;   // per image: valid count, a1, a2, a3 hits, sum se, sum sle, sum abs_rel, sum sq_rel
 
+// torch's clamp_min (and relu) keep a NaN (fmaxf would drop it)
+__device__ __forceinline__ float clamp_min_nan(float x, float lo) { return isnan(x) ? x : fmaxf(x, lo); }
+// torch.max(a, b) of two tensors propagates a NaN of either side
+__device__ __forceinline__ float max_nan(float a, float b) { return (isnan(a) || isnan(b)) ? __int_as_float(0x7fc00000) : fmaxf(a, b); }
+// torch's relu as it treats the zeros: NaN and -0.0 pass through (1 / -0.0 is -inf in the reference, a hit in a1-a3)
+__device__ __forceinline__ float relu_torch(float x) { return x < 0.f ? 0.f : x; }
+
 struct MetricArgs {
     const float* pred;     // [B,1,H,W] predicted inverse depth (data_dict["result"])
     const float* gt;       // [B,1,H,W] sparse ground-truth inverse depth (0 = no measurement)
@@ -44,11 +51,13 @@ __global__ void sparse_metric_sums_kernel(const MetricArgs a) {
         if (!a.pred_all_valid) masked = masked || (p == 0.f);
         if (a.mvobj != nullptr) masked = masked || !(__ldg(a.mvobj + o) > 0.5f);
         if (masked) continue;
-        // get_positive_depth, get_absolute_depth (utils/util.py:46-65): relu, clamp_min(1 / max_distance), 1 / x
-        p = fmaxf(p, 0.f); g = fmaxf(g, 0.f);
-        if (a.inv_max > 0.f) { p = fmaxf(p, a.inv_max); g = fmaxf(g, a.inv_max); }
+        // get_positive_depth, get_absolute_depth (utils/util.py:46-65): relu, clamp_min(1 / max_distance), 1 / x.  A NaN
+        // prediction or target at an unmasked pixel stays NaN, as in the reference: rmse, rmse_log, abs_rel and sq_rel of its
+        // rows are NaN (and the evaluater drops the batch), a1-a3 count it as a miss
+        p = relu_torch(p); g = relu_torch(g);
+        if (a.inv_max > 0.f) { p = clamp_min_nan(p, a.inv_max); g = clamp_min_nan(g, a.inv_max); }
         const float dp = __fdiv_rn(1.0f, p), dg = __fdiv_rn(1.0f, g);
-        const float th = fmaxf(__fdiv_rn(dg, dp), __fdiv_rn(dp, dg));
+        const float th = max_nan(__fdiv_rn(dg, dp), __fdiv_rn(dp, dg));
         const float diff = dp - dg, ld = logf(dp) - logf(dg);
         acc[0] += 1.f;
         acc[1] += (th < 1.25f) ? 1.f : 0.f;
@@ -107,11 +116,6 @@ __global__ void sparse_metric_finalize_kernel(const double* sums, int B, int gro
 // ---- dense metrics (model/metric_functions/sparse_metrics.py:6-78, dense_metrics.py, completeness_metrics.py) -------------
 constexpr int kDenseSums = 13;  // per image: a1, a2, a3 hits, sum se, sle, abs_rel, sq_rel, E, E^2 (sc_inv), |p - g| (l1_inv),
                                 // and over the whole image: result != 0, result != 0 where target == 0, target == 0
-
-// torch's relu / clamp_min keep a NaN (fmaxf would drop it)
-__device__ __forceinline__ float clamp_min_nan(float x, float lo) { return isnan(x) ? x : fmaxf(x, lo); }
-// torch.max(a, b) of two tensors propagates a NaN of either side
-__device__ __forceinline__ float max_nan(float a, float b) { return (isnan(a) || isnan(b)) ? __int_as_float(0x7fc00000) : fmaxf(a, b); }
 
 struct DenseArgs {
     const float* pred;     // [B,1,H,W] data_dict["result"]
@@ -351,14 +355,6 @@ __global__ void images_u8_to_f32_kernel(const unsigned char* src, float* dst, in
     for (int ch = 0; ch < 3; ++ch) d[(size_t)ch * H * W] = __fsub_rn(__fdiv_rn((float)s[ch], 255.0f), 0.5f);
 }
 
-// python slicing semantics of preprocess_roi (utils/util.py:36-43): [r0:r1, c0:c1], clipped; roi == nullptr: the whole image
-void clip_roi(const int* roi, int H, int W, int& r0, int& r1, int& c0, int& c1) {
-    r0 = 0; r1 = H; c0 = 0; c1 = W;
-    if (roi == nullptr) return;
-    auto clip = [](int v, int n) { if (v < 0) v += n; return v < 0 ? 0 : (v > n ? n : v); };
-    r0 = clip(roi[0], H); r1 = clip(roi[1], H); c0 = clip(roi[2], W); c1 = clip(roi[3], W);
-}
-
 // blocks per image of a grid-stride pass over n pixels: ~8 pixels per thread, at most one block per SM and image
 int blocks_per_image(int n, int threads, int* blocks) {
     int dev = 0, sms = 0;
@@ -392,7 +388,7 @@ extern "C" int mr_dense_metrics(const float* result, const float* target, int B,
     MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "mr_dense_metrics: workspace must be 8-byte aligned");
     DenseArgs a{};
     a.pred = result; a.gt = target; a.B = B; a.H = H; a.W = W;
-    clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
+    mr::clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
     MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "mr_dense_metrics: empty region of interest (roi)");
     a.min_inv = min_inv_depth;
     a.sums = static_cast<double*>(workspace);
@@ -460,7 +456,7 @@ extern "C" int mr_sparse_metrics(const float* result, const float* target, const
     MR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 7) == 0, "mr_sparse_metrics: workspace must be 8-byte aligned");
     MetricArgs a{};
     a.pred = result; a.gt = target; a.mvobj = mvobj_mask; a.B = B; a.H = H; a.W = W;
-    clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
+    mr::clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);
     MR_REQUIRE(a.r1 > a.r0 && a.c1 > a.c0, "mr_sparse_metrics: empty region of interest");
     a.inv_max = max_distance > 0.f ? 1.0f / max_distance : 0.f;
     a.pred_all_valid = pred_all_valid;

@@ -19,6 +19,16 @@ int launch_cost_volume(const float* keyframe, const float* const* frames, const 
                        void* sf_nhwc = nullptr, int sf_nhwc_dtype = 0, int per_pixel_depths = 0,
                        int matching = MR_CV_SSIM, int centered = 1, int out_dtype = MR_DT_F32, int channels = 3);
 
+// python slicing semantics of a roi {r0, r1, c0, c1} = [r0:r1, c0:c1] (preprocess_roi, utils/util.py:36-43, and the masking
+// of PLYSaver.add_depthmap, utils/ply_utils.py:39-43): a negative bound counts from the end, a bound past the edge is clipped;
+// the region may come out empty (r1 <= r0 or c1 <= c0).  roi == nullptr: the whole image
+inline void clip_roi(const int* roi, int H, int W, int& r0, int& r1, int& c0, int& c1) {
+    r0 = 0; r1 = H; c0 = 0; c1 = W;
+    if (roi == nullptr) return;
+    auto clip = [](int v, int n) { if (v < 0) v += n; return v < 0 ? 0 : (v > n ? n : v); };
+    r0 = clip(roi[0], H); r1 = clip(roi[1], H); c0 = clip(roi[2], W); c1 = clip(roi[3], W);
+}
+
 inline int check_cuda(cudaError_t e, const char* what) {
     if (e == cudaSuccess) return MR_OK;
     set_error("%s: %s", what, cudaGetErrorString(e));

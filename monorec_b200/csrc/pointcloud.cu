@@ -73,7 +73,7 @@ struct PcArgs {
     int min_hits;
     const float* rnd;         // [B,1,H,W] uniform numbers for the dropout, or nullptr
     float dropout, min_d, max_d;
-    int B, H, W, r0, r1, c0, c1, use_roi;
+    int B, H, W, r0, r1, c0, c1;      // region of interest [r0, r1) x [c0, c1), clipped (the whole image without a roi)
     int* counts;              // [B * blocks_per_image] kept vertices per block, then exclusive offsets (in place)
     float* out;               // [capacity][6]
     long long capacity;
@@ -90,11 +90,9 @@ __device__ __forceinline__ bool keep_vertex(const PcArgs<Vote>& a, int b, int i,
         inv *= (s > (float)(a.vote.n_masks - a.min_hits)) ? 1.f : 0.f;
     }
     depth = __fdiv_rn(1.0f, inv);                           // ply_utils.py:36 (1 / 0 = inf fails the range test below)
+    const int y = i / a.W, x = i - y * a.W;
     bool ok = (a.min_d <= depth) && (depth <= a.max_d);     // :38
-    if (a.use_roi) {                                        // :39-43
-        const int y = i / a.W, x = i - y * a.W;
-        ok = ok && y >= a.r0 && y < a.r1 && x >= a.c0 && x < a.c1;
-    }
+    ok = ok && y >= a.r0 && y < a.r1 && x >= a.c0 && x < a.c1;   // :39-43
     if (a.rnd != nullptr && a.dropout > 0.f) ok = ok && (__ldg(a.rnd + o) > a.dropout);   // :44-45
     return ok;
 }
@@ -225,8 +223,7 @@ int add_vertices(PcArgs<Vote>& a, const float* inv_depth, const float* keyframe,
     a.min_hits = min_hits;
     a.rnd = dropout_rand; a.dropout = dropout; a.min_d = min_d; a.max_d = max_d;
     a.B = B; a.H = H; a.W = W;
-    a.use_roi = roi != nullptr;
-    if (roi) { a.r0 = roi[0]; a.r1 = roi[1]; a.c0 = roi[2]; a.c1 = roi[3]; }
+    mr::clip_roi(roi, H, W, a.r0, a.r1, a.c0, a.c1);       // python slices, as PLYSaver masks; an empty roi keeps nothing
     a.base = static_cast<long long*>(workspace);
     a.counts = reinterpret_cast<int*>(a.base + 1);
     a.out = vertices; a.capacity = capacity; a.total = n_after;

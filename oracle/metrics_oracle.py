@@ -23,7 +23,8 @@ def sparse_metrics(pred, gt, mvobj_mask=None, roi=None, max_distance=None, pred_
         mask |= pred == 0
     if mvobj_mask is not None:                                     # sparse_metrics.py:86 `mask |= ~(mvobj_mask > .5)`
         mask |= ~(np.asarray(mvobj_mask, np.float32) > 0.5)
-    p, g = np.maximum(pred, 0), np.maximum(gt, 0)                  # :59-65
+    # :59-65, torch's relu: NaN and -0.0 pass through (np.maximum(-0.0, 0) would give +0.0, whose inverse is +inf, not -inf)
+    p, g = np.where(pred < 0, np.float32(0), pred), np.where(gt < 0, np.float32(0), gt)
     if max_distance is not None:                                   # :46-56
         p = np.maximum(p, np.float32(1.0 / max_distance))
         g = np.maximum(g, np.float32(1.0 / max_distance))
