@@ -436,6 +436,26 @@ int mr_reprojection_loss_bwd(const float* keyframe, const float* const* frames, 
                              const float* grad_errors, const int* winner, int B, int F, int H, int W,
                              float* out_grad_inv_depth, void* stream);
 
+/* ---- photometric residual image -------------------------------------------------------------------------------------------
+ * Replaces ResidualImageModule.forward (reference: model/layers.py:161-217; the ResidualImage wrapper, :147-158, is the module
+ * with inv_depth_max = 0, inv_depth_min = 1): out[b,0,v,u] = min over the F frames of mean_c SSIM(warped - 0.5, keyframe + 0.5)
+ * (3x3 box, reflection padding, not comp mode: layers.py:91-139), +inf for a frame whose sample is masked (some channel of
+ * grid_sample(frame + 1) is exactly 0), and 0 where every frame is masked.
+ *   keyframe, frames[f]  [B,C,H,W]; C = 1 reads one-channel images as the three-channel images whose planes equal them (the
+ *                        result is that of the replicated images bit for bit)
+ *   proj                 [B,F,12] rows of mr_projection_tables (depths = NULL) for the F frames of this call
+ *   inv_depth            [B,1,H,W] predicted_inverse_depths[0] = p
+ *   inv_depth_range      device float[2] = {inv_depth_max, inv_depth_min}, or NULL for {0, 1}: the back-projection divides by
+ *                        (1 - p) inv_depth_max + p inv_depth_min, rounded op by op as the reference's torch expression (:172)
+ *   out                  [B,1,H,W]
+ * Non-finite and non-positive inverse depths follow the reference's arithmetic: a point behind a source camera is sampled at
+ * its mirrored projection; a position that is not finite gives a NaN sample, which is not masked, and NaN propagates through
+ * the SSIM windows and the minimum over the frames.  Constraints: 1 <= F <= MR_MAX_FRAMES, C in {1, 3}, 2 <= H, W <= 16384,
+ * 1 <= B <= 65535, every pointer non-null (but inv_depth_range) and 4-byte aligned.  All arguments are checked before the first
+ * CUDA call; one launch, no host synchronisation. */
+int mr_residual_image(const float* keyframe, const float* const* frames, const float* proj, const float* inv_depth,
+                      const float* inv_depth_range, int B, int F, int C, int H, int W, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,4 +12,7 @@ def __getattr__(name):
     if name in ("MonoRecModel", "CostVolumeModule", "MaskModule", "DepthModule", "ResnetEncoder"):
         from . import model as _m
         return getattr(_m, name)
+    if name in ("ResidualImage", "ResidualImageModule"):
+        from . import layers as _l
+        return getattr(_l, name)
     raise AttributeError(name)

@@ -86,6 +86,8 @@ SIGNATURES = {
                                          c_void_p, c_void_p, c_void_p]),
     "mr_reprojection_loss_bwd": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
                                          c_int, c_void_p, c_void_p]),
+    "mr_residual_image": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                  c_void_p, c_void_p]),
 }
 
 

@@ -18,6 +18,7 @@ calls the implementation directly, with no dispatcher in front of its ~150 launc
 - `sparse_metrics`, `dense_metrics`, `median_scaling`: the evaluation passes.
 - `reprojection_loss_fwd` (projection tables + forward pass) and `reprojection_loss_bwd`, joined by
   `torch.library.register_autograd`, so that a compiled loss backpropagates to `depth_prediction`.
+- `residual_image`: projection tables + the residual-image kernel (`layers.ResidualImage`, `ResidualImageModule`).
 
 The Mask, Depth and trunk ops compute from the weights they are given: the module's parameters (and the trunk's BatchNorm
 buffers) are tensor inputs, next to the module's configuration.  The implementation binds them into a module of that
@@ -39,6 +40,7 @@ from torch import Tensor
 
 from . import conv as C
 from . import cost_volume as CV
+from . import layers as LY
 from . import losses as L
 from . import metrics as MT
 
@@ -244,7 +246,18 @@ def _loss_backward(ctx, grad_errors, _grad_winner, _grad_proj):
 torch.library.register_autograd("monorec_b200::reprojection_loss_fwd", _loss_backward, setup_context=_loss_setup_context)
 
 
+# ---- residual image ------------------------------------------------------------------------------------------------
+residual_image = torch.library.custom_op("monorec_b200::residual_image", LY.residual_image_impl, mutates_args=(),
+                                         device_types="cuda")
+
+
+@residual_image.register_fake
+def _(keyframe, frames, keyframe_pose, keyframe_intrinsics, poses, intrinsics, inv_depth, inv_depth_range):
+    B, _, H, W = keyframe.shape
+    return keyframe.new_empty(B, 1, H, W, dtype=torch.float32)
+
+
 OPS = {"cost_volume": cost_volume, "resnet_trunk": resnet_trunk, "mask_module": mask_module,
        "depth_module": depth_module, "mask_volume": mask_volume, "sparse_metrics": sparse_metrics,
        "dense_metrics": dense_metrics, "median_scaling": median_scaling, "reprojection_loss_fwd": reprojection_loss_fwd,
-       "reprojection_loss_bwd": reprojection_loss_bwd}
+       "reprojection_loss_bwd": reprojection_loss_bwd, "residual_image": residual_image}

@@ -11,6 +11,7 @@ right camera's frame (`return_stereo`) and a moving-object mask (`return_mvobj_m
 sequence takes those as `keys=`, `stereo=True` and `mvobj_masks=True`.
 """
 import bisect
+import functools
 import sys
 
 import torch
@@ -114,6 +115,12 @@ class MonoRecSequence:
     the three-channel images whose planes equal them (MonoRecModel.forward), so the outputs are those of a colour sequence
     fed the replicated frames, bit for bit; the key frame's `keyframe` output is the one-channel image.
 
+    `residual_image=True`: each key frame's outputs also hold `residual_image` [1,1,H,W], the reference's photometric
+    residual image (layers.ResidualImage) of its `result`, an inverse depth, against the frames and poses its cost volume
+    used (the mono frames, then the stereo frame of a `use_stereo` model).  It is computed in the same forward, inside the
+    graph replay when `graphed`, with no host synchronisation; the other outputs are those of residual_image=False bit for
+    bit.
+
     `model` is a MonoRecModel (or any callable that adds its outputs to the reference's data dict and returns that dict,
     as MonoRecModel.forward does); `device` defaults to the device of its parameters.  A `use_stereo` model without
     `stereo=True`, and `pretrain_mode == 3` without `mvobj_masks=True`, raise NotImplementedError: a plain frame stream
@@ -121,13 +128,16 @@ class MonoRecSequence:
     """
 
     def __init__(self, model, frame_count=2, dilation=1, batch_size=8, graphed=True, device=None, first_frame=0,
-                 key_end=None, keys=None, stereo=False, mvobj_masks=False, use_color=True):
+                 key_end=None, keys=None, stereo=False, mvobj_masks=False, use_color=True, residual_image=False):
         if getattr(model, "use_stereo", False) and not stereo:
             raise NotImplementedError("MonoRecSequence: use_stereo needs stereo frames: MonoRecSequence(stereo=True) and "
                                       "push(..., stereo=(image, pose, intrinsics))")
         if int(getattr(model, "pretrain_mode", 0)) == 3 and not mvobj_masks:
             raise NotImplementedError("MonoRecSequence: pretrain_mode 3 needs moving-object masks: "
                                       "MonoRecSequence(mvobj_masks=True) and push(..., mvobj_mask=...)")
+        if residual_image and int(getattr(model, "pretrain_mode", 0)) == 2:
+            raise NotImplementedError("MonoRecSequence: residual_image needs an inverse depth as `result`; pretrain_mode 2 "
+                                      "returns the mask there")
         if batch_size < 1:
             raise ValueError(f"batch_size ({batch_size}) must be >= 1")
         if first_frame < 0:
@@ -138,6 +148,11 @@ class MonoRecSequence:
         self.graphed = bool(graphed)
         self.stereo, self.mvobj_masks = bool(stereo), bool(mvobj_masks)
         self.use_color = bool(use_color)
+        self.residual_image = bool(residual_image)
+        # what a batch runs: the model, or the model and the residual image of its result.  A function of the model only,
+        # not a method of the sequence: the CUDA graph keeps it, and a sequence -> graph -> sequence cycle would leave a
+        # dropped sequence's graph to the cyclic collector, which may then destroy it during another graph's capture
+        self._forward = functools.partial(_with_residual_image, model) if self.residual_image else model
         self.channels = 3 if self.use_color else 1
         self.device = torch.device(device) if device is not None else next(model.parameters()).device
         lo, self._hi = min(0, min(self.offsets)), max(self.offsets)
@@ -288,9 +303,9 @@ class MonoRecSequence:
         # a pinned copy does not synchronise; the host allocator keeps the block until the copy is done
         idx = idx.pin_memory().to(self.device, non_blocking=True) if self.device.type == "cuda" else idx
         if not graphed:
-            out = self.model(self._assemble(idx))
+            out = self._forward(self._assemble(idx))
         elif self._graph is None:
-            self._graph = GraphedMonoRec(self.model, self._assemble(idx))
+            self._graph = GraphedMonoRec(self._forward, self._assemble(idx))
             out = self._graph.replay()
         else:
             self._assemble(idx, out=self._graph.static_in)
@@ -301,8 +316,21 @@ class MonoRecSequence:
             self._free.append(self._slot.pop(f)[0])
         return [(i, _row(out, j)) for j, i in enumerate(index)]
 
+
+def _with_residual_image(model, data):
+    """`model` on one batch dict, and the residual image (layers.ResidualImage) of its `result` against the frames its
+    cost volume used, as `residual_image`."""
+    from .layers import residual_image
+    from .losses import _collect
+    out = model(data)
+    frames, poses, intrinsics = _collect(out, getattr(model, "use_mono", True), getattr(model, "use_stereo", False))
+    out["residual_image"] = residual_image(out["keyframe"], out["keyframe_pose"], out["keyframe_intrinsics"], out["result"],
+                                           frames, poses, intrinsics)
+    return out
+
+
 _ROW_KEYS = ("result", "cv_mask", "cost_volume", "keyframe", "keyframe_pose", "keyframe_intrinsics", "stereoframe",
-             "stereoframe_pose", "stereoframe_intrinsics", "mvobj_mask", "target")
+             "stereoframe_pose", "stereoframe_intrinsics", "mvobj_mask", "target", "residual_image")
 
 
 def _row(out, j):
