@@ -160,19 +160,10 @@ class SequenceEvaluater:
         return emitted
 
     def _check_slice(self, seq):
-        if seq is None or self._slices is None:
-            return
-        if self._slice >= len(self._slices):
-            raise ValueError(f"SequenceEvaluater: a sequence after the shard's {len(self._slices)} slices")
-        emit = self._slices[self._slice].emit
-        if seq.key_begin > emit[0] or (seq.key_end is not None and seq.key_end < emit[1]):
-            raise ValueError(f"SequenceEvaluater: the sequence runs key frames {seq.key_begin} ... {seq.key_end}, which "
-                             f"do not cover the shard's key frames {emit[0]} ... {emit[1] - 1}")
+        check_slice(self._slices, self._slice, seq)
 
     def _consume(self, emitted):
-        if self._slices is not None:
-            e0, e1 = self._slices[self._slice].emit if self._slice < len(self._slices) else (0, 0)
-            emitted = [(i, o) for i, o in emitted if e0 <= i < e1]
+        emitted = emitted_in_slice(self._slices, self._slice, emitted)
         if not emitted:
             return
         # the key frames' results and the targets (and masks) the sequence gathered into their batch
@@ -261,6 +252,28 @@ class SequenceEvaluater:
 
 LANE = "lane"
 """SequenceEvaluater(group=LANE, shard=...): a lane of lanes.MultiDeviceEvaluater, whose rows its driver folds."""
+
+
+def check_slice(slices, k, seq):
+    """Refuses `seq` as the sequence of slice k of a shard (`slices`; None: no shard) unless it runs every key frame the
+    slice emits."""
+    if seq is None or slices is None:
+        return
+    if k >= len(slices):
+        raise ValueError(f"SequenceEvaluater: a sequence after the shard's {len(slices)} slices")
+    emit = slices[k].emit
+    if seq.key_begin > emit[0] or (seq.key_end is not None and seq.key_end < emit[1]):
+        raise ValueError(f"SequenceEvaluater: the sequence runs key frames {seq.key_begin} ... {seq.key_end}, which "
+                         f"do not cover the shard's key frames {emit[0]} ... {emit[1] - 1}")
+
+
+def emitted_in_slice(slices, k, emitted):
+    """The key frames of `emitted` (a sequence's (index, outputs) list) that slice k of a shard evaluates: all of them
+    without a shard (`slices` None), none after the shard's last slice."""
+    if slices is None:
+        return emitted
+    e0, e1 = slices[k].emit if k < len(slices) else (0, 0)
+    return [(i, o) for i, o in emitted if e0 <= i < e1]
 
 
 def sort_rows(rows):

@@ -10,7 +10,8 @@ lane's device busy.  Devices may repeat (`devices=[0, 0, 0]`: three lanes taking
 needed (sequence, frame) across lanes.  `MultiDeviceEvaluater` and `MultiDevicePointCloud` run the unchanged
 `SequenceEvaluater` / `SequencePointCloud` on each lane and merge the results: the same row sort and fold as the
 `torchrun` path, and the vertices in lane order, which is key-frame order.  Both give the one-process log and PLY bit for
-bit (the two alignment rules of `shard_sequences`).
+bit (the two alignment rules of `shard_sequences`).  `MultiDeviceModelsEvaluater` runs evaluate.py's list of models the
+same way, with a `MultiModelEvaluater` on each lane.
 
     runner = MultiDeviceEvaluater(model, [0, 1, 2, 3], lengths, metrics, batch_size=2, ...)
     for s, n in runner.order:              # the (sequence, frame) to read next
@@ -26,6 +27,7 @@ import torch
 
 from .dist import shard_sequences
 from .evaluation import LANE, SequenceEvaluater, fold_rows, log_dict
+from .models_eval import MultiModelEvaluater, results_list, share_groups
 from .pointcloud import PLYSaver, SequencePointCloud, write_ply
 from .sequence import MonoRecSequence, needs_frame, neighbour_offsets
 
@@ -204,6 +206,74 @@ class MultiDeviceEvaluater(_Lanes):
         with self._context(0):
             rows = torch.cat([ev.tagged_rows(dev) for ev in lanes])
             return log_dict(fold_rows(rows, m), m)
+
+
+class MultiDeviceModelsEvaluater(_Lanes):
+    """evaluate.py's list of models over the concatenated sequences of `lengths` frames, split over one lane per entry of
+    `devices`: `MultiDeviceEvaluater` with `models` (MonoRecModels in eval mode on one device) in place of `model`.
+
+    Lane r runs the slices of MultiDeviceEvaluater's lane r with a `MultiModelEvaluater(group=LANE, shard=)` on devices[r],
+    over replicas of every model on that device, so each lane reads and copies every frame it needs once and shares the
+    cost-volume and trunk stages as one device does.  The sharing (`cv_groups`, `trunk_groups`) is decided once, on
+    `models`; every lane runs with it, and each device's replicas are checked to give the same groups.  Every lane holds
+    every model and one captured graph of their shared forward.
+
+    `order`, `push(sequence, frame, image, pose, intrinsics, target, mvobj_mask=None, stereo=None)` and `flush()` are
+    MultiDeviceEvaluater's (each lane skips the frames of its slices that it does not need).  `logs()`: one log per model, in list order, each the one-process log bit for bit (every
+    lane's rows of that model folded on devices[0]); `results(dataset_dict)`: evaluate.py's results.json list."""
+
+    def __init__(self, models, devices, lengths, metrics, batch_size, frame_count=2, dilation=1, seq_batch=8, keys=None,
+                 roi=None, max_distance=None, median_scaling=False, graphed=True, stereo=False, mvobj_masks=False,
+                 use_color=True):
+        self.models = list(models)
+        if not self.models:
+            raise ValueError("MultiDeviceModelsEvaluater: models is empty")
+        home = next(self.models[0].parameters()).device
+        for m in self.models:
+            if next(m.parameters()).device != home:
+                raise ValueError(f"MultiDeviceModelsEvaluater: a model is on {next(m.parameters()).device}, not {home}")
+        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), eval_batch=batch_size, keys=keys)
+        super().__init__(plan, devices)
+        self.cv_groups, self.trunk_groups = share_groups(self.models)
+        replicas = [_replicas(m, self.devices) for m in self.models]
+        self._models = {}
+        for d in replicas[0]:
+            self._models[d] = [rep[d] for rep in replicas]
+            groups = share_groups(self._models[d])
+            if groups != (self.cv_groups, self.trunk_groups):
+                raise RuntimeError(f"MultiDeviceModelsEvaluater: the replicas on {d} share stages as {groups}, the models "
+                                   f"as {(self.cv_groups, self.trunk_groups)}")
+        kw = dict(roi=roi, max_distance=max_distance, median_scaling=median_scaling, frame_count=frame_count,
+                  dilation=dilation, seq_batch=seq_batch, stereo=stereo, mvobj_masks=mvobj_masks, use_color=use_color,
+                  graphed=graphed, group=LANE, groups=(self.cv_groups, self.trunk_groups))
+        self.evaluaters = [MultiModelEvaluater(self._models[d], metrics, batch_size, device=d, shard=sl, **kw) if sl
+                           else None for d, sl in zip(self.devices, plan.slices)]
+        self.names = next(ev for ev in self.evaluaters if ev is not None).names
+
+    def _open(self, r, sl):
+        ev = self.evaluaters[r]
+        ev.next_sequence(None if self.plan.keys is None else self.plan.keys[sl.sequence], first_frame=sl.frames[0],
+                         key_end=sl.run[1])
+        return ev
+
+    def _close(self, r):
+        self.evaluaters[r].flush()
+
+    def logs(self):
+        """The one-process log of every model, in list order (one device-to-host read each; call after `flush`)."""
+        dev = self.devices[0]
+        lanes = [ev for ev in self.evaluaters if ev is not None]
+        m = len(self.names)
+        out = []
+        with self._context(0):
+            for k in range(len(self.models)):
+                rows = torch.cat([ev.evaluaters[k].tagged_rows(dev) for ev in lanes])
+                out.append(log_dict(fold_rows(rows, m), m))
+        return out
+
+    def results(self, dataset_dict):
+        """evaluate.py's results.json list: per model {"model", "dataset", "result"}, as MultiModelEvaluater.results."""
+        return results_list(self.models, self.names, self.logs(), dataset_dict)
 
 
 class MultiDevicePointCloud(_Lanes):

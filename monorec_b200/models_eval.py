@@ -17,7 +17,7 @@ import pathlib
 import numpy as np
 import torch
 
-from .evaluation import SequenceEvaluater
+from .evaluation import LANE, SequenceEvaluater, check_slice, emitted_in_slice, fold_rows, log_dict
 from .model import rgb_keyframe
 from .sequence import MonoRecSequence
 
@@ -120,22 +120,35 @@ class MultiModelEvaluater:
     `push(image, pose, intrinsics, target, mvobj_mask=None, stereo=None)`, `skip()` and `flush()` are SequenceEvaluater's
     and return what the sequence emits: per key frame (index, outputs), where `outputs["models"][m]` holds model m's
     `result`, `cv_mask`, `cost_volume`, `predicted_inverse_depths` and `outputs` the key frame's `target` (and
-    `mvobj_mask`).  `next_sequence(keys=None)` runs the rest of the current sequence and continues on a new one with the
-    same settings and key-frame list `keys`; the totals and open evaluater batches carry over.  Once the sequence has
-    captured its graph (its first full batch), `push` and `flush` never synchronise with the host.
+    `mvobj_mask`).  `next_sequence(keys=None, first_frame=0, key_end=None)` runs the rest of the current sequence and
+    continues on a new one with the same settings and key-frame list `keys`; the totals and open evaluater batches carry
+    over.  Once the sequence has captured its graph (its first full batch), `push` and `flush` never synchronise with the
+    host.
 
     The sharing is decided once, here (`share_groups`; `cv_groups` / `trunk_groups` hold it), and like GraphedMonoRec a
     sequence's captured graph keeps running on the weights it was captured with.  Build a new evaluater after changing a
-    model's weights or options.
+    model's weights or options.  `groups` gives that sharing instead, decided on models equal to these (the lanes of
+    lanes.MultiDeviceModelsEvaluater, which checks it).  `graphed=False` runs the sequences without CUDA-graph replay.
 
     `logs()`: one log per model, in list order.  `results(dataset_dict)`: evaluate.py's results.json list.
+
+    One slice of a split run (one rank under `torchrun`, or one lane): `group` and `shard` as on SequenceEvaluater, a
+    process group (or evaluation.LANE) and this rank's slices, `dist.shard_sequences(..., eval_batch=batch_size)`.  The
+    evaluater then opens no sequence itself: `next_sequence(keys, first_frame=slice.frames[0], key_end=slice.run[1])`
+    starts each slice in turn (and refuses a sequence that does not run the slice's key frames), the slice's frames
+    slice.frames[0] ... slice.frames[1] - 1 are pushed (or skipped), and only the key frames of the slice's `emit` range
+    are evaluated.  `logs()` is then a collective: every rank calls it and gets every model's log of the whole run, the
+    one-process logs bit for bit.  A lane's logs are folded by its driver.
     """
 
     def __init__(self, models, metrics, batch_size, roi=None, max_distance=None, median_scaling=False, frame_count=2,
-                 dilation=1, seq_batch=8, keys=None, stereo=False, mvobj_masks=False, device=None, use_color=True):
+                 dilation=1, seq_batch=8, keys=None, stereo=False, mvobj_masks=False, device=None, use_color=True,
+                 graphed=True, group=None, shard=None, groups=None):
         self.models = list(models)
         if not self.models:
             raise ValueError("MultiModelEvaluater: models is empty")
+        if shard is not None and keys is not None:
+            raise ValueError("MultiModelEvaluater: with a shard, each slice's key list goes to next_sequence(keys, ...)")
         self.device = torch.device(device) if device is not None else next(self.models[0].parameters()).device
         for m in self.models:
             if next(m.parameters()).device != self.device:
@@ -147,18 +160,21 @@ class MultiModelEvaluater:
                 raise NotImplementedError("MultiModelEvaluater: a pretrain_mode 3 model needs mvobj_masks=True and "
                                           "push(..., mvobj_mask=...)")
         self.evaluaters = [SequenceEvaluater(None, metrics, batch_size, roi=roi, max_distance=max_distance,
-                                             median_scaling=median_scaling) for _ in self.models]
+                                             median_scaling=median_scaling, group=group, shard=shard) for _ in self.models]
         self.names = self.evaluaters[0].names
         self.stereo = bool(stereo)
-        self.cv_groups, self.trunk_groups = share_groups(self.models)
+        self.group, self._slices, self._slice = group, None if shard is None else list(shard), 0
+        self.cv_groups, self.trunk_groups = share_groups(self.models) if groups is None else groups
         self._forward = _SharedForward(self.models, self.cv_groups, self.trunk_groups)
         self._seq_args = dict(frame_count=frame_count, dilation=dilation, batch_size=seq_batch, device=self.device,
-                              use_color=use_color,
+                              use_color=use_color, graphed=graphed,
                               stereo=self.stereo and any(m.use_stereo for m in self.models),
                               mvobj_masks=bool(mvobj_masks) and any(int(m.pretrain_mode) == 3 for m in self.models))
-        self.seq = MonoRecSequence(self._forward, keys=keys, **self._seq_args)
+        self.seq = None if shard is not None else MonoRecSequence(self._forward, keys=keys, **self._seq_args)
 
     def push(self, image, pose, intrinsics, target, mvobj_mask=None, stereo=None):
+        if self.seq is None:
+            raise ValueError("MultiModelEvaluater.push: no sequence open (with a shard, next_sequence starts each slice)")
         ev = self.evaluaters[0]
         ev._check_frame(image, target, mvobj_mask)
         if stereo is not None and not self.stereo:
@@ -174,20 +190,28 @@ class MultiModelEvaluater:
         self.seq.skip()
 
     def flush(self):
-        emitted = self.seq.flush()
+        emitted = self.seq.flush() if self.seq is not None else []
         self._consume(emitted)
         for ev in self.evaluaters:
             ev.flush()
         return emitted
 
-    def next_sequence(self, keys=None):
-        emitted = self.seq.flush()
+    def next_sequence(self, keys=None, first_frame=0, key_end=None):
+        """Runs the key frames the current sequence still holds, then continues on a new one with key-frame list `keys`,
+        starting at frame `first_frame` and running the key frames before `key_end` (MonoRecSequence's; the defaults run
+        the whole sequence).  Returns what the current sequence's flush returns."""
+        emitted = self.seq.flush() if self.seq is not None else []
         self._consume(emitted)
+        if self._slices is not None and self.seq is not None:
+            self._slice += 1
         self.seq = None                   # (the old graph's memory is released before the new sequence captures one)
-        self.seq = MonoRecSequence(self._forward, keys=keys, **self._seq_args)
+        seq = MonoRecSequence(self._forward, keys=keys, first_frame=first_frame, key_end=key_end, **self._seq_args)
+        check_slice(self._slices, self._slice, seq)
+        self.seq = seq
         return emitted
 
     def _consume(self, emitted):
+        emitted = emitted_in_slice(self._slices, self._slice, emitted)
         if not emitted:
             return
         # cut into evaluater batches as SequenceEvaluater._consume does, once per model, on the shared targets (and masks)
@@ -197,15 +221,27 @@ class MultiModelEvaluater:
             ev.add(torch.cat([o["models"][m]["result"] for _, o in emitted]), target, mask)
 
     def logs(self):
-        """Evaluater.eval's dict of every model, in list order (one device-to-host read each)."""
-        return [ev.log() for ev in self.evaluaters]
+        """Evaluater.eval's dict of every model, in list order (one device-to-host read each).  With a process group, a
+        collective that gathers every rank's rows (SequenceEvaluater.log)."""
+        if self.group is None or self.group is LANE:
+            return [ev.log() for ev in self.evaluaters]
+        from .dist import all_gather_rows
+        m = len(self.names)
+        return [log_dict(fold_rows(all_gather_rows(ev.tagged_rows(self.device), self.group), m), m)
+                for ev in self.evaluaters]
 
     def results(self, dataset_dict):
         """evaluate.py's results.json list: per model {"model": its public attributes, "dataset": those of
-        `dataset_dict` (the dataset's `__dict__`), "result": its log with `metrics_info`, the metric names}."""
-        dataset = public_dict(dataset_dict)
-        out = []
-        for model, log in zip(self.models, self.logs()):
-            log["metrics_info"] = list(self.names)
-            out.append({"model": public_dict(model), "dataset": dict(dataset), "result": log})
-        return out
+        `dataset_dict` (the dataset's `__dict__`), "result": its log with `metrics_info`, the metric names}.  With a process
+        group, a collective as `logs()` is."""
+        return results_list(self.models, self.names, self.logs(), dataset_dict)
+
+
+def results_list(models, names, logs, dataset_dict):
+    """evaluate.py's results.json list of `models` with their `logs` over the metrics `names`."""
+    dataset = public_dict(dataset_dict)
+    out = []
+    for model, log in zip(models, logs):
+        log["metrics_info"] = list(names)
+        out.append({"model": public_dict(model), "dataset": dict(dataset), "result": log})
+    return out
