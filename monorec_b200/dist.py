@@ -31,7 +31,7 @@ class SequenceSlice(NamedTuple):
 
 
 def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eval_batch=None, buffer_length=None,
-                    keys=None):
+                    keys=None, layout=None):
     """The slices of sequences of `lengths` frames that `rank` of `world` runs, in sequence order (sequences it does not
     touch are left out; a rank may get none).  Exactly one of:
 
@@ -52,19 +52,32 @@ def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eva
     the list, or keys=None, for every key frame with its neighbours).  Everything above is then counted in listed key
     frames: positions, evaluater batches, model batches and the vote windows' neighbours.  `run` and `emit` stay sequence
     indices ([first, last + 1) of the listed key frames in them), and `frames` spans the run's neighbours; a rank passes the
-    frames in it that no listed key frame needs with MonoRecSequence.skip."""
+    frames in it that no listed key frame needs with MonoRecSequence.skip.
+
+    `layout`: one sequence.FrameLayout per sequence (MonoRecSequence's `layout`), in place of frame_count, dilation and
+    `keys`.  Its key frames are counted as a `keys` list is, and `frames` spans the run's frames at the layout's offsets."""
     if (eval_batch is None) == (buffer_length is None):
         raise ValueError("shard_sequences: give exactly one of eval_batch and buffer_length")
     if batch_size < 1 or world < 1 or not 0 <= rank < world:
         raise ValueError(f"shard_sequences: batch_size ({batch_size}) >= 1 and 0 <= rank ({rank}) < world ({world}) needed")
     from .sequence import check_keys, neighbour_offsets
-    offs = neighbour_offsets(frame_count, dilation)
-    lo, hi = min(0, min(offs)), max(offs)
+    if keys is not None and layout is not None:
+        raise ValueError("shard_sequences: give keys or layout, not both (a layout holds its key frames)")
     if keys is not None and len(keys) != len(lengths):
         raise ValueError(f"shard_sequences: {len(keys)} key lists for {len(lengths)} sequences")
-    # the key frames of each sequence: the listed ones, or -lo .. n - hi - 1
-    K = [range(-lo, int(n) - hi) if keys is None or keys[s] is None else check_keys(keys[s], offs, n)
-         for s, n in enumerate(lengths)]
+    if layout is None:
+        offs = neighbour_offsets(frame_count, dilation)
+        lo, hi = min(0, min(offs)), max(offs)
+        spread = [(lo, hi)] * len(lengths)
+        # the key frames of each sequence: the listed ones, or -lo .. n - hi - 1
+        K = [range(-lo, int(n) - hi) if keys is None or keys[s] is None else check_keys(keys[s], offs, n)
+             for s, n in enumerate(lengths)]
+    else:
+        if len(layout) != len(lengths):
+            raise ValueError(f"shard_sequences: {len(layout)} layouts for {len(lengths)} sequences")
+        # the frames key frame i uses are i + lo ... i + hi, its own included
+        spread = [(min(0, min(lay.offsets)), max(0, max(lay.offsets))) for lay in layout]
+        K = [check_keys(lay.keys, lay.offsets, n) for lay, n in zip(layout, lengths)]
     n_keys = [len(k) for k in K]
     if eval_batch is not None:
         if eval_batch < 1:
@@ -89,6 +102,7 @@ def shard_sequences(lengths, frame_count, dilation, batch_size, rank, world, eva
             r0 = (a - before) // batch_size * batch_size
             r1 = min(k, -(-(b + after) // batch_size) * batch_size)
             key = K[s]
+            lo, hi = spread[s]
             out.append(SequenceSlice(s, (key[r0] + lo, key[r1 - 1] + hi + 1), (key[r0], key[r1 - 1] + 1),
                                      (key[a], key[b - 1] + 1), offset + a - p0))
         offset += p1 - p0

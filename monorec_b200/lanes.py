@@ -40,22 +40,29 @@ class LanePlan:
     push order: the frames of each slice that `MonoRecSequence.needs` accepts (the others are passed with `skip`).
     `order`: every (sequence, frame) some lane needs, once.  Lanes take turns, each reading up to `batch_size` frames it
     needs that no lane has read yet, so every lane gets about one model batch per turn; a frame a later lane has already
-    read (a boundary frame two lanes run) is held until this lane reaches it."""
+    read (a boundary frame two lanes run) is held until this lane reaches it.
 
-    def __init__(self, lengths, frame_count, dilation, batch_size, lanes, eval_batch=None, buffer_length=None, keys=None):
+    `layout`: one sequence.FrameLayout per sequence, in place of frame_count, dilation and `keys` (shard_sequences')."""
+
+    def __init__(self, lengths, frame_count, dilation, batch_size, lanes, eval_batch=None, buffer_length=None, keys=None,
+                 layout=None):
         if lanes < 1:
             raise ValueError(f"LanePlan: lanes ({lanes}) must be >= 1")
-        self.lanes, self.keys = int(lanes), keys
+        self.lanes, self.keys, self.layout = int(lanes), keys, layout
         self.slices = [shard_sequences(lengths, frame_count, dilation, batch_size, r, lanes, eval_batch=eval_batch,
-                                       buffer_length=buffer_length, keys=keys) for r in range(lanes)]
+                                       buffer_length=buffer_length, keys=keys, layout=layout) for r in range(lanes)]
         offsets = neighbour_offsets(frame_count, dilation)
         self.frames = []
         for sl in self.slices:
             mine = []
             for k, s in enumerate(sl):
-                listed = range(*s.run) if keys is None or keys[s.sequence] is None else keys[s.sequence]
+                if layout is not None:
+                    listed, offs = layout[s.sequence].keys, layout[s.sequence].offsets
+                else:
+                    listed = range(*s.run) if keys is None or keys[s.sequence] is None else keys[s.sequence]
+                    offs = offsets
                 run = [int(x) for x in listed if s.run[0] <= int(x) < s.run[1]]
-                mine += [(k, s.sequence, n) for n in range(*s.frames) if needs_frame(run, offsets, n)]
+                mine += [(k, s.sequence, n) for n in range(*s.frames) if needs_frame(run, offs, n)]
             self.frames.append(mine)
         self.users = {}                    # (sequence, frame) -> the lanes that need it
         for r, mine in enumerate(self.frames):
@@ -72,6 +79,12 @@ class LanePlan:
                         read.add(f)
                         self.order.append(f)
                         taken += 1
+
+    def sequence_kw(self, sequence):
+        """MonoRecSequence's key-frame argument for sequence `sequence`: its `keys` list or its `layout`."""
+        if self.layout is not None:
+            return dict(layout=self.layout[sequence])
+        return dict(keys=None if self.keys is None else self.keys[sequence])
 
 
 class _Lanes:
@@ -171,6 +184,7 @@ class MultiDeviceEvaluater(_Lanes):
     keys=keys)` on devices[r]: a `MonoRecSequence(first_frame=, key_end=, keys=)` per slice, with `graphed` CUDA-graph
     replay (each lane captures its own graph), under a `SequenceEvaluater(group=LANE, shard=)`.  `metrics`, `batch_size`,
     `roi`, `max_distance` and `median_scaling` are the evaluater's; `stereo` / `mvobj_masks` / `use_color` the sequences'.
+    `layout`: one sequence.FrameLayout per sequence, in place of frame_count, dilation and keys.
 
     `push(sequence, frame, image, pose, intrinsics, target, mvobj_mask=None, stereo=None)` in `order`, then `flush()`.
     `log()` brings every lane's closed evaluater-batch rows to devices[0], sorts them by global batch index and runs the
@@ -178,8 +192,9 @@ class MultiDeviceEvaluater(_Lanes):
 
     def __init__(self, model, devices, lengths, metrics, batch_size, frame_count=2, dilation=1, seq_batch=8, keys=None,
                  roi=None, max_distance=None, median_scaling=False, graphed=True, stereo=False, mvobj_masks=False,
-                 use_color=True):
-        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), eval_batch=batch_size, keys=keys)
+                 use_color=True, layout=None):
+        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), eval_batch=batch_size, keys=keys,
+                        layout=layout)
         super().__init__(plan, devices)
         self._models = _replicas(model, self.devices)
         self._seq_kw = dict(frame_count=frame_count, dilation=dilation, batch_size=seq_batch, graphed=graphed,
@@ -190,9 +205,8 @@ class MultiDeviceEvaluater(_Lanes):
 
     def _open(self, r, sl):
         ev = self.evaluaters[r]
-        keys = None if self.plan.keys is None else self.plan.keys[sl.sequence]
         ev.next_sequence(MonoRecSequence(self._models[self.devices[r]], device=self.devices[r], first_frame=sl.frames[0],
-                                         key_end=sl.run[1], keys=keys, **self._seq_kw))
+                                         key_end=sl.run[1], **self.plan.sequence_kw(sl.sequence), **self._seq_kw))
         return ev
 
     def _close(self, r):
@@ -219,12 +233,12 @@ class MultiDeviceModelsEvaluater(_Lanes):
     every model and one captured graph of their shared forward.
 
     `order`, `push(sequence, frame, image, pose, intrinsics, target, mvobj_mask=None, stereo=None)` and `flush()` are
-    MultiDeviceEvaluater's (each lane skips the frames of its slices that it does not need).  `logs()`: one log per model, in list order, each the one-process log bit for bit (every
+    MultiDeviceEvaluater's (each lane skips the frames of its slices that it does not need), and so is `layout`.  `logs()`: one log per model, in list order, each the one-process log bit for bit (every
     lane's rows of that model folded on devices[0]); `results(dataset_dict)`: evaluate.py's results.json list."""
 
     def __init__(self, models, devices, lengths, metrics, batch_size, frame_count=2, dilation=1, seq_batch=8, keys=None,
                  roi=None, max_distance=None, median_scaling=False, graphed=True, stereo=False, mvobj_masks=False,
-                 use_color=True):
+                 use_color=True, layout=None):
         self.models = list(models)
         if not self.models:
             raise ValueError("MultiDeviceModelsEvaluater: models is empty")
@@ -232,7 +246,8 @@ class MultiDeviceModelsEvaluater(_Lanes):
         for m in self.models:
             if next(m.parameters()).device != home:
                 raise ValueError(f"MultiDeviceModelsEvaluater: a model is on {next(m.parameters()).device}, not {home}")
-        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), eval_batch=batch_size, keys=keys)
+        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), eval_batch=batch_size, keys=keys,
+                        layout=layout)
         super().__init__(plan, devices)
         self.cv_groups, self.trunk_groups = share_groups(self.models)
         replicas = [_replicas(m, self.devices) for m in self.models]
@@ -252,8 +267,7 @@ class MultiDeviceModelsEvaluater(_Lanes):
 
     def _open(self, r, sl):
         ev = self.evaluaters[r]
-        ev.next_sequence(None if self.plan.keys is None else self.plan.keys[sl.sequence], first_frame=sl.frames[0],
-                         key_end=sl.run[1])
+        ev.next_sequence(first_frame=sl.frames[0], key_end=sl.run[1], **self.plan.sequence_kw(sl.sequence))
         return ev
 
     def _close(self, r):
@@ -282,7 +296,8 @@ class MultiDevicePointCloud(_Lanes):
 
     Lane r runs `shard_sequences(..., r, len(devices), buffer_length=buffer_length, keys=keys)` on devices[r]: per slice a
     `MonoRecSequence` (with `stereo`, `mvobj_masks`, `use_color`) and a `SequencePointCloud(emit=slice.emit)` into the
-    lane's own `PLYSaver(height, width, min_d, max_d, roi=roi, dropout=dropout)`.
+    lane's own `PLYSaver(height, width, min_d, max_d, roi=roi, dropout=dropout)`.  `layout`: one sequence.FrameLayout per
+    sequence, in place of frame_count, dilation and keys.
 
     `push(sequence, frame, image, pose, intrinsics, rand=None, stereo=None, mvobj_mask=None)` in `order`, then `flush()`;
     `rand` are the frame's dropout numbers, keyed by sequence index as in `SequencePointCloud`.  `vertices` (on
@@ -290,8 +305,9 @@ class MultiDevicePointCloud(_Lanes):
 
     def __init__(self, model, devices, lengths, height, width, frame_count=2, dilation=1, seq_batch=8, keys=None,
                  buffer_length=5, min_hits=1, mask_fill=32, min_d=3, max_d=400, roi=None, dropout=0, graphed=True,
-                 stereo=False, mvobj_masks=False, use_color=True):
-        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), buffer_length=buffer_length, keys=keys)
+                 stereo=False, mvobj_masks=False, use_color=True, layout=None):
+        plan = LanePlan(lengths, frame_count, dilation, seq_batch, len(devices), buffer_length=buffer_length, keys=keys,
+                        layout=layout)
         super().__init__(plan, devices)
         self._models = _replicas(model, self.devices)
         self._seq_kw = dict(frame_count=frame_count, dilation=dilation, batch_size=seq_batch, graphed=graphed,
@@ -303,9 +319,8 @@ class MultiDevicePointCloud(_Lanes):
     def _open(self, r, sl):
         if self._runner[r] is not None:
             self._runner[r].flush()
-        keys = None if self.plan.keys is None else self.plan.keys[sl.sequence]
         seq = MonoRecSequence(self._models[self.devices[r]], device=self.devices[r], first_frame=sl.frames[0],
-                              key_end=sl.run[1], keys=keys, **self._seq_kw)
+                              key_end=sl.run[1], **self.plan.sequence_kw(sl.sequence), **self._seq_kw)
         return SequencePointCloud(seq, self.savers[r], emit=sl.emit, **self._pc_kw)
 
     def _push(self, r, runner, args, kwargs):

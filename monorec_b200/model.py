@@ -815,12 +815,20 @@ class GraphedMonoRec:
 
     The forward is ~150 small launches; issued from Python it is bound by the host (SURVEY.md §3.5 "hidden syncs" are gone,
     the launch overhead is not).  Capturing once and replaying removes the host from the loop.  Inputs are copied into
-    static buffers, outputs are the static tensors of the captured run (valid until the next call).
+    static buffers, outputs are the static tensors of the captured run (valid until the next call).  A tensor that appears
+    several times in `example` (a key frame that is also one of its own source frames) gets one static buffer, so the
+    captured forward reads it through the same pointers as an eager one.
     """
 
     def __init__(self, model, example, warmup=2):
         self.model = model
-        self.static_in = {k: ([t.clone() for t in v] if isinstance(v, (list, tuple)) else v.clone())
+        buffers = {}
+
+        def static(t):
+            if id(t) not in buffers:
+                buffers[id(t)] = t.clone()
+            return buffers[id(t)]
+        self.static_in = {k: ([static(t) for t in v] if isinstance(v, (list, tuple)) else static(v))
                           for k, v in example.items() if torch.is_tensor(v) or isinstance(v, (list, tuple))}
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())

@@ -125,6 +125,10 @@ class MultiModelEvaluater:
     over.  Once the sequence has captured its graph (its first full batch), `push` and `flush` never synchronise with the
     host.
 
+    `layout` (a sequence.FrameLayout: `kitti_layout` with `offset_d` / `max_length`, `tum_mono_vo_layout`,
+    `robotcar_layout`) replaces frame_count, dilation and keys, for the first sequence; `next_sequence(layout=...)` gives
+    the next one's.
+
     The sharing is decided once, here (`share_groups`; `cv_groups` / `trunk_groups` hold it), and like GraphedMonoRec a
     sequence's captured graph keeps running on the weights it was captured with.  Build a new evaluater after changing a
     model's weights or options.  `groups` gives that sharing instead, decided on models equal to these (the lanes of
@@ -143,12 +147,13 @@ class MultiModelEvaluater:
 
     def __init__(self, models, metrics, batch_size, roi=None, max_distance=None, median_scaling=False, frame_count=2,
                  dilation=1, seq_batch=8, keys=None, stereo=False, mvobj_masks=False, device=None, use_color=True,
-                 graphed=True, group=None, shard=None, groups=None):
+                 graphed=True, group=None, shard=None, groups=None, layout=None):
         self.models = list(models)
         if not self.models:
             raise ValueError("MultiModelEvaluater: models is empty")
-        if shard is not None and keys is not None:
-            raise ValueError("MultiModelEvaluater: with a shard, each slice's key list goes to next_sequence(keys, ...)")
+        if shard is not None and (keys is not None or layout is not None):
+            raise ValueError("MultiModelEvaluater: with a shard, each slice's key list or layout goes to "
+                             "next_sequence(keys, ...) / next_sequence(layout=...)")
         self.device = torch.device(device) if device is not None else next(self.models[0].parameters()).device
         for m in self.models:
             if next(m.parameters()).device != self.device:
@@ -170,7 +175,8 @@ class MultiModelEvaluater:
                               use_color=use_color, graphed=graphed,
                               stereo=self.stereo and any(m.use_stereo for m in self.models),
                               mvobj_masks=bool(mvobj_masks) and any(int(m.pretrain_mode) == 3 for m in self.models))
-        self.seq = None if shard is not None else MonoRecSequence(self._forward, keys=keys, **self._seq_args)
+        self.seq = None if shard is not None else MonoRecSequence(self._forward, keys=keys, layout=layout,
+                                                                  **self._seq_args)
 
     def push(self, image, pose, intrinsics, target, mvobj_mask=None, stereo=None):
         if self.seq is None:
@@ -196,16 +202,17 @@ class MultiModelEvaluater:
             ev.flush()
         return emitted
 
-    def next_sequence(self, keys=None, first_frame=0, key_end=None):
-        """Runs the key frames the current sequence still holds, then continues on a new one with key-frame list `keys`,
-        starting at frame `first_frame` and running the key frames before `key_end` (MonoRecSequence's; the defaults run
-        the whole sequence).  Returns what the current sequence's flush returns."""
+    def next_sequence(self, keys=None, first_frame=0, key_end=None, layout=None):
+        """Runs the key frames the current sequence still holds, then continues on a new one with key-frame list `keys`
+        (or frame layout `layout`), starting at frame `first_frame` and running the key frames before `key_end`
+        (MonoRecSequence's; the defaults run the whole sequence).  Returns what the current sequence's flush returns."""
         emitted = self.seq.flush() if self.seq is not None else []
         self._consume(emitted)
         if self._slices is not None and self.seq is not None:
             self._slice += 1
         self.seq = None                   # (the old graph's memory is released before the new sequence captures one)
-        seq = MonoRecSequence(self._forward, keys=keys, first_frame=first_frame, key_end=key_end, **self._seq_args)
+        seq = MonoRecSequence(self._forward, keys=keys, first_frame=first_frame, key_end=key_end, layout=layout,
+                              **self._seq_args)
         check_slice(self._slices, self._slice, seq)
         self.seq = seq
         return emitted

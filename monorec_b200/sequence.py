@@ -9,10 +9,15 @@ one at a time instead: each is copied to the device once, into a ring of frames,
 The reference's KITTI loader can also select the key frames (`use_index_mask`; `loader_keys` restates its list), add the
 right camera's frame (`return_stereo`) and a moving-object mask (`return_mvobj_mask`) to every key frame's dict; the
 sequence takes those as `keys=`, `stereo=True` and `mvobj_masks=True`.
+
+The reference's other frame streams pick their key and source frames differently: KITTI with `offset_d` or `max_length`,
+TUM Mono-VO and Oxford RobotCar.  A `FrameLayout` (`kitti_layout`, `tum_mono_vo_layout`, `robotcar_layout`) holds one
+sequence's source-frame offsets in the loader's list order and its key frames; the sequence takes it as `layout=`.
 """
 import bisect
 import functools
 import sys
+from typing import NamedTuple, Tuple
 
 import torch
 
@@ -46,11 +51,106 @@ def loader_keys(length, frame_count=2, dilation=1, lidar_depth=False, annotated_
     return list(keys)
 
 
+class FrameLayout(NamedTuple):
+    """One sequence's frame layout: which frames a key frame's dict holds, and which key frames the loader serves.
+
+    `offsets`: the sequence offsets of the source frames from the key frame, in the order of the dict's `frames` / `poses`
+    / `intrinsics` lists (the fused cost volume sums over the frames in that order).  They may include 0 (the key frame is
+    one of its own source frames) and need not be symmetric.  `keys`: the key frames' sequence indices, increasing."""
+    offsets: Tuple[int, ...]
+    keys: Tuple[int, ...]
+
+
+def _inside(keys, offsets, length, drop, loader):
+    """The key frames whose source frames all lie in the sequence [0, length).  A key frame with a source frame outside
+    raises ValueError, unless `drop`: the reference loader would read a frame before 0 at a negative index, which Python
+    wraps to the end of the sequence, and a frame past the end raises IndexError there."""
+    lo, hi = min(offsets), max(offsets)
+    out = []
+    for k in keys:
+        if k + lo >= 0 and k + hi < length:
+            out.append(k)
+        elif not drop:
+            if k + lo < 0:
+                raise ValueError(f"{loader}: key frame {k} needs frame {k + lo}, before the sequence; the reference loader's "
+                                 f"negative index wraps to frame {k + lo + length}.  drop_outside=True leaves such key "
+                                 "frames out")
+            raise ValueError(f"{loader}: key frame {k} needs frame {k + hi}, past the sequence of {length} frames (the "
+                             "reference loader raises IndexError).  drop_outside=True leaves such key frames out")
+    return out
+
+
+def kitti_layout(length, frame_count=2, dilation=1, offset_d=0, max_length=None, lidar_depth=False, annotated_lidar=True,
+                 index_masks=None, drop_outside=False):
+    """The KITTI loader's layout of one sequence of `length` frames.
+
+    The key frames are `loader_keys(length, frame_count, dilation, lidar_depth, annotated_lidar, index_masks)`, cut to the
+    first `max_length` (kitti_odometry_dataset.py:78-79, after the index masks).  The source frames are at k + i + offset_d
+    for i in neighbour_offsets(frame_count, dilation) (:253-258): `offset_d` shifts the sources, not the key range, so a
+    negative one puts the key frame among its own sources (offset_d=-1, frame_count=2: k-2 and k) and makes the stream
+    causal.  The key frames whose sources fall outside the sequence (a negative `offset_d` on the first key frames, a
+    positive one on the last) raise ValueError unless `drop_outside` (see `_inside`).  The defaults give
+    neighbour_offsets(frame_count, dilation) and loader_keys(length, frame_count, dilation)."""
+    offsets = [i + int(offset_d) for i in neighbour_offsets(frame_count, dilation)]
+    keys = loader_keys(length, frame_count, dilation, lidar_depth, annotated_lidar, index_masks)
+    if max_length is not None:
+        if max_length < 0:
+            raise ValueError(f"max_length ({max_length}) must be None or >= 0")
+        keys = keys[:int(max_length)]
+    return FrameLayout(tuple(offsets), tuple(_inside(keys, offsets, int(length), drop_outside, "kitti_layout")))
+
+
+def tum_mono_vo_layout(length, frame_count=2, dilation=1, max_length=None, keyframe_indices=None):
+    """The TUM Mono-VO loader's layout of one sequence of `length` frames (the rows of its result.txt).
+
+    With offset = (frame_count // 2) * dilation, the source frames are at k - offset + i for i in range(0, (frame_count + 1)
+    * dilation, dilation) except i == offset, in that order (tum_mono_vo_dataset.py:115-139).  The key frames are offset
+    ... offset + min(length - frame_count * dilation, max_length) - 1 (:64-72); with `keyframe_indices` (the loader's
+    `only_keyframes`), those of the given sequence indices that pass the loader's border rule, k >= offset and
+    k < length - (frame_count // 2 + 1) * dilation (:164-174), and `max_length` does not apply, as in the loader.
+
+    `keyframe_indices` are the sequence indices of the frames with a depth map; the loader maps each
+    images_depth/NNNNN_d.exr to the first result.txt row whose image is not before NNNNN (data loading, the caller's)."""
+    if frame_count < 1 or dilation < 1:
+        raise ValueError(f"frame_count ({frame_count}) and dilation ({dilation}) must be >= 1")
+    offset = (frame_count // 2) * dilation
+    offsets = [i - offset for i in range(0, (frame_count + 1) * dilation, dilation) if i != offset]
+    length = int(length)
+    if keyframe_indices is None:
+        n = length - frame_count * dilation
+        if max_length is not None:
+            if max_length < 0:
+                raise ValueError(f"max_length ({max_length}) must be None or >= 0")
+            n = min(n, int(max_length))
+        keys = list(range(offset, offset + max(n, 0)))
+    else:
+        border = length - (frame_count // 2 + 1) * dilation
+        keys = [int(k) for k in keyframe_indices if offset <= int(k) < border]
+    return FrameLayout(tuple(offsets), tuple(_inside(keys, offsets, length, False, "tum_mono_vo_layout")))
+
+
+def robotcar_layout(length, frame_count=2, dilation=1, drop_outside=False):
+    """The Oxford RobotCar loader's layout of one sequence of `length` frames (oxford_robotcar_dataset.py:55-61, :80-85).
+
+    The source frames are at k + i * dilation for i in range(-frame_count // 2, (frame_count + 1) // 2 + 1), i != 0, with
+    Python's floor division: an odd frame_count gives frame_count + 1 source frames (3: -2, -1, 1, 2).  The key frames are
+    offset ... length - frame_count + offset - 1 with offset = (frame_count // 2) * dilation; the loader trims frame_count
+    frames, not frame_count * dilation, so with dilation > 1 the last key frames need frames past the sequence, and an odd
+    frame_count makes the first one need frame -1.  Those raise ValueError unless `drop_outside` (see `_inside`)."""
+    if frame_count < 1 or dilation < 1:
+        raise ValueError(f"frame_count ({frame_count}) and dilation ({dilation}) must be >= 1")
+    offsets = [i * dilation for i in range(-frame_count // 2, (frame_count + 1) // 2 + 1) if i != 0]
+    offset = (frame_count // 2) * dilation
+    keys = range(offset, int(length) - frame_count + offset)
+    return FrameLayout(tuple(offsets), tuple(_inside(keys, offsets, int(length), drop_outside, "robotcar_layout")))
+
+
 def check_keys(keys, offsets, length=None):
     """`keys` as a list of ints, checked to be increasing sequence indices of key frames with all their neighbours (at
-    `offsets`) in the sequence: from -min(offsets) on, and before length - max(offsets) when `length` is given."""
+    `offsets`) in the sequence: from -min(offsets) on, and before length - max(offsets) when `length` is given (the key
+    frame itself counts as offset 0)."""
     keys = [int(k) for k in keys]
-    lo, hi = min(0, min(offsets)), max(offsets)
+    lo, hi = min(0, min(offsets)), max(0, max(offsets))
     end = None if length is None else int(length) - hi
     if any(b <= a for a, b in zip(keys, keys[1:])) or (keys and (keys[0] < -lo or (end is not None and keys[-1] >= end))):
         raise ValueError(f"key frames must be increasing sequence indices in [{-lo}, {'...' if end is None else end}): the "
@@ -121,6 +221,12 @@ class MonoRecSequence:
     graph replay when `graphed`, with no host synchronisation; the other outputs are those of residual_image=False bit for
     bit.
 
+    `layout` (a FrameLayout: `kitti_layout` with `offset_d` / `max_length`, `tum_mono_vo_layout`, `robotcar_layout`)
+    replaces frame_count, dilation and keys: each key frame's `frames` / `poses` / `intrinsics` are the frames at its
+    layout offsets, in their order, and the layout's key frames are run as a `keys` list is.  Offset 0 gathers the key
+    frame's own frame again.  A key frame is run once its largest offset (or itself, when all are negative) is pushed: a
+    causal layout runs each key frame at the push of that frame.
+
     `model` is a MonoRecModel (or any callable that adds its outputs to the reference's data dict and returns that dict,
     as MonoRecModel.forward does); `device` defaults to the device of its parameters.  A `use_stereo` model without
     `stereo=True`, and `pretrain_mode == 3` without `mvobj_masks=True`, raise NotImplementedError: a plain frame stream
@@ -128,7 +234,8 @@ class MonoRecSequence:
     """
 
     def __init__(self, model, frame_count=2, dilation=1, batch_size=8, graphed=True, device=None, first_frame=0,
-                 key_end=None, keys=None, stereo=False, mvobj_masks=False, use_color=True, residual_image=False):
+                 key_end=None, keys=None, stereo=False, mvobj_masks=False, use_color=True, residual_image=False,
+                 layout=None):
         if getattr(model, "use_stereo", False) and not stereo:
             raise NotImplementedError("MonoRecSequence: use_stereo needs stereo frames: MonoRecSequence(stereo=True) and "
                                       "push(..., stereo=(image, pose, intrinsics))")
@@ -142,8 +249,16 @@ class MonoRecSequence:
             raise ValueError(f"batch_size ({batch_size}) must be >= 1")
         if first_frame < 0:
             raise ValueError(f"first_frame ({first_frame}) must be >= 0")
+        if layout is not None and keys is not None:
+            raise ValueError("MonoRecSequence: give keys or layout, not both (a layout holds its key frames)")
         self.model = model
-        self.offsets = neighbour_offsets(frame_count, dilation)
+        self.layout = layout
+        if layout is None:
+            self.offsets = neighbour_offsets(frame_count, dilation)
+        else:
+            self.offsets, keys = [int(u) for u in layout.offsets], layout.keys
+            if not self.offsets:
+                raise ValueError("MonoRecSequence: the layout has no source frames")
         self.batch_size = int(batch_size)
         self.graphed = bool(graphed)
         self.stereo, self.mvobj_masks = bool(stereo), bool(mvobj_masks)
@@ -155,7 +270,8 @@ class MonoRecSequence:
         self._forward = functools.partial(_with_residual_image, model) if self.residual_image else model
         self.channels = 3 if self.use_color else 1
         self.device = torch.device(device) if device is not None else next(model.parameters()).device
-        lo, self._hi = min(0, min(self.offsets)), max(self.offsets)
+        # the frames a key frame i uses are i + lo ... i + hi (its own frame included)
+        lo, self._hi = min(0, min(self.offsets)), max(0, max(self.offsets))
         self.first_key = -lo               # the sequence's first key frame with all its neighbours in the sequence
         self.key_begin = int(first_frame) - lo
         self.key_end = None if key_end is None else int(key_end)
@@ -285,14 +401,17 @@ class MonoRecSequence:
 
     def _assemble(self, idx, out=None):
         """The batch dict, with the reference's keys and list order, gathered from the rings at slots `idx` [1+F, n];
-        written into `out`'s tensors when given (the graph's static inputs)."""
+        written into `out`'s tensors when given (the graph's static inputs).  A source frame at offset 0 is the key frame's
+        own tensor (its image, pose and intrinsics): gathered once, read twice (GraphedMonoRec keeps that aliasing)."""
         frames, poses, intrinsics = self._rings
         data = {}
         for key, ring in (("keyframe", frames), ("keyframe_pose", poses), ("keyframe_intrinsics", intrinsics)):
             data[key] = torch.index_select(ring, 0, idx[0], out=None if out is None else out[key])
-        for key, ring in (("frames", frames), ("poses", poses), ("intrinsics", intrinsics)):
-            data[key] = [torch.index_select(ring, 0, idx[1 + f], out=None if out is None else out[key][f])
-                         for f in range(len(self.offsets))]
+        for key, own, ring in (("frames", "keyframe", frames), ("poses", "keyframe_pose", poses),
+                               ("intrinsics", "keyframe_intrinsics", intrinsics)):
+            data[key] = [data[own] if u == 0 else
+                         torch.index_select(ring, 0, idx[1 + f], out=None if out is None else out[key][f])
+                         for f, u in enumerate(self.offsets)]
         for key, ring in self._maps.items():
             data[key] = torch.index_select(ring, 0, idx[0], out=None if out is None else out[key])
         return data
