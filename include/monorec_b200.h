@@ -456,6 +456,31 @@ int mr_reprojection_loss_bwd(const float* keyframe, const float* const* frames, 
 int mr_residual_image(const float* keyframe, const float* const* frames, const float* proj, const float* inv_depth,
                       const float* inv_depth_range, int B, int F, int C, int H, int W, float* out, void* stream);
 
+/* ---- Oxford RobotCar lidar depth targets ---------------------------------------------------------------------------------
+ * Replaces OxfordRobotCarDataset.get_depth (reference: data_loader/oxford_robotcar_dataset.py:121-144) with the RobotCar SDK's
+ * pinhole CameraModel.project.  World points live in a device ring `ring` [capacity,4] float64 (x, y, z, w); a window of
+ * `count` points starting at row `first` occupies rows first, first + 1, ... modulo capacity.
+ *   mr_lidar_to_world: ring rows (first + i) mod capacity = M @ [x_i, y_i, z_i, 1] for the n points of `scan` (device
+ *     [n,3] float64, 8-byte aligned); M: host double[16], row-major, lidar_pose @ lidar_transform (:129).  0 <= n <= capacity,
+ *     0 <= first < capacity, ring 16-byte aligned.  One launch (none for n = 0).
+ *   mr_lidar_depth: K key frames' inverse-depth targets.  Key frame k's points are the `count[k]` ring rows from `first[k]`
+ *     (host long long[K]); cam: host double[16 K], row-major camera_transform @ inv(pose_k @ swapaxes_) (:131); G: host
+ *     double[16] G_camera_image; proj: host double[8] = {fx, fy, cx, cy, lo, u_hi, v_hi, scale}.  Per point, in float64 op by
+ *     op in the naive left-to-right order: q = cam_k p, (x, y, z) = rows 0-2 of G q; kept iff z > 0 and lo <= u <= u_hi,
+ *     lo <= v <= v_hi for u = fx x / z + cx, v = fy y / z + cy; pixel (trunc(v scale), trunc(u scale)) of an Hd x Wd array;
+ *     value (float) (1 / z).  out [K,1,crop[1]-crop[0],crop[3]-crop[2]] float32 = the largest value landing on each pixel of
+ *     the window rows crop[0]:crop[1], columns crop[2]:crop[3] (host int[4]), 0 where none lands.  out_of_array [K] int32
+ *     counts the kept points whose pixel lies outside the Hd x Wd array (where the loader raises IndexError).  Both outputs
+ *     are zero-filled by the call.  Constraints: 1 <= K <= 65535, 1 <= Hd, Wd <= 65535, a non-empty crop window inside the
+ *     array, scale > 0, every matrix and proj entry finite, 0 <= count[k] <= capacity, 0 <= first[k] < capacity, ring
+ *     16-byte, out and out_of_array 4-byte aligned.  All arguments are checked before the first CUDA call; two memsets and one
+ *     launch per 16 key frames, no host synchronisation. */
+int mr_lidar_to_world(const double* scan, long long n, const double* M, double* ring, long long capacity, long long first,
+                      void* stream);
+int mr_lidar_depth(const double* ring, long long capacity, int K, const long long* first, const long long* count,
+                   const double* cam, const double* G, const double* proj, int Hd, int Wd, const int* crop, float* out,
+                   int* out_of_array, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,4 +15,7 @@ def __getattr__(name):
     if name in ("ResidualImage", "ResidualImageModule"):
         from . import layers as _l
         return getattr(_l, name)
+    if name in ("RobotCarLidar", "lidar_depth"):
+        from . import robotcar as _r
+        return getattr(_r, name)
     raise AttributeError(name)

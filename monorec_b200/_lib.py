@@ -88,6 +88,9 @@ SIGNATURES = {
                                          c_int, c_void_p, c_void_p]),
     "mr_residual_image": (c_int, [c_void_p, POINTER(c_void_p), c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                   c_void_p, c_void_p]),
+    "mr_lidar_to_world": (c_int, [c_void_p, c_longlong, c_void_p, c_void_p, c_longlong, c_longlong, c_void_p]),
+    "mr_lidar_depth": (c_int, [c_void_p, c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                               c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 
